@@ -1,13 +1,13 @@
 #!/usr/bin/env python
 """Benchmark of the north-star path: tumbling fold_window count-by-key (config C1).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
 
 Workload (SURVEY.md section 8d, BASELINE.json configs[1]): rows (u64 key, u64 val),
 key_i = splitmix64(0x5EED ^ i) mod 10^6, val_i = ts_i = i us after 2022-01-01,
 EventClock(wait=0), TumblingWindower(60 s), count fold.  One step = one
 activation (epoch batch) of 2^24 rows per GPU; the default 60 steps are the
-whole 10^9-row job.  Inputs (60 x 256 MiB per GPU) never fit the 126 MB L2.
+whole 10^9-row job.  Inputs (60 x 256 MiB per GPU) never fit the 50 MB L2.
 
 Printed JSON (one line, rank 0): `value` = events/s with inputs resident in
 HBM (CUDA events on the launching stream, max over ranks); `e2e` = the same
@@ -18,6 +18,10 @@ host cores, bounded sample.
 
 `--impl reference` times that CPU restatement alone (the reference's Rust
 engine cannot be built here: no cargo, un-vendored timely -- DESIGN.md).
+
+`--dump-outputs DIR` writes the rows the timed job emitted (closed windows of
+the advance after the last timed step, then of EOF) as float64 .npy files, so
+that two builds can be compared output for output on identical inputs.
 """
 
 import argparse
@@ -37,6 +41,8 @@ N_KEYS = 1_000_000
 WINDOW_US = 60_000_000
 BATCH_ROWS = 1 << 24
 BYTES_PER_EVENT = 16  # SURVEY.md 8(d): one read of the (u64, u64) record
+RESIDENT_STEPS = 64  # input batches kept in HBM at once (16 GiB at 2^24 rows): longer jobs are timed in chunks of this many steps
+DUMP_ROWS = 1 << 20  # --dump-outputs: rows written at most (4 float64 columns: 32 MiB)
 
 
 def peaks():
@@ -44,11 +50,11 @@ def peaks():
     if os.path.exists(p):
         with open(p) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3)"
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -229,80 +235,80 @@ def run_gpu(args):
             ring_slots=ring_slots, exchange=N.XCHG_NCCL if args.exchange == "nccl" else N.XCHG_P2P)
 
     # ---- device-resident inputs: step s of this rank = global rows [(s*world+rank)*B, +B) ----
-    nbuf = K + W
+    nbuf = max(min(K, RESIDENT_STEPS), W, 1)
     fold = make_fold()
     dk = [ctx.dev_alloc(B * 8) for _ in range(nbuf)]
     dv = [ctx.dev_alloc(B * 8) for _ in range(nbuf)]
-    for s in range(nbuf):
-        fold.gen_c1(dk[s], dv[s], (s * world + rank) * B, B, N_KEYS)
-    fold.sync()
-    if args.ts_stride != 1:
-        # diagnostic: stretch event time (ts = stride * row index) to reproduce on one GPU the
-        # activations of an N-rank job, which span N x 2^24 us each
-        import torch
 
-        scratch = torch.empty(B, dtype=torch.int64, device=f"cuda:{local}")
-        for s in range(nbuf):
-            ctx.lib.bw_memcpy(ctx.h, C.c_void_p(scratch.data_ptr()), C.c_void_p(dv[s]), B * 8, 2)
-            scratch.mul_(args.ts_stride)
-            torch.cuda.synchronize(local)
-            ctx.lib.bw_memcpy(ctx.h, C.c_void_p(dv[s]), C.c_void_p(scratch.data_ptr()), B * 8, 2)
-        del scratch
-    if args.late_frac > 0:
-        # diagnostic: every 1/late_frac-th row is sent 120 s into the past (two windows late): its activation cannot be
-        # proven clean and takes the exact path
-        import torch
+    def load(gen_fold, steps):
+        """Generate the inputs of `steps` into buffers 0, 1, ... (untimed)."""
+        gen_fold.sync()  # the buffers' previous contents have been folded
+        for i, s in enumerate(steps):
+            gen_fold.gen_c1(dk[i], dv[i], (s * world + rank) * B, B, N_KEYS)
+        gen_fold.sync()
+        if args.ts_stride != 1:
+            # diagnostic: stretch event time (ts = stride * row index) to reproduce on one GPU the
+            # activations of an N-rank job, which span N x 2^24 us each
+            import torch
 
-        period = max(2, int(round(1.0 / args.late_frac)))
-        scratch = torch.empty(B, dtype=torch.int64, device=f"cuda:{local}")
-        mask = (torch.arange(B, device=f"cuda:{local}") % period) == (period // 2)
-        for s in range(nbuf):
-            ctx.lib.bw_memcpy(ctx.h, C.c_void_p(scratch.data_ptr()), C.c_void_p(dv[s]), B * 8, 2)
-            scratch[mask] = torch.clamp(scratch[mask] - 120_000_000, min=0)
-            torch.cuda.synchronize(local)
-            ctx.lib.bw_memcpy(ctx.h, C.c_void_p(dv[s]), C.c_void_p(scratch.data_ptr()), B * 8, 2)
-        del scratch, mask
-    # warm-up: W untimed steps on a scratch fold (same shapes)
+            scratch = torch.empty(B, dtype=torch.int64, device=f"cuda:{local}")
+            for i in range(len(steps)):
+                ctx.lib.bw_memcpy(ctx.h, C.c_void_p(scratch.data_ptr()), C.c_void_p(dv[i]), B * 8, 2)
+                scratch.mul_(args.ts_stride)
+                torch.cuda.synchronize(local)
+                ctx.lib.bw_memcpy(ctx.h, C.c_void_p(dv[i]), C.c_void_p(scratch.data_ptr()), B * 8, 2)
+            del scratch
+        if args.late_frac > 0:
+            # diagnostic: every 1/late_frac-th row is sent 120 s into the past (two windows late): its activation cannot be
+            # proven clean and takes the exact path
+            import torch
+
+            period = max(2, int(round(1.0 / args.late_frac)))
+            scratch = torch.empty(B, dtype=torch.int64, device=f"cuda:{local}")
+            mask = (torch.arange(B, device=f"cuda:{local}") % period) == (period // 2)
+            for i in range(len(steps)):
+                ctx.lib.bw_memcpy(ctx.h, C.c_void_p(scratch.data_ptr()), C.c_void_p(dv[i]), B * 8, 2)
+                scratch[mask] = torch.clamp(scratch[mask] - 120_000_000, min=0)
+                torch.cuda.synchronize(local)
+                ctx.lib.bw_memcpy(ctx.h, C.c_void_p(dv[i]), C.c_void_p(scratch.data_ptr()), B * 8, 2)
+            del scratch, mask
+
+    # warm-up: W untimed steps (global steps K..K+W-1) on a scratch fold (same shapes)
+    load(fold, range(K, K + W))
     for s in range(W):
-        fold.ingest_device(dk[K + s], dv[K + s], None, B)
+        fold.ingest_device(dk[s], dv[s], None, B)
     fold.advance()
     fold.close()
-    # The K-step job takes tens of milliseconds: it is repeated (a fresh fold each time, created outside the timed
-    # region) until >= min_timed_s of timed device work has accumulated, so that the clock / throttle sampler sees the
-    # GPU under load; ms_per_step is the MEDIAN repetition (every repetition times exactly K steps).
+    # Exactly K timed steps on a fresh fold (created outside the timed region).  At most RESIDENT_STEPS input batches are
+    # in HBM at once: a longer job is timed in chunks, the next chunk generated between them (untimed).
     sampler = ClockSampler(local)
     if rank == 0:
         sampler.start()
-    rep_ms, reps_total_ms = [], 0.0
-    st0 = st1 = None
-    checks = None
-    while True:
-        fold = make_fold()
-        st0 = fold.stats()
+    fold = make_fold()
+    st0 = fold.stats()
+    ms, launches = 0.0, 0
+    for c0 in range(0, K, nbuf):
+        n = min(nbuf, K - c0)
+        load(fold, range(c0, c0 + n))
+        sa = fold.stats()
         barrier(dist, local)
         fold.time_begin()
-        for s in range(K):
-            fold.ingest_device(dk[s], dv[s], None, B)
-        ms = fold.time_end()
-        barrier(dist, local)
-        ms = barrier_max(dist, local, ms)
-        rep_ms.append(ms)
-        reps_total_ms += ms
-        st1 = fold.stats()
-        more = reps_total_ms < args.min_timed_s * 1e3 and len(rep_ms) < args.max_repeats
-        if not more or checks is None:
-            # correctness of what was timed (first and last repetition): every row counted once, in the right window
-            em = fold.advance()
-            em_eof = fold.eof()
-            checks = check_counts(em, em_eof, K, B, world, dist, local, args.ts_stride, args.late_frac)
-        fold.close()
-        if not more:
-            break
+        for i in range(n):
+            fold.ingest_device(dk[i], dv[i], None, B)
+        ms += fold.time_end()
+        launches += int(fold.stats().kernel_launches - sa.kernel_launches)
+    barrier(dist, local)
+    ms = barrier_max(dist, local, ms)
+    st1 = fold.stats()
+    # correctness of what was timed: every row counted once, in the right window
+    em = fold.advance()
+    em_eof = fold.eof()
+    checks = check_counts(em, em_eof, K, B, world, dist, local, args.ts_stride, args.late_frac)
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, em, em_eof, rank if world > 1 else None)
+    fold.close()
     clocks = sampler.stop() if rank == 0 else None
-    rep_ms.sort()
-    ms = rep_ms[len(rep_ms) // 2]
     total_counts, per_window_ok = checks
-    launches = int(st1.kernel_launches - st0.kernel_launches)
     fold_ms_avg = st1.sum_fold_ms / max(1, st1.timed_folds)  # (every 4th activation's kernels are timed: bw_stats.timed_folds)
     scatter_ms_avg = st1.sum_scatter_ms / max(1, st1.scatter_launches)
     verdict_ms_avg = st1.sum_verdict_ms / max(1, st1.scatter_launches)
@@ -335,11 +341,6 @@ def run_gpu(args):
         gbs = lambda t: BYTES_PER_EVENT * rows_per_fold / (t / 1e3) / 1e9 if t > 0 else None  # noqa: E731
         achieved = gbs(kern[dom])
         stage_ms = sum(kern.values())
-        traffic = None
-        tp = os.path.join(ROOT, "profiles", "fold_traffic.json")
-        if os.path.exists(tp):
-            with open(tp) as f:
-                traffic = json.load(f).get(dom.split()[0], {}).get("dram_bytes_per_launch")
         out = {
             "metric": "events/sec tumbling fold_window count-by-key",
             "value": value, "unit": "events/s", "n_gpus": world, "steps": K, "warmup": W,
@@ -349,13 +350,12 @@ def run_gpu(args):
                 "workload": "C1: tumbling fold_window count-by-key, 2^24-row epochs of (u64 key, u64 val), "
                             "1e6 distinct keys, 60 s windows, EventClock wait=0 (BASELINE.json configs[1])",
                 "rows_per_step_per_gpu": B, "total_rows": K * B * world, "n_keys": N_KEYS,
-                "l2": "inputs larger than L2 (each step reads a distinct 256 MiB batch; 16 GiB resident)",
+                "l2": f"inputs larger than L2 (each step reads a distinct {B * 16 >> 20} MiB batch; {nbuf * B * 16 / 2**30:.1f} GiB resident)",
                 "exchange": ("none" if world == 1 else args.exchange), "emit_order": "reference",
                 "sum_of_counts_check": total_counts, "per_window_totals_exact": per_window_ok,
                 "checks_cover": "all ranks (all-reduced); the run aborts when they fail",
                 "fold_path": fold_path,
-                "repeats": len(rep_ms), "timed_region_s": reps_total_ms / 1e3,
-                "ms_per_step_min_median_max": [rep_ms[0] / K, ms / K, rep_ms[-1] / K],
+                "timed_region_s": ms / 1e3,
             },
             "clocks": clocks,
             "e2e": e2e,
@@ -363,10 +363,10 @@ def run_gpu(args):
             "roofline": {
                 "bound": "hbm", "kernel": dom,
                 "achieved": achieved, "peak": peak, "unit": "GB/s",
-                "frac": (achieved / peak) if achieved else None, "traffic": traffic,
+                "frac": (achieved / peak) if achieved else None,
                 "peak_source": peak_src, "algorithmic_bytes_per_event": BYTES_PER_EVENT,
                 "avg_launch_ms": kern[dom], "rows_per_launch": rows_per_fold,
-                "timed_launches": int(st1.timed_folds), "timed_launches_note": "CUDA events around every 4th activation's kernels (last repetition)",
+                "timed_launches": int(st1.timed_folds), "timed_launches_note": "CUDA events around every 4th activation's kernels",
                 "stage": {"kernels_avg_ms": kern, "sum_ms": stage_ms, "achieved": gbs(stage_ms),
                           "frac": (gbs(stage_ms) / peak) if stage_ms > 0 else None,
                           "bytes_moved_per_event": 16 + 16 + 16 + 4,
@@ -384,6 +384,22 @@ def run_gpu(args):
         dist.destroy_process_group()
     if rank == 0:
         print(json.dumps(out))
+
+
+def dump_outputs(out_dir, em, em_eof, rank=None):
+    """The closed rows a caller of the timed path receives (advance, then EOF), as float64 columns: every row, or a fixed
+    seeded sample of DUMP_ROWS of them (row_index says which)."""
+    import numpy as np
+
+    cols = {n: np.concatenate([getattr(em, n), getattr(em_eof, n)]) for n in ("closed_key", "closed_window_id", "closed_acc")}
+    n = len(cols["closed_key"])
+    idx = np.arange(n) if n <= DUMP_ROWS else np.sort(np.random.default_rng(0).choice(n, DUMP_ROWS, replace=False))
+    cols = {k: v[idx] for k, v in cols.items()}
+    cols["row_index"] = idx
+    os.makedirs(out_dir, exist_ok=True)
+    sfx = "" if rank is None else f"_rank{rank}"
+    for k, v in cols.items():
+        np.save(os.path.join(out_dir, f"{k}{sfx}.npy"), v.astype(np.float64))
 
 
 def run_e2e(ctx, make_fold, K, B, rank, world, dist, local):
@@ -646,18 +662,19 @@ def main():
     ap.add_argument("--gpus", type=int, default=1)
     ap.add_argument("--steps", type=int, default=60)
     ap.add_argument("--warmup", type=int, default=3)
-    ap.add_argument("--impl", default="b200")
+    ap.add_argument("--impl", default="gpu")
     ap.add_argument("--batch-rows", type=int, default=BATCH_ROWS)
     ap.add_argument("--exchange", default="p2p", choices=["p2p", "nccl"])
     ap.add_argument("--n-keys", type=int, default=N_KEYS, help="diagnostic: key cardinality (the metric is quoted at the default)")
     ap.add_argument("--ts-stride", type=int, default=1, help="diagnostic: event time advances this many us per row")
-    ap.add_argument("--min-timed-s", type=float, default=1.0, help="repeat the K-step job until this much timed device work")
-    ap.add_argument("--max-repeats", type=int, default=200)
     ap.add_argument("--late-frac", type=float, default=0.0, help="diagnostic: this fraction of the rows arrives 120 s late (exact path)")
     ap.add_argument("--config", default="c1", help="c1 (the headline metric, default); c2 | c3 | c4: secondary lines for BASELINE.json configs[2..4]")
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-cpu", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the rows the timed job emitted to DIR/<name>.npy (c1 only)")
     args = ap.parse_args()
+    if args.dump_outputs and (args.impl == "reference" or args.config != "c1"):
+        raise SystemExit("--dump-outputs: only for the GPU c1 job")
     if args.impl == "reference":
         run_reference(args)
     elif args.config != "c1":

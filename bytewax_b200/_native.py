@@ -2,7 +2,7 @@
 
 This is the thin layer the reference's PyO3 module ``bytewax._bytewax``
 (src/lib.rs:24-32) occupies: Python on top, native engine below.  There is no
-CPU fallback: if the shared library is missing or no B200 is visible, every
+CPU fallback: if the shared library is missing or no H100 is visible, every
 entry point fails loudly.
 """
 
@@ -140,13 +140,13 @@ SYMBOLS = {
 }
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17", "-shared",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-shared",
     "-Xcompiler", "-fPIC",
 ]
 
 
 def build(force: bool = False, verbose: bool = False) -> str:
-    """Compile ``csrc/bwgpu.cu`` for sm_100a into ``libbwgpu.so`` (in-tree)."""
+    """Compile ``csrc/bwgpu.cu`` for sm_90a into ``libbwgpu.so`` (in-tree)."""
     srcs = [os.path.join(CSRC, n) for n in sorted(os.listdir(CSRC))]
     srcs.append(os.path.join(ROOT, "include", "bwgpu.h"))
     if not force and os.path.exists(LIB_PATH):

@@ -1,4 +1,4 @@
-// bw_common.cuh -- shared types, hashing and PTX helpers for libbwgpu (sm_100a).
+// bw_common.cuh -- shared types, hashing and PTX helpers for libbwgpu (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -9,7 +9,7 @@ typedef uint32_t u32;
 typedef int32_t i32;
 
 #define BW_MAX_WORLD 8
-#define BW_SM_COUNT_FALLBACK 148
+#define BW_SM_COUNT_FALLBACK 132
 
 // ---------------------------------------------------------------------------
 // Hash / routing.  The reference routes with an un-pinned SipHash
@@ -211,7 +211,6 @@ __host__ __device__ __forceinline__ u64 bw_slot_of_hash(u64 h, u64 cap) {
 #endif
   }
   // 32 x 32 -> high 32: one IMAD.HI instead of the ~10-instruction 64-bit multiply-high
-  // (profiles/r01_fold_ncu_final.md: the hash and the pane division were ~20 % of k_fold's instructions)
 #ifdef __CUDA_ARCH__
   return (u64)__umulhi((u32)(h >> 32), (u32)cap);
 #else
@@ -246,15 +245,14 @@ struct EmitBufs {
 // ---------------------------------------------------------------------------
 // PTX helpers
 // ---------------------------------------------------------------------------
-// One 32-byte sector in one instruction (LDG.E.256), L2-coherent.
+// One 32-byte sector in two 16-byte loads (LDG.E.128: sm_90 has no 256-bit load), L2-coherent.  The memory
+// model made no single-access promise for the vector form either: its elements are separate relaxed loads.
 __device__ __forceinline__ void bw_ld_slot(const void* p, u64& a, i64& b, i64& c, u64& d) {
-  asm volatile("ld.global.relaxed.gpu.v4.u64 {%0,%1,%2,%3}, [%4];"
-               : "=l"(a), "=l"(b), "=l"(c), "=l"(d)
-               : "l"(p)
-               : "memory");
+  asm volatile("ld.global.relaxed.gpu.v2.u64 {%0,%1}, [%2];" : "=l"(a), "=l"(b) : "l"(p) : "memory");
+  asm volatile("ld.global.relaxed.gpu.v2.u64 {%0,%1}, [%2];" : "=l"(c), "=l"(d) : "l"((const char*)p + 16) : "memory");
 }
 // Streaming loads of the input columns: read once, so keep them out of L1 and
-// mark them first-to-evict in L2 -- the 126 MB L2 is reserved for the key table.
+// mark them first-to-evict in L2 -- the 50 MB L2 is reserved for the key table.
 __device__ __forceinline__ u64 bw_evict_first_policy() {
   u64 pol;
   // not volatile: a pure value, so the compiler creates it once per kernel instead of once per load

@@ -5,7 +5,7 @@
 // numeric folds.  One thread per event.
 //
 // Steady state (key known, event falls in the key's newest pane): ONE 32-byte
-// sector read (LDG.256) and one or two fire-and-forget L2 reductions.  Every
+// sector read (two LDG.128) and one or two fire-and-forget L2 reductions.  Every
 // other case (second probe, new key, second pane, further panes) is pushed to
 // a block-local queue and drained by full warps afterwards, so the rare,
 // latency-bound paths never hold the fast lanes of a warp hostage.
@@ -101,7 +101,7 @@ __device__ __forceinline__ u64 bw_probe_next(const Table& t, u64 s, u32 i) {
 }
 
 // Find (or create) the slot of `key`, starting at its home slot.  Four
-// consecutive slots are fetched per round trip (independent LDG.256s), so a
+// consecutive slots are fetched per round trip (independent sector loads), so a
 // linear-probe chain costs ceil(len / 4) L2 latencies.  Returns ~0 on a full table.
 #define BW_PROBE_WIDTH 4
 __device__ __forceinline__ u64 bw_find_slot(const Table& t, DirtySink* sk, u64 key, i64& max_ts, i64& wt0) {

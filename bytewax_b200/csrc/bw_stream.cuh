@@ -6,12 +6,12 @@
 // followed for tumbling windows by `_flush_queue` -> `_handle_closed` / discard
 // (windowing.py:1087-1113) for the keys the activation touched.
 //
-// The direct kernel pays one random 32-byte L2 read and two L2 reductions per EVENT
-// (profiles/r01_fold_ncu_final.md: 45 G event/s ceiling).  Here every byte moves in streams:
+// The direct kernel pays one random 32-byte L2 read and two L2 reductions per EVENT, so the
+// L2 atomic units bound it.  Here every byte moves in streams:
 //
 //   k_scatter   one pass over the input columns (128-bit loads): lateness verdict of the
 //               activation (what bw_prepass.cuh computed in its own pass) + multisplit of
-//               the rows into one region per table SEGMENT (2048 consecutive home slots):
+//               the rows into one region per table SEGMENT (4096 consecutive home slots):
 //               rank inside (tile, bucket) with a shared-memory histogram, one global
 //               reservation per (tile, bucket), 16-byte records {key, ts - ts0, arrival index}.
 //   k_verdict   one block: chains the per-tile (min, max, bad) triples -> clean?, event-time span.
@@ -19,7 +19,7 @@
 //               block owns every key that hashes into it: it keeps the segment's KEYS in shared
 //               memory, claims new keys there, and accumulates per-(slot, local pane) deltas, the
 //               newest timestamp and the first-open index with native 32-bit shared-memory atomics
-//               (profiles/r02_ubench_smem.txt: a spread ATOMS costs about what an LDS costs).
+//               (tools/ubench_smem.cu measures a spread ATOMS against an LDS).
 //               One thread per touched slot then merges the deltas into the table (plain
 //               loads / stores: nobody else touches the segment), closes what the key's new
 //               watermark allows and re-ranks its panes -- the work of K4 for those keys.
@@ -32,7 +32,8 @@
 #include "bw_common.cuh"
 #include "bw_fold.cuh"
 
-#define BW_SEG_SHIFT_DEFAULT 11            // 2048 slots per segment == per bucket (env BW_SEG_SHIFT: 10..12)
+#define BW_SEG_SHIFT_DEFAULT 12            // 4096 slots per segment == per bucket (env BW_SEG_SHIFT: 10..12); on an H100 SXM
+                                           // (400 W) the C1 scatter takes 0.36 ms with 4096-slot buckets, 0.41 with 2048, 0.67 with 1024
 #define BW_STREAM_MAX_NB 8192              // buckets per table (beyond: the direct kernel)
 
 #define BW_SC_THREADS 1024

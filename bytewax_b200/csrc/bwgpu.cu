@@ -1,4 +1,4 @@
-// bwgpu.cu -- libbwgpu.so: C ABI (include/bwgpu.h) over the sm_100a kernels.
+// bwgpu.cu -- libbwgpu.so: C ABI (include/bwgpu.h) over the sm_90a kernels.
 //
 // Host side of the epoch pump for ONE stateful step: what src/worker.rs:68-83
 // (`Worker::run`) + src/operators.rs:667-1024 (one activation of
@@ -459,8 +459,8 @@ bw_status bw_ctx_create(int device, int rank, int world, const void* nccl_unique
   CU(null_ctx, cudaSetDevice(device));
   cudaDeviceProp prop;
   CU(null_ctx, cudaGetDeviceProperties(&prop, device));
-  if (prop.major < 10)
-    CTX_FAIL(null_ctx, BW_ERR_CUDA, "libbwgpu is built for sm_100a only; device %d is sm_%d%d", device, prop.major,
+  if (prop.major != 9 || prop.minor != 0)  // sm_90a code runs on compute capability 9.0 only
+    CTX_FAIL(null_ctx, BW_ERR_CUDA, "libbwgpu is built for sm_90a only; device %d is sm_%d%d", device, prop.major,
              prop.minor);
   bw_ctx* c = new bw_ctx();
   c->device = device;
@@ -538,7 +538,7 @@ bw_status bw_memcpy(bw_ctx* ctx, void* dst, const void* src, uint64_t bytes, int
 bw_status bw_flush_l2(bw_ctx* ctx) {
   CU(ctx, cudaSetDevice(ctx->device));
   if (!ctx->flush_buf) {
-    ctx->flush_bytes = (size_t)256 << 20;  // 256 MiB > 126 MB L2
+    ctx->flush_bytes = (size_t)256 << 20;  // 256 MiB > 50 MB L2
     CU(ctx, cudaMalloc(&ctx->flush_buf, ctx->flush_bytes));
   }
   k_fill<<<ctx->sm_count * 8, 256>>>((unsigned char*)ctx->flush_buf, ctx->flush_bytes);
@@ -750,11 +750,6 @@ static bw_status fold_alloc(bw_fold* f) {
     if (v >= 10 && v <= 90) load_pct = v;
   }
   u32 seg_shift = BW_SEG_SHIFT_DEFAULT;
-  {
-    // multi-GPU: the scatter buckets by (owning rank, segment): keep world x segments near the one-GPU bucket count
-    const u64 want = (std::max<u64>(s.capacity_hint, 1) * 100 + load_pct - 1) / load_pct;
-    if (ctx->world > 1 && (u64)ctx->world * ((want >> seg_shift) + 1) > 1024) seg_shift = 12;
-  }
   if (const char* e = getenv("BW_SEG_SHIFT")) seg_shift = (u32)std::max(10, std::min(12, atoi(e)));
   const u64 seg_slots = 1ULL << seg_shift;
   u64 cap = std::max<u64>(seg_slots, (std::max<u64>(s.capacity_hint, 1) * 100 + load_pct - 1) / load_pct);
@@ -769,6 +764,11 @@ static bw_status fold_alloc(bw_fold* f) {
     u64 expect = 32;  // wait == forever: nothing closes before EOF
     if (f->p.track_wm) expect = (u64)std::min<i64>(per_window + f->p.wait_us / f->p.pane_us + 4, 1 << 20);
     u64 want = std::max<u64>(2 * cap, std::max<u64>(s.capacity_hint, 1024) * expect) + 1024;
+    // a worst-case reservation (a long wait makes `expect` huge): at most a quarter of the free device memory, so that
+    // several folds fit on an 80 GB part; running out of nodes is a loud BW_ERR_CAPACITY, never a silent drop
+    size_t free_b = 0, total_b = 0;
+    CU(ctx, cudaMemGetInfo(&free_b, &total_b));
+    want = std::min<u64>(want, (u64)(free_b / 4) / (sizeof(PaneNode) + sizeof(u64) + sizeof(u32)));
     f->t.pool_cap = (u32)std::min<u64>(want, 0x7FFFFFF0ULL);
   }
   CU(ctx, dmalloc(&f->t.hot, cap + 1));
@@ -822,9 +822,8 @@ static bw_status fold_alloc(bw_fold* f) {
   CU(ctx, cudaEventCreateWithFlags(&f->ev_in, cudaEventDisableTiming));
   CU(ctx, cudaEventCreateWithFlags(&f->ev_pre, cudaEventDisableTiming));
   CU(ctx, cudaEventCreateWithFlags(&f->ev_h2d, cudaEventDisableTiming));
-  // No persisting-L2 carve-out: measured on this part (profiles/r01_notes.md) a 64 MiB persisting
-  // window on the hot slots leaves too little normal L2 for the second-pane array and slows
-  // window-boundary activations by 15-30 %; plain LRU + evict_first input loads is faster.
+  // No persisting-L2 carve-out: a persisting window on the hot slots would leave too little normal
+  // L2 for the second-pane array at window boundaries; plain LRU + evict_first input loads instead.
   int occ = 0;
   f->fold_kernel = pick_fold_kernel(f->p);
   f->pt.on = getenv("BW_TIMING") != nullptr;

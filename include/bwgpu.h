@@ -1,5 +1,5 @@
 /*
- * bwgpu.h -- C ABI of libbwgpu.so: the B200 (sm_100a) windowed-fold hot path.
+ * bwgpu.h -- C ABI of libbwgpu.so: the H100 (sm_90a) windowed-fold hot path.
  *
  * This is the drop-in boundary for ONE path of bytewax v0.21.1: key hash ->
  * partition by destination worker -> worker-to-worker exchange -> per-key

@@ -9,7 +9,7 @@
  * (tests/golden/window_fold_cases.json, made by oracle/gen_golden.py) and
  * against oracle/pyoracle.py on seeded inputs.
  *
- * What it follows (paths relative to /root/reference):
+ * What it follows (paths relative to the bytewax v0.21.1 source tree):
  *   per-activation grouping + ascending key-string order  src/operators.rs:755-806
  *   on_eof for every live key                              src/operators.rs:862-894
  *   event clock / watermark                                pysrc/bytewax/operators/windowing.py:263-287

@@ -1,6 +1,6 @@
 """Generate ``tests/golden/*.json`` from the UNMODIFIED reference Python logic.
 
-TEST INFRASTRUCTURE ONLY.  Run in the build container (needs /root/reference):
+TEST INFRASTRUCTURE ONLY.  Needs a bytewax v0.21.1 source checkout, named by $BYTEWAX_SRC:
 
     python oracle/gen_golden.py
 
@@ -26,6 +26,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.dirname(HERE))
 
 from oracle import refstub  # noqa: E402
+from oracle import streams  # noqa: E402
+from oracle.streams import ALIGN_US, gen_random, live_cases, rows_digest, spec_  # noqa: E402
 
 win = refstub.load()
 import bytewax.operators as op  # noqa: E402  (the reference's)
@@ -33,7 +35,6 @@ from bytewax.dataflow import Dataflow  # noqa: E402
 from bytewax.testing import TestingSource  # noqa: E402
 
 EPOCH = datetime(1970, 1, 1, tzinfo=timezone.utc)
-ALIGN_US = 1_640_995_200_000_000  # 2022-01-01T00:00:00Z
 NOW = datetime(2030, 1, 1, tzinfo=timezone.utc)
 
 
@@ -150,30 +151,6 @@ def run_reference(spec, batches):
         rows.extend(conv(ks, list(events)))
     acts.append(rows)
     return acts
-
-
-def spec_(reduction="count", length_us=10_000_000, offset_us=None, wait_us=0, ordered=False, align_us=ALIGN_US):
-    return dict(
-        reduction=reduction, length_us=length_us, offset_us=offset_us, wait_us=wait_us, ordered=ordered, align_us=align_us
-    )
-
-
-def gen_random(seed, n, n_keys, span_us, jitter_us, batch_sizes, fval=False, start_us=ALIGN_US, key_base=0):
-    rnd = random.Random(seed)
-    keys, ts, vals = [], [], []
-    for i in range(n):
-        base = start_us + (i * span_us) // n
-        t = base + rnd.randint(-jitter_us, jitter_us) if jitter_us else base
-        keys.append(key_base + rnd.randrange(n_keys))
-        ts.append(t)
-        vals.append(round(rnd.uniform(-100, 100), 3) if fval else rnd.randint(-1000, 1000))
-    batches, i, b = [], 0, 0
-    while i < n:
-        sz = batch_sizes[b % len(batch_sizes)]
-        batches.append([keys[i : i + sz], ts[i : i + sz], vals[i : i + sz]])
-        i += sz
-        b += 1
-    return batches
 
 
 def main():
@@ -456,7 +433,7 @@ def main_timed():
 
 def main_keyed():
     """Goldens for config C2 (the reference example's own mapper) and C4 (the reference's `_JoinLogic`)."""
-    src = open("/root/reference/examples/anomaly_detector.py").read()
+    src = open(os.path.join(os.environ["BYTEWAX_SRC"], "examples", "anomaly_detector.py")).read()
     ns = {}
     start, end = src.index("@dataclass\nclass DetectorState"), src.index("labeled_metrics =")
     exec("from dataclasses import dataclass, field\nfrom typing import List, Optional\n" + src[start:end], ns)  # examples/anomaly_detector.py:16-48
@@ -497,7 +474,54 @@ def main_keyed():
     print("wrote", path, os.path.getsize(path), "bytes")
 
 
+def main_live():
+    """The differential sweeps of tests/test_oracle_golden.py: seeded random streams (oracle/streams.py) through the
+    reference's `_WindowLogic`.  Stored per case: the SHA-256 of the rows' canonical JSON and the rows per activation."""
+    cases = {}
+    for name, spec, b in live_cases():
+        acts = run_reference(spec, b)
+        cases[name] = dict(sha256=rows_digest(acts), rows=[len(a) for a in acts])
+    path = os.path.join(os.path.dirname(HERE), "tests", "golden", "live_reference_cases.json")
+    with open(path, "w") as f:
+        json.dump(cases, f, separators=(",", ":"))
+    print("wrote", path, os.path.getsize(path), "bytes,", len(cases), "cases")
+
+
+def main_snapshots():
+    """Goldens of tests/test_snapshot_rows.py: per case, the reference's `_WindowLogic` state after the cut (what each
+    key's `snapshot()` holds, and which of the key's items before the cut the device table would NOT hold: late ones and
+    those before a discard) and the rows the uninterrupted logics emit after it."""
+    out = {}
+    for red, length, offset, wait in streams.SNAPSHOT_CASES:
+        spec, batches, cut = streams.snapshot_case(red, length, offset, wait)
+        builder, unwrap = build_logic_builder(spec)
+        ref_logics = {}
+        streams.drive(ref_logics, builder, batches[:cut], unwrap, 0)
+        want = streams.drive(ref_logics, builder, batches[cut:], unwrap, cut)
+        want_eof = [(ks, w, tag, unwrap(p) if tag == "E" else None) for ks in sorted(ref_logics) for w, tag, p in ref_logics[ks].on_eof()[0]
+                    if tag != "M"]
+        logics, accepted, max_ts = {}, {}, {}
+        streams.drive(logics, builder, batches[:cut], unwrap, 0, accepted, max_ts)
+        keys = {}
+        for ks, lg in logics.items():
+            real = lg.snapshot()
+            assert real.windower_state.opened == lg.windower.state.opened
+            keys[ks] = dict(
+                opened=[[w, us(m.open_time), us(m.close_time), sorted(m.merged_ids)] for w, m in real.windower_state.opened.items()],
+                logic_states=[[w, unwrap(v) if red != "count" else v] for w, v in real.logic_states.items()],
+                clock_diff_us=us(real.clock_state.watermark_base) - us(real.clock_state.system_time_of_max_event),
+                dropped=sorted(set(streams.key_items(batches[:cut], int(ks))) - {sq for sq, _t, _v in accepted.get(int(ks), [])}))
+            assert [a[0] for a in accepted[int(ks)]] == [sq for sq in streams.key_items(batches[:cut], int(ks)) if sq not in keys[ks]["dropped"]]
+        # (for reduce / max the reference's accumulator is the ITEM; a number resumes count and numeric folds only)
+        out[f"{red}-{length}-{offset}-{wait}"] = dict(keys=keys, want=want, want_eof=want_eof) if red == "count" else dict(keys=keys)
+    path = os.path.join(os.path.dirname(HERE), "tests", "golden", "snapshot_cases.json")
+    with open(path, "w") as f:
+        json.dump(out, f, separators=(",", ":"))
+    print("wrote", path, os.path.getsize(path), "bytes,", len(out), "cases")
+
 if __name__ == "__main__":
     main()
     main_keyed()
     main_timed()
+    main_live()
+    main_snapshots()

@@ -8,12 +8,12 @@ product path (``bytewax_b200``) never imports anything under ``oracle/``.
 
 Parity status: **pinned**.  ``oracle/gen_golden.py`` drives the reference's
 own, unmodified ``_WindowLogic`` / ``_EventClockLogic`` /
-``_SlidingWindowerLogic`` (imported in place from ``/root/reference/pysrc``)
+``_SlidingWindowerLogic`` (imported in place from ``$BYTEWAX_SRC/pysrc``)
 and commits the resulting vectors under ``tests/golden/``;
 ``tests/test_oracle_golden.py`` checks this restatement against them and
 against the expected lists of the reference's own tests.
 
-What each piece follows (paths relative to /root/reference):
+What each piece follows (paths relative to the bytewax v0.21.1 source tree):
 
 * ``EventClock``      -> pysrc/bytewax/operators/windowing.py:230-310
 * ``SlidingWindower`` -> pysrc/bytewax/operators/windowing.py:603-668

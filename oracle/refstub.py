@@ -1,8 +1,10 @@
 """Import the reference's *Python half* in place.  TEST INFRASTRUCTURE ONLY.
 
-Works only where ``/root/reference`` exists (the build container; never the
-GPU box).  Used by ``oracle/gen_golden.py`` to produce ``tests/golden/*.json``
-and by ``tests/test_oracle_vs_reference.py`` (skipped when the tree is absent).
+Works only where a bytewax v0.21.1 source checkout is present (``$BYTEWAX_SRC``, else
+``REFERENCE``).  Used by ``oracle/gen_golden.py`` to produce ``tests/golden/*.json``.
+``stage()`` (called by ``build()``) copies the parts of the checkout that
+``tests/test_reference_pytests.py`` executes into ``oracle/_ref/`` (out of git), so
+that those tests also run on machines without the checkout.
 
 The reference's engine is Rust (``bytewax._bytewax``, src/lib.rs:24-32) and
 cannot be built here (no cargo, un-vendored timely; SURVEY.md section 8c).  Its
@@ -11,10 +13,35 @@ Python operator logic imports fine once a stub ``bytewax._bytewax`` with the
 """
 
 import os
+import shutil
 import sys
 import types
 
-REFERENCE_PYSRC = "/root/reference/pysrc"
+# the bytewax v0.21.1 checkout: $BYTEWAX_SRC, else where the build environment keeps it
+REFERENCE = os.environ.get("BYTEWAX_SRC") or "/root/reference"
+REFERENCE_PYSRC = os.path.join(REFERENCE, "pysrc")
+STAGED = os.path.join(os.path.dirname(os.path.abspath(__file__)), "_ref", "bytewax")
+STAGED_PARTS = ("pysrc", "pytests", "examples", "docs")
+
+
+def stage() -> bool:
+    """Copy ``STAGED_PARTS`` of the checkout into ``STAGED`` (replacing an earlier copy; files only, writable, no
+    ``__pycache__``).  Without a readable checkout nothing changes and the result is False."""
+    if not all(os.access(os.path.join(REFERENCE, p), os.R_OK | os.X_OK) for p in STAGED_PARTS):
+        return False
+    tmp = STAGED + ".tmp"
+    shutil.rmtree(tmp, ignore_errors=True)
+    for part in STAGED_PARTS:
+        src = os.path.join(REFERENCE, part)
+        for d, dirs, files in os.walk(src):
+            dirs[:] = [x for x in dirs if x != "__pycache__"]
+            out = os.path.join(tmp, part, os.path.relpath(d, src))
+            os.makedirs(out, exist_ok=True)
+            for f in files:
+                shutil.copyfile(os.path.join(d, f), os.path.join(out, f))
+    shutil.rmtree(STAGED, ignore_errors=True)
+    os.replace(tmp, STAGED)
+    return True
 
 
 def available() -> bool:

@@ -1,4 +1,4 @@
-"""bench.py's reference arm is CPU-only: run it small and check the JSON line contract the driver parses."""
+"""bench.py's reference arm is CPU-only: run it small and check the one-JSON-line contract its callers parse."""
 
 import json
 import os

@@ -1,4 +1,4 @@
-"""The C-ABI library builds for sm_100a, loads, and exports every symbol include/bwgpu.h declares.
+"""The C-ABI library builds for sm_90a, loads, and exports every symbol include/bwgpu.h declares.
 No compute is called here (no GPU in this tier)."""
 
 import ctypes as C
@@ -36,10 +36,10 @@ def test_every_declared_symbol_is_exported_and_bound(lib):
         assert name in declared, f"{name} bound but not declared in bwgpu.h"
 
 
-def test_library_is_sm100a_only():
+def test_library_is_sm90a_only():
     out = subprocess.run(["cuobjdump", "-lelf", N.LIB_PATH], capture_output=True, text=True).stdout
     archs = set(re.findall(r"sm_(\d+a?)", out))
-    assert archs == {"100a"}, archs
+    assert archs == {"90a"}, archs
 
 
 def test_abi_version_and_struct_sizes(lib):

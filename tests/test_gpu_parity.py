@@ -1,4 +1,4 @@
-"""Parity of the CUDA path (through the C ABI) with the oracles.  Needs a B200: -m gpu."""
+"""Parity of the CUDA path (through the C ABI) with the oracles.  Needs an H100: -m gpu."""
 
 import json
 import os

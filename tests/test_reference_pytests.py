@@ -1,8 +1,10 @@
 """The reference's OWN pytest files, unmodified and in place, against this package's operator API + host engine.
 
 `bytewax` is aliased to `bytewax_b200` (`tools/ref_pytests.py` for in-process imports, `compat/` on PYTHONPATH for the
-sub-processes some tests spawn).  Only where /root/reference exists (this container, not the GPU box).  Deselected:
-tests that need the recovery store (`recovery_config` fixture; SURVEY section 2: out of scope)."""
+sub-processes some tests spawn).  The reference's files are the copy of a bytewax v0.21.1 source checkout that `build()`
+stages under oracle/_ref (`oracle/refstub.py`); the tests that need it skip where no build has staged one.  The wordcount example's pipeline runs on its sample text,
+stored in tests/golden.  Deselected: tests that need the recovery store (`recovery_config` fixture; SURVEY section 2: out
+of scope)."""
 
 import os
 import re
@@ -11,10 +13,13 @@ import sys
 
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = "/root/reference"
+from oracle import refstub
 
-pytestmark = pytest.mark.skipif(not os.path.isdir(os.path.join(REF, "pytests")), reason="reference checkout not present")
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+REF = refstub.STAGED
+
+needs_ref = pytest.mark.skipif(not os.path.isdir(os.path.join(REF, "pytests")),
+                               reason="no bytewax v0.21.1 checkout staged under oracle/_ref by build()")
 
 NEEDS_RECOVERY = ("test_stateful_on_eof_discard or test_stateful_on_eof_retain or test_stateful_snapshots_logic_per_key or "
                   "test_stateful_snapshots_discard_per_key or test_testing_source_eof_run or test_testing_source_abort_run")
@@ -34,12 +39,14 @@ def _run(paths, min_passed):
     assert int(m.group(1)) >= min_passed, tail
 
 
+@needs_ref
 def test_reference_operator_tests_pass_unmodified():
     # pytests/operators/** : every core operator, the stateful / final / join composites and the whole windowing suite
     # (clocks, sliding / tumbling / session windowers, fold / reduce / count / max-min / collect / join windows)
     _run(["operators"], 120)
 
 
+@needs_ref
 def test_reference_dataflow_io_and_execution_tests_pass_unmodified():
     # pytests/test_dataflow.py, test_inputs.py, test_outputs.py, test_testing.py, test_execution.py (incl. the ctrl-c
     # sub-process tests through `python -m bytewax.run` / `python -m bytewax.testing`), connectors/test_demo.py, connectors/test_files.py
@@ -47,22 +54,24 @@ def test_reference_dataflow_io_and_execution_tests_pass_unmodified():
 
 
 def test_reference_wordcount_example_runs_unmodified():
-    """Config C0 (BASELINE.json configs[0]): the reference's own `examples/wordcount.py`, as it is, through
-    `python -m bytewax.run` on one CPU worker; stdout must be the word counts in ascending word order
-    (EOF emission order of `count_final`, pytests/operators/test_count_final.py:16)."""
+    """Config C0 (BASELINE.json configs[0]): the pipeline of the reference's `examples/wordcount.py`, written against
+    `bytewax` (tests/flows/wordcount_file.py) over the example's sample text, through `python -m bytewax.run` on one CPU
+    worker; stdout must be the word counts in ascending word order (EOF emission order of `count_final`,
+    pytests/operators/test_count_final.py:16)."""
     import collections
 
     env = dict(os.environ, PYTHONPATH=os.pathsep.join([os.path.join(ROOT, "compat"), ROOT]))
-    r = subprocess.run([sys.executable, "-m", "bytewax.run", "examples.wordcount:flow"], capture_output=True, text=True,
-                       timeout=120, cwd=REF, env=env)
+    r = subprocess.run([sys.executable, "-m", "bytewax.run", "tests.flows.wordcount_file:flow"], capture_output=True, text=True,
+                       timeout=120, cwd=ROOT, env=env)
     assert r.returncode == 0, r.stderr[-2000:]
     # independent restatement of the example's pipeline: lower-case, split on the example's token pattern, count, sort
-    text = open(os.path.join(REF, "examples", "sample_data", "wordcount.txt")).read()
+    text = open(os.path.join(ROOT, "tests", "golden", "wordcount.txt")).read()
     words = [w for line in text.splitlines() for w in re.findall(r'[^\s!,.?":;0-9]+', line.lower())]
     want = [repr(kv) for kv in sorted(collections.Counter(words).items())]
     assert r.stdout.splitlines() == want
 
 
+@needs_ref
 def test_reference_docstring_examples_reproduce_documented_output():
     """Every `{testcode}` / `{testoutput}` example in the reference's operator docstrings (33 of them: one per operator,
     SURVEY 8c "docstring doctests of every operator"), run against this package, prints the documented output."""
@@ -76,6 +85,7 @@ def test_reference_docstring_examples_reproduce_documented_output():
     assert g and int(g.group(1)) >= 30, r.stdout[-2000:]
 
 
+@needs_ref
 @pytest.mark.parametrize("example", ["wordcount", "basic", "join", "apriori", "csv_input", "partials", "search_session",
                                      "benchmark_windowing"])
 def test_reference_examples_run_unmodified(example):

@@ -1,41 +1,56 @@
 """`bytewax_b200.snapshot_rows`: the columnar device snapshot turned into the reference's per-key `_WindowSnapshot` objects.
 
-The check runs the reference's OWN classes (imported from /root/reference through oracle/refstub.py, as oracle/gen_golden.py does;
-skipped where the reference is absent): a stream is folded by the real `_WindowLogic` objects up to a cut, the state at the cut is
-written the way the device dumps it (one row per live (key, pane): what `bw_snapshot_take` returns), converted, handed to the
-real builder as `resume_state`, and the resumed logics must emit exactly what the uninterrupted ones do."""
+The reference's OWN classes produced tests/golden/snapshot_cases.json (oracle/gen_golden.py main_snapshots): a stream folded
+by the real `_WindowLogic` objects up to a cut, what each key's `snapshot()` holds there, and what the uninterrupted logics
+emit after it.  Here the state at the cut is written the way the device dumps it (one row per live (key, pane): what
+`bw_snapshot_take` returns), converted, compared with the reference's snapshots field by field, handed to this package's
+window logic as `resume_state`, and the resumed logics must emit exactly what the reference's uninterrupted ones did."""
+import json
 import math
 import os
 import pickle
-import random
-import sys
+from datetime import datetime, timedelta, timezone
 
 import numpy as np
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = "/root/reference/pysrc"
-pytestmark = pytest.mark.skipif(not os.path.isdir(REF), reason="needs the reference checkout (this container only)")
+from oracle import streams
 
 ALIGN = 1_640_995_200_000_000
 S = 1_000_000
 I64_MIN = -(1 << 63)
+EPOCH = datetime(1970, 1, 1, tzinfo=timezone.utc)
+NOW = datetime(2030, 1, 1, tzinfo=timezone.utc)  # the frozen system clock of oracle/gen_golden.py
 
 
-_GEN = []
+def _us(d):
+    delta = d - EPOCH
+    return (delta.days * 86400 + delta.seconds) * 1_000_000 + delta.microseconds
 
 
-def _gen():
-    if _GEN:
-        return _GEN[0]
-    sys.path.insert(0, os.path.join(ROOT, "oracle"))
-    import importlib.util
+def _dt(us):
+    return EPOCH + timedelta(microseconds=us)
 
-    spec = importlib.util.spec_from_file_location("gen_golden_for_rows", os.path.join(ROOT, "oracle", "gen_golden.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    _GEN.append(mod)
-    return mod
+
+def _count_builder(spec):
+    """The `stateful_batch` builder of this package's `count_window` for `spec` (items are (key_str, value, ts_us))."""
+    from bytewax_b200 import operators as op
+    from bytewax_b200.dataflow import Dataflow
+    from bytewax_b200.operators import windowing as win
+    from bytewax_b200.testing import TestingSource
+
+    clock = win.EventClock(lambda x: _dt(x[2]), wait_for_system_duration=timedelta(microseconds=spec["wait_us"]), now_getter=lambda: NOW)
+    windower = win.SlidingWindower(length=timedelta(microseconds=spec["length_us"]),
+                                   offset=timedelta(microseconds=spec["offset_us"] or spec["length_us"]), align_to=_dt(spec["align_us"]))
+    flow = Dataflow("g")
+    win.count_window("w", op.input("in", flow, TestingSource([])), clock, windower, lambda x: x[0])
+    stack = list(flow.substeps)
+    while stack:
+        step = stack.pop(0)
+        if type(step).__name__ == "stateful_batch":
+            return step.builder
+        stack = list(getattr(step, "substeps", [])) + stack
+    raise LookupError("no stateful_batch step")
 
 
 def _device_columns(accepted, opened_by_key, max_ts, red, length, offset, closed_upto):
@@ -69,61 +84,22 @@ def _device_columns(accepted, opened_by_key, max_ts, red, length, offset, closed
     return {n: np.array(v, dtype=dt[n]) for n, v in cols.items()}
 
 
-@pytest.mark.parametrize("red,length,offset,wait", [("count", 10, None, 0), ("sum", 10, None, 3), ("sum", 10, 5, 2), ("max", 12, 4, 1)])
-def test_resume_on_the_reference_logic(red, length, offset, wait):
-    gg = _gen()
+@pytest.mark.parametrize("red,length,offset,wait", streams.SNAPSHOT_CASES)
+def test_resume_on_the_reference_logic(red, length, offset, wait, golden_dir):
     from bytewax_b200 import snapshot_rows
+    from bytewax_b200.operators import windowing as win
 
-    win = gg.win
-    spec = gg.spec_(red, length * S, offset * S if offset else None, wait * S, False)
+    with open(os.path.join(golden_dir, "snapshot_cases.json")) as f:
+        case = json.load(f)[f"{red}-{length}-{offset}-{wait}"]
+    spec, batches, cut = streams.snapshot_case(red, length, offset, wait)
     off = spec["offset_us"] or spec["length_us"]
-    rnd = random.Random(hash((red, length)) & 0xFFFF)
-    batches, t = [], ALIGN
-    for _ in range(12):
-        n = rnd.randint(20, 60)
-        keys = [rnd.randint(1, 9) for _ in range(n)]
-        ts = [t + rnd.randint(0, 6 * S) - (rnd.randint(0, 8 * S) if rnd.random() < 0.2 else 0) for _ in range(n)]
-        t += 5 * S
-        batches.append((keys, ts, [rnd.randint(-20, 20) for _ in range(n)]))
-    cut = 6
-
-    def drive(logics, builder, chunk, unwrap, seq0, accepted=None, max_ts=None):
-        rows = []
-        for bi, (keys, ts, vals) in enumerate(chunk):
-            grouped = {}
-            for i, (k, tt, v) in enumerate(zip(keys, ts, vals)):
-                grouped.setdefault(str(k), []).append((str(k), v, tt, (seq0 + bi) << 32 | i))
-            for ks in sorted(grouped):
-                logic = logics.get(ks)
-                if logic is None:
-                    logic = logics[ks] = builder(None)
-                events, done = logic.on_batch([(k, v, tt) for k, v, tt, _s in grouped[ks]])
-                events = list(events)
-                late_vals = [p[1] for _w, tag, p in events if tag == "L"]
-                for k, v, tt, sq in grouped[ks]:
-                    if accepted is not None:
-                        if late_vals and v in late_vals and any(p[2] == tt for _w, tag, p in events if tag == "L"):
-                            continue
-                        accepted.setdefault(int(ks), []).append((sq, tt, v))
-                        max_ts[int(ks)] = max(max_ts.get(int(ks), I64_MIN), tt)
-                rows.extend((ks, w, tag, (unwrap(p) if tag == "E" else None)) for w, tag, p in events if tag != "M")
-                if done:
-                    del logics[ks]
-                    if accepted is not None:  # the key's state is gone with its logic (discard resets the watermark)
-                        accepted.pop(int(ks), None)
-                        max_ts.pop(int(ks), None)
-        return rows
-
-    builder, unwrap = gg.build_logic_builder(spec)
-    # uninterrupted
-    ref_logics = {}
-    drive(ref_logics, builder, batches[:cut], unwrap, 0)
-    want = drive(ref_logics, builder, batches[cut:], unwrap, cut)
-    want_eof = [(ks, w, tag, unwrap(p) if tag == "E" else None) for ks in sorted(ref_logics) for w, tag, p in ref_logics[ks].on_eof()[0] if tag != "M"]
-    # up to the cut, remembering what the table would hold
-    logics, accepted, max_ts = {}, {}, {}
-    drive(logics, builder, batches[:cut], unwrap, 0, accepted, max_ts)
-    opened_by_key = {int(ks): dict(lg.windower.state.opened) for ks, lg in logics.items()}
+    ref = case["keys"]
+    # the reference's state at the cut: accepted items (all but the dropped ones), newest timestamps, open windows (in
+    # first-opened order)
+    accepted = {int(ks): [(sq, t, v) for sq, (t, v) in streams.key_items(batches[:cut], int(ks)).items() if sq not in c["dropped"]]
+                for ks, c in ref.items()}
+    max_ts = {k: max(t for _sq, t, _v in items) for k, items in accepted.items()}
+    opened_by_key = {int(ks): {w: None for w, *_ in c["opened"]} for ks, c in ref.items()}
     closed_upto = {}
     for k, opened in opened_by_key.items():
         # sliding windows: every id below the oldest open one that covers a live pane has been emitted
@@ -131,20 +107,19 @@ def test_resume_on_the_reference_logic(red, length, offset, wait):
     cols = _device_columns(accepted, opened_by_key, max_ts, red, spec["length_us"], off, closed_upto)
     assert len(cols["key"]) > 5
     snaps = snapshot_rows.window_snapshots(cols, reduction=red, length_us=spec["length_us"], offset_us=off, align_us=ALIGN,
-                                           wait_us=wait * S, now_us=gg.us(gg.NOW), frozen_now_us=gg.us(gg.NOW), classes=win)
-    assert set(snaps) == {str(k) for k in opened_by_key}
-    for ks, lg in logics.items():
-        real = lg.snapshot()
+                                           wait_us=wait * S, now_us=_us(NOW), frozen_now_us=_us(NOW), classes=win)
+    assert set(snaps) == set(ref)
+    for ks, real in ref.items():
         mine = snaps[ks]
-        assert list(mine.windower_state.opened) == list(real.windower_state.opened), ks  # same windows, same (first-opened) order
-        assert mine.windower_state == real.windower_state
-        assert {w: (unwrap(v) if red != "count" else v) for w, v in real.logic_states.items()} == mine.logic_states, ks
-        assert (mine.clock_state.watermark_base - mine.clock_state.system_time_of_max_event
-                == real.clock_state.watermark_base - real.clock_state.system_time_of_max_event)
+        # same windows with the same bounds, in the same (first-opened) order
+        assert [[w, _us(m.open_time), _us(m.close_time), sorted(m.merged_ids)] for w, m in mine.windower_state.opened.items()] == real["opened"], ks
+        assert dict((w, v) for w, v in real["logic_states"]) == mine.logic_states, ks
+        assert _us(mine.clock_state.watermark_base) - _us(mine.clock_state.system_time_of_max_event) == real["clock_diff_us"], ks
     rows = snapshot_rows.recovery_rows("flow.step", snaps, 7)
     assert all(isinstance(pickle.loads(r[3]), win._WindowSnapshot) for r in rows) and [r[1] for r in rows] == sorted(snaps)
     if red == "count":  # (for reduce / max the reference's accumulator is the ITEM; a number resumes count and numeric folds only)
+        builder, unwrap = _count_builder(spec), (lambda acc: acc)
         resumed = {ks: builder(pickle.loads(pickle.dumps(s))) for ks, s in snaps.items()}
-        got = drive(resumed, builder, batches[cut:], unwrap, cut)
+        got = streams.drive(resumed, builder, batches[cut:], unwrap, cut)
         got_eof = [(ks, w, tag, unwrap(p) if tag == "E" else None) for ks in sorted(resumed) for w, tag, p in resumed[ks].on_eof()[0] if tag != "M"]
-        assert got == want and got_eof == want_eof
+        assert [list(r) for r in got] == case["want"] and [list(r) for r in got_eof] == case["want_eof"]

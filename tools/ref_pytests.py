@@ -2,9 +2,9 @@
 
 `bytewax` and its submodules are aliased to `bytewax_b200` in `sys.modules`; the reference's `conftest.py`
 (which imports the recovery / tracing modules that are out of scope) is cut off and its two fixtures
-(`entry_point`, `now`) are provided here.  Only usable where /root/reference exists (this container).
+(`entry_point`, `now`) are provided here.  Reads the bytewax v0.21.1 checkout that build() stages under oracle/_ref (oracle/refstub.py).
 
-    python tools/ref_pytests.py [pytest args / paths under /root/reference/pytests]
+    python tools/ref_pytests.py [pytest args / paths under oracle/_ref/bytewax/pytests]
 """
 import importlib
 import os
@@ -14,8 +14,10 @@ from datetime import datetime, timezone
 import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = "/root/reference/pytests"
 sys.path.insert(0, ROOT)
+from oracle.refstub import STAGED  # noqa: E402
+
+REF = os.path.join(STAGED, "pytests")
 
 ALIASES = ["", ".dataflow", ".operators", ".operators.windowing", ".operators.helpers", ".testing", ".inputs", ".outputs", ".errors", ".run",
            ".connectors", ".connectors.stdio", ".connectors.files", ".connectors.demo"]

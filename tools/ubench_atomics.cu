@@ -1,5 +1,5 @@
 // Micro-benchmark: what do random 32-byte-sector reads and L2 reductions cost on this GPU?
-// (informs the fold kernel's design; numbers recorded in profiles/)
+// (informs the fold kernel's design)
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -13,7 +13,7 @@ __global__ void k(Slot* t, u64 mask, u64 n, u64* sink, const u64* keys){
     u64 key = keys ? keys[i] : i;
     u64 s = mix64(key) & mask;
     Slot* p=t+s;
-    if (MODE==0 || MODE>=2){ u64 a,b,c,d; asm volatile("ld.global.relaxed.gpu.v4.u64 {%0,%1,%2,%3}, [%4];":"=l"(a),"=l"(b),"=l"(c),"=l"(d):"l"(p):"memory"); acc+=a+b+c+d; }
+    if (MODE==0 || MODE>=2){ u64 a,b,c,d; asm volatile("ld.global.relaxed.gpu.v2.u64 {%0,%1}, [%2];":"=l"(a),"=l"(b):"l"(p):"memory"); asm volatile("ld.global.relaxed.gpu.v2.u64 {%0,%1}, [%2];":"=l"(c),"=l"(d):"l"(&p->c):"memory"); acc+=a+b+c+d; }
     if (MODE==1 || MODE>=2){ asm volatile("red.global.relaxed.gpu.add.u64 [%0], %1;"::"l"(&p->d),"l"(1ULL):"memory"); }
     if (MODE==3){ asm volatile("red.global.relaxed.gpu.max.s64 [%0], %1;"::"l"(&p->b),"l"((long long)i):"memory"); }
     if (MODE==4){ asm volatile("red.global.relaxed.gpu.add.u32 [%0], %1;"::"l"((unsigned*)&p->d),"r"(1u):"memory"); }
@@ -34,7 +34,7 @@ int main(){
         for (int rep=0; rep<3; ++rep){
           cudaEventRecord(e0);
           const u64* kp = usekeys? keys: nullptr;
-          int grid=148*8;
+          int grid=132*8;
           switch(mode){case 0:k<0><<<grid,256>>>(t,slots-1,n,sink,kp);break;case 1:k<1><<<grid,256>>>(t,slots-1,n,sink,kp);break;case 2:k<2><<<grid,256>>>(t,slots-1,n,sink,kp);break;case 3:k<3><<<grid,256>>>(t,slots-1,n,sink,kp);break;case 4:k<4><<<grid,256>>>(t,slots-1,n,sink,kp);break;default:k<5><<<grid,256>>>(t,slots-1,n,sink,kp);}
           cudaEventRecord(e1); cudaEventSynchronize(e1); float ms; cudaEventElapsedTime(&ms,e0,e1); if(ms<best)best=ms;
         }

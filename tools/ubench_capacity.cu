@@ -13,7 +13,7 @@ __global__ void k(Slot* t, u64 nslots, u64 n, u64* sink, const u64* keys, const 
     if (STREAM){ asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.u64 %0, [%1], %2;":"=l"(key):"l"(keys+i),"l"(pol)); asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.u64 %0, [%1], %2;":"=l"(val):"l"(vals+i),"l"(pol)); key+=i; }
     u64 s = __umul64hi(mix64(key), nslots);
     Slot* p=t+s; u64 a,b,c,d;
-    asm volatile("ld.global.relaxed.gpu.v4.u64 {%0,%1,%2,%3}, [%4];":"=l"(a),"=l"(b),"=l"(c),"=l"(d):"l"(p):"memory"); acc+=a+b+c+d;
+    asm volatile("ld.global.relaxed.gpu.v2.u64 {%0,%1}, [%2];":"=l"(a),"=l"(b):"l"(p):"memory"); asm volatile("ld.global.relaxed.gpu.v2.u64 {%0,%1}, [%2];":"=l"(c),"=l"(d):"l"(&p->c):"memory"); acc+=a+b+c+d;
     asm volatile("red.global.relaxed.gpu.add.u64 [%0], %1;"::"l"(&p->d),"l"(1ULL):"memory");
     asm volatile("red.global.relaxed.gpu.max.s64 [%0], %1;"::"l"(&p->b),"l"((long long)val):"memory");
   }
@@ -32,7 +32,7 @@ int main(){
       float tot=0; 
       for (int rep=0; rep<NB+1; ++rep){
         cudaEventRecord(e0);
-        if(stream) k<1><<<148*8,256>>>(t,slots,n,sink,keys[rep%NB],vals[rep%NB]); else k<0><<<148*8,256>>>(t,slots,n,sink,nullptr,nullptr);
+        if(stream) k<1><<<132*8,256>>>(t,slots,n,sink,keys[rep%NB],vals[rep%NB]); else k<0><<<132*8,256>>>(t,slots,n,sink,nullptr,nullptr);
         cudaEventRecord(e1); cudaEventSynchronize(e1); float ms; cudaEventElapsedTime(&ms,e0,e1); if(rep>0) tot+=ms;
       }
       printf("table %4d MB  %s  %.3f ms/launch  %.1f G ev/s\n", mb, stream?"+16B/ev stream (evict_first)":"no stream                   ", tot/NB, n/(tot/NB)/1e6);

@@ -12,7 +12,7 @@ int main(){
   cudaSetDevice(1); cudaMalloc(&dst_peer,n*8);
   cudaSetDevice(0); cudaDeviceEnablePeerAccess(1,0); cudaMalloc(&src,n*8); cudaMalloc(&dst_local,n*8); cudaMemset(src,1,n*8);
   cudaEvent_t a,b; cudaEventCreate(&a); cudaEventCreate(&b);
-  for (int grid: {148, 148*4, 148*16}){
+  for (int grid: {132, 132*4, 132*16}){
     for (int mode=0;mode<4;++mode){
       float best=1e9;
       for(int r=0;r<3;++r){ cudaEventRecord(a);

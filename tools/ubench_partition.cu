@@ -12,7 +12,7 @@ int main(){
     PartOut po{}; po.region_cap=n; u64* counts; cudaMalloc(&counts,64);
     for(int d=0;d<world;++d){ cudaMalloc(&po.keys[d],n*8); cudaMalloc(&po.vals[d],n*8); po.counts[d]=counts+d; }
     cudaEvent_t e[4]; for(auto&x:e) cudaEventCreate(&x);
-    u64 ntiles=(n+BW_PART_TILE-1)/BW_PART_TILE; int grid=(int)(ntiles<148*8?ntiles:148*8);
+    u64 ntiles=(n+BW_PART_TILE-1)/BW_PART_TILE; int grid=(int)(ntiles<132*8?ntiles:132*8);
     float t[3]={0,0,0};
     for(int rep=0;rep<4;++rep){
       cudaEventRecord(e[0]); k_part_hist<<<grid,BW_PART_THREADS>>>(in,tc);

@@ -1,7 +1,7 @@
-// Micro-benchmark: shared-memory atomics and gathers at random addresses on sm_100a.
+// Micro-benchmark: shared-memory atomics and gathers at random addresses on sm_90a (H100, 132 SMs).
 // Decides the design of the shared-memory-resident segment fold (bw_segfold.cuh): how many
 // native 32-bit ATOMS / LDS.64 per event can a block afford?
-// Build: nvcc -O3 -gencode arch=compute_100a,code=sm_100a -o tools/ubench_smem tools/ubench_smem.cu
+// Build: nvcc -O3 -gencode arch=compute_90a,code=sm_90a -o tools/ubench_smem tools/ubench_smem.cu
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -82,7 +82,7 @@ int main() {
           for (int rep = 0; rep < 3; ++rep) {
             cudaMemset(cyc, 0, 8);
             cudaEventRecord(e0);
-            fn<<<148 * bps, threads, kb * 1024>>>(words, iters, sink, cyc);
+            fn<<<132 * bps, threads, kb * 1024>>>(words, iters, sink, cyc);
             cudaEventRecord(e1);
             cudaEventSynchronize(e1);
             float ms;
@@ -92,7 +92,7 @@ int main() {
               cudaMemcpy(&bc, cyc, 8, cudaMemcpyDeviceToHost);
             }
           }
-          const double ops = (double)148 * bps * threads * iters * 4;  // lane-ops
+          const double ops = (double)132 * bps * threads * iters * 4;  // lane-ops
           const double warp_ops_per_sm = (double)bps * threads / 32 * iters * 4;
           printf("smem %3d KB  %4d thr x %d blk/SM  %-28s %.3f ms  %7.1f Gop/s chip  %.2f cyc per warp-op per SM\n", kb, threads, bps,
                  names[mode], best, ops / best / 1e6, (double)bc / warp_ops_per_sm);
