@@ -33,7 +33,8 @@
 #include "bw_fold.cuh"
 
 #define BW_SEG_SHIFT_DEFAULT 12            // 4096 slots per segment == per bucket (env BW_SEG_SHIFT: 10..12); on an H100 SXM
-                                           // (400 W) the C1 scatter takes 0.36 ms with 4096-slot buckets, 0.41 with 2048, 0.67 with 1024
+                                           // (700 W) the C1 scatter takes 0.309 ms with 4096-slot buckets, 0.401 with 2048, 0.657
+                                           // with 1024 (16 staging records per bucket where they fit, else 8)
 #define BW_STREAM_MAX_NB 8192              // buckets per table (beyond: the direct kernel)
 
 #define BW_SC_THREADS 1024
@@ -213,8 +214,9 @@ __host__ __device__ __forceinline__ size_t bw_scatter_smem(int tsm, int vb_in, u
 // nothing to pad (the fold reads each lane's row count).  A lane that fills up (skewed keys) overflows into
 // the spill list.  The last warp to finish with a stage refills it.
 //
-// Writing every 16-byte record straight to its lane costs the LSU one wavefront per ROW (32 lanes, 32 lines:
-// measured 0.21 ms of a 0.34 ms kernel).  So the records of a bucket are first assembled in shared memory,
+// Writing every 16-byte record straight to its lane costs the LSU one wavefront per ROW (32 lanes, 32 lines) and
+// cuts every 128-byte line of the output into pieces (C1 on an H100 SXM, 700 W: 0.63 ms against 0.309 ms with 16
+// staging records per bucket).  So the records of a bucket are first assembled in shared memory,
 // stg_cap per bucket, and every stg_every tiles the block writes what it has assembled: eight lanes per bucket,
 // one 128-byte line per wavefront.  A bucket that outruns its staging rows writes those straight out.
 template <int TSM, int VB_IN, int VB_OUT>
