@@ -65,7 +65,7 @@ class BwStats(C.Structure):
         ("pane_nodes_used", C.c_uint64), ("last_fold_ms", C.c_float), ("sum_fold_ms", C.c_float),
         ("fold_launches", C.c_uint64), ("fold_rows", C.c_uint64), ("combined_folds", C.c_uint64),
         ("sum_scatter_ms", C.c_float), ("sum_verdict_ms", C.c_float), ("scatter_launches", C.c_uint64),
-        ("split_batches", C.c_uint64), ("timed_folds", C.c_uint64),
+        ("split_batches", C.c_uint64), ("timed_folds", C.c_uint64), ("scatter_spill_rows", C.c_uint64),
     ]
 
 

@@ -1495,6 +1495,7 @@ static bw_status stream_resolve_multi(bw_fold* f, const Deferred& d) {
   cudaStream_t s = f->s_compute;
   const int W = ctx->world, R = ctx->rank;
   const StreamVerdict sv = f->h_sv[d.side];
+  f->st.scatter_spill_rows += sv.n_spill;
   // this activation's verdicts: gathered by the previous activation's exchange barrier, else (first activation, or
   // after a flush) by a collective of their own
   if (f->vg_pending[d.side]) {
@@ -1704,6 +1705,7 @@ static bw_status stream_resolve(bw_fold* f) {
     bw_status lst = late_split(f, d, bv, &sv, &split);
     if (lst != BW_OK) return lst;
   }
+  f->st.scatter_spill_rows += sv.n_spill;
   i64 q_lo = 0, q_hi = 0;
   if (sv.tmax >= sv.tmin) {
     q_lo = bw_floordiv(sv.tmin - p.align_us, p.pane_us);

@@ -185,6 +185,7 @@ typedef struct bw_stats {
   uint64_t split_batches;   /* not-clean activations whose late rows were found without the sort (streaming fold for the rest) */
   uint64_t timed_folds;     /* fold launches behind sum_fold_ms / fold_rows: every BW_TIMER_STRIDE-th activation (default 4) is
                              * timed -- an event record with timing drains the stream for a few microseconds */
+  uint64_t scatter_spill_rows; /* rows the bucket scatter put in the spill list (a lane was full), summed over activations */
 } bw_stats;
 
 /* ---- context ---------------------------------------------------------- */
