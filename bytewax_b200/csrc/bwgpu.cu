@@ -20,8 +20,10 @@
 #include <condition_variable>
 #include <cstdio>
 #include <cstring>
+#include <memory>
 #include <mutex>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "../../include/bwgpu.h"
@@ -103,6 +105,77 @@ struct bw_ctx {
                __LINE__);                                                                           \
   } while (0)
 
+// Every CUDA resource of one native object (bw_fold, bw_smap, bw_join): device and pinned host memory, events and
+// streams are made through it, and it releases them in reverse order when it goes.  A failed call leaves its field
+// null.  regrow() frees a buffer before it allocates the new one, so peak memory does not rise, and a failure leaves
+// the field null, never pointing at freed memory.
+class Owner {
+ public:
+  enum Kind { DEV, HOST, EVENT, STREAM };
+  Owner() = default;
+  Owner(const Owner&) = delete;
+  Owner& operator=(const Owner&) = delete;
+  ~Owner() {
+    for (size_t i = res_.size(); i-- > 0;) free_one(res_[i]);
+  }
+  // n elements of T (bytes when T is void), at least one
+  template <typename T>
+  cudaError_t dev(T** p, size_t n) { return mem(DEV, p, n); }
+  template <typename T>
+  cudaError_t host(T** p, size_t n) { return mem(HOST, p, n); }
+  template <typename T>
+  cudaError_t regrow(Kind k, T** p, size_t n) {
+    release(*p);
+    *p = nullptr;
+    return mem(k, p, n);
+  }
+  cudaError_t event(cudaEvent_t* e, unsigned flags = cudaEventDisableTiming) {
+    return keep(cudaEventCreateWithFlags(e, flags), EVENT, e);
+  }
+  cudaError_t stream(cudaStream_t* s, int priority = 0) {
+    return keep(cudaStreamCreateWithPriority(s, cudaStreamNonBlocking, priority), STREAM, s);
+  }
+  // release one resource made here before the object goes (null: nothing)
+  void release(const void* h) {
+    if (!h) return;
+    for (size_t i = res_.size(); i-- > 0;)
+      if (res_[i].h == h) {
+        free_one(res_[i]);
+        res_.erase(res_.begin() + i);
+        return;
+      }
+  }
+
+ private:
+  struct Res {
+    Kind kind;
+    void* h;
+  };
+  std::vector<Res> res_;
+  template <typename T>
+  cudaError_t mem(Kind k, T** p, size_t n) {
+    const size_t bytes = (n ? n : 1) * sizeof(std::conditional_t<std::is_void<T>::value, char, T>);
+    void* q = nullptr;
+    cudaError_t e = k == DEV ? cudaMalloc(&q, bytes) : cudaHostAlloc(&q, bytes, cudaHostAllocDefault);
+    *p = (T*)q;
+    return keep(e, k, p);
+  }
+  template <typename H>
+  cudaError_t keep(cudaError_t e, Kind k, H* h) {
+    if (e == cudaSuccess) res_.push_back({k, (void*)*h});
+    else *h = nullptr;
+    return e;
+  }
+  static void free_one(const Res& r) {
+    switch (r.kind) {
+      case DEV: cudaFree(r.h); break;
+      case HOST: cudaFreeHost(r.h); break;
+      case EVENT: cudaEventDestroy((cudaEvent_t)r.h); break;
+      case STREAM: cudaStreamDestroy((cudaStream_t)r.h); break;
+    }
+  }
+};
+
 // ---- collectives: NCCL, or the loopback world's rendezvous ----
 // all-gather of `bytes` per rank, device buffers, in stream order on `s`
 static bw_status coll_allgather(bw_ctx* ctx, const void* send, void* recv, size_t bytes, cudaStream_t s) {
@@ -146,15 +219,14 @@ static bw_status coll_share_base(bw_ctx* ctx, void* base, void** peers, cudaStre
   CU(ctx, cudaIpcGetMemHandle(&mine, base));
   static_assert(sizeof(cudaIpcMemHandle_t) == 64, "ipc handle size");
   unsigned char *d_in = nullptr, *d_all = nullptr;
-  CU(ctx, cudaMalloc(&d_in, 64));
-  CU(ctx, cudaMalloc(&d_all, 64 * W));
+  Owner tmp;  // the two staging buffers, freed on every way out
+  CU(ctx, tmp.dev(&d_in, 64));
+  CU(ctx, tmp.dev(&d_all, 64 * W));
   CU(ctx, cudaMemcpy(d_in, &mine, 64, cudaMemcpyHostToDevice));
   NC(ctx, ncclAllGather(d_in, d_all, 64, ncclChar, ctx->comm, s));
   CU(ctx, cudaStreamSynchronize(s));
   std::vector<cudaIpcMemHandle_t> all(W);
   CU(ctx, cudaMemcpy(all.data(), d_all, 64 * W, cudaMemcpyDeviceToHost));
-  cudaFree(d_in);
-  cudaFree(d_all);
   for (int r = 0; r < W; ++r) {
     if (r == ctx->rank) peers[r] = base;
     else CU(ctx, cudaIpcOpenMemHandle(&peers[r], all[r], cudaIpcMemLazyEnablePeerAccess));
@@ -182,10 +254,10 @@ struct PhaseTimer {
   const char* names[NPH] = {"part_hist+scan+scatter", "barrier", "prepass", "fold", "close", "scatter + verdict", "segfold", "spill + close"};
   std::vector<cudaEvent_t> ev[NPH][2];
   bool on = false;
+  Owner* own = nullptr;  // the fold's
   void mark(int ph, int which, cudaStream_t s) {
-    if (!on) return;
     cudaEvent_t e;
-    cudaEventCreate(&e);
+    if (!on || own->event(&e, cudaEventDefault) != cudaSuccess) return;
     cudaEventRecord(e, s);
     ev[ph][which].push_back(e);
   }
@@ -221,6 +293,54 @@ struct EventPair {
 typedef void (*scatter_kernel_t)(ScatterArgs, FoldParams);
 typedef void (*segfold_kernel_t)(SegArgs, Table, FoldParams, EmitBufs);
 
+// Scratch of the reference-order permutation (order_perm): sort keys, the permutation, one gathered column and CUB's
+// temporary storage.
+struct SortScratch {
+  u64 cap = 0;
+  u64 *sk = nullptr, *sk2 = nullptr, *gather = nullptr;
+  u32 *perm = nullptr, *perm2 = nullptr;
+  void* cub = nullptr;
+  size_t cub_bytes = 0;
+  // room for n rows: when they do not fit, reallocate for grow_to (>= n) rows once nothing on `s` reads the old buffers
+  cudaError_t reserve(Owner& own, u64 n, u64 grow_to, cudaStream_t s) {
+    if (n <= cap) return cudaSuccess;
+    cudaError_t e = cudaStreamSynchronize(s);
+    cap = 0;
+    for (u64** p : {&sk, &sk2, &gather})
+      if (!e) e = own.regrow(Owner::DEV, p, grow_to);
+    for (u32** p : {&perm, &perm2})
+      if (!e) e = own.regrow(Owner::DEV, p, grow_to);
+    if (e) return e;
+    size_t b = 0;
+    cub::DeviceRadixSort::SortPairs(nullptr, b, sk, sk2, perm, perm2, (int)grow_to, 0, 64, s);
+    if ((e = grow_cub(own, b + 256))) return e;
+    cap = grow_to;
+    return cudaSuccess;
+  }
+  // CUB's temporary storage: at least `bytes`, never shrunk
+  cudaError_t grow_cub(Owner& own, size_t bytes) {
+    if (bytes <= cub_bytes) return cudaSuccess;
+    cub_bytes = 0;
+    cudaError_t e = own.regrow(Owner::DEV, &cub, bytes);
+    if (!e) cub_bytes = bytes;
+    return e;
+  }
+};
+
+// Five pinned host columns of 8-byte values, grown together: the rows an advance hands to the caller.
+struct HostCols {
+  u64 cap = 0;
+  u64* col[5] = {};
+  cudaError_t reserve(Owner& own, u64 n, u64 grow_to) {
+    if (n <= cap) return cudaSuccess;
+    cap = 0;
+    for (u64*& c : col)
+      if (cudaError_t e = own.regrow(Owner::HOST, &c, grow_to)) return e;
+    cap = grow_to;
+    return cudaSuccess;
+  }
+};
+
 struct Stage;
 // An activation whose scatter + verdict are queued but whose fold stage is not: the host looks at a
 // verdict only after the NEXT activation's scatter is queued, so the device never waits for the host.
@@ -237,6 +357,7 @@ struct Deferred {
 };
 
 struct bw_fold {
+  Owner own;  // every buffer, event and stream below
   bw_ctx* ctx = nullptr;
   bw_fold_spec spec{};
   FoldParams p{};
@@ -268,21 +389,11 @@ struct bw_fold {
   i64 *d_tsflat = nullptr, *d_tssorted = nullptr, *d_prefmax = nullptr;
   u32 *d_idx = nullptr, *d_idxsorted = nullptr;
   unsigned char* d_late = nullptr;
-  void* d_cub = nullptr;
-  size_t cub_bytes = 0;
-  // emit sort temp (lazy)
-  u64 sort_cap = 0;
-  u64 *d_sk = nullptr, *d_sk2 = nullptr, *d_gather = nullptr;
-  u32 *d_perm = nullptr, *d_perm2 = nullptr;
+  // emission ordering scratch, sized at create; the slow path shares its CUB storage
+  SortScratch srt;
   // Rows of CLOSED epochs are ordered and copied to the host while later activations run (side stream s_out, its own
   // sort scratch): bw_advance then only has the newest rows left to do.  One rank, see flush_rows().
-  struct OutScratch {
-    u64 cap = 0;
-    u64 *sk = nullptr, *sk2 = nullptr, *gather = nullptr;
-    u32 *perm = nullptr, *perm2 = nullptr;
-    void* cub = nullptr;
-    size_t cub_bytes = 0;
-  } fl;
+  SortScratch fl;
   struct RowMark {
     u64 epoch = 0, next_epoch = 0;  // next_epoch: 1 + epoch of the activation folded after this one (0: none yet)
     cudaEvent_t ev = nullptr;       // the counts below are on the host once this has happened
@@ -296,12 +407,9 @@ struct bw_fold {
   bool flush_on = true;                   // env BW_FLUSH=0: order and copy everything in bw_advance
   bool host_ingest = false;               // the caller commits HOST batches (PCIe-bound: the device has time to spare between
                                           // activations; a device-resident caller keeps every SM busy and is left alone)
-  // host output (pinned, grown on demand)
-  u64 hout_cap_c = 0, hout_cap_l = 0;
-  u64 *ho_ckey = nullptr, *ho_cacc = nullptr, *ho_ccount = nullptr, *ho_cepoch = nullptr;
-  i64* ho_cwid = nullptr;
-  u64 *ho_lkey = nullptr, *ho_lval = nullptr, *ho_lepoch = nullptr;
-  i64 *ho_lwid = nullptr, *ho_lts = nullptr;
+  // host output (pinned, grown on demand): closed {key, window id, acc, count, epoch}, late {key, window id, value,
+  // timestamp, epoch}
+  HostCols ho_c, ho_l;
   // bookkeeping
   u32 batch_no = 0;
   u64 last_epoch = 0, min_epoch = 0;  // epochs are non-decreasing; rows carry the user epoch
@@ -370,8 +478,6 @@ struct bw_fold {
 };
 
 #define FAIL(f, code, ...) CTX_FAIL((f)->ctx, code, __VA_ARGS__)
-static bw_status ensure_sort_cap(bw_fold* f, u64 n);
-static bw_status grow_host(bw_fold* f, u64 nc, u64 nl);
 static bw_status mark_rows(bw_fold* f, u64 epoch);
 static bw_status flush_rows(bw_fold* f);
 
@@ -559,11 +665,6 @@ static i64 gcd_i64(i64 a, i64 b) {
   return a;
 }
 
-template <typename T>
-static cudaError_t dmalloc(T** p, size_t n) {
-  return cudaMalloc((void**)p, (n ? n : 1) * sizeof(T));
-}
-
 // k_fold instantiations: accumulator op x watermark tracking (+ MEAN keeps counts)
 typedef void (*fold_kernel_t)(BatchView, Table, FoldParams, u32, u32, u32);
 template <int OP, int CNT>
@@ -617,6 +718,7 @@ static scatter_kernel_t pick_scatter_kernel(int tsm, int vb_in, int vb_out) {
 
 static bw_status stream_alloc(bw_fold* f) {
   bw_ctx* ctx = f->ctx;
+  Owner& own = f->own;
   StreamBufs& sb = f->sb;
   const u64 rows = f->spec.max_batch_rows;
   const int W = ctx->world;
@@ -645,26 +747,26 @@ static bw_status stream_alloc(bw_fold* f) {
   sb.val_bytes = (f->p.op == BW_OP_ADD_ONE && !f->p.need_count) ? 0 : f->val_bytes;
   const size_t region_rows = (size_t)sb.nb * sb.nlanes * sb.lane_cap;
   for (int i = 0; i < 2; ++i) {
-    CU(ctx, dmalloc(&sb.side[i].rec, region_rows));
-    if (sb.val_bytes) CU(ctx, cudaMalloc(&sb.side[i].val, region_rows * (size_t)sb.val_bytes));
-    CU(ctx, dmalloc(&sb.side[i].cnt, (size_t)sb.nb * sb.nlanes));
+    CU(ctx, own.dev(&sb.side[i].rec, region_rows));
+    if (sb.val_bytes) CU(ctx, own.dev(&sb.side[i].val, region_rows * (size_t)sb.val_bytes));
+    CU(ctx, own.dev(&sb.side[i].cnt, (size_t)sb.nb * sb.nlanes));
     CU(ctx, cudaMemsetAsync(sb.side[i].cnt, 0, sizeof(u32) * sb.nb * sb.nlanes, f->s_compute));
-    CU(ctx, dmalloc(&sb.side[i].spill, sb.spill_cap));
-    CU(ctx, dmalloc(&sb.side[i].sv, 1));
+    CU(ctx, own.dev(&sb.side[i].spill, sb.spill_cap));
+    CU(ctx, own.dev(&sb.side[i].sv, 1));
     CU(ctx, cudaMemsetAsync(sb.side[i].sv, 0, sizeof(StreamVerdict), f->s_compute));
-    CU(ctx, cudaEventCreateWithFlags(&f->ev_sv[i], cudaEventDisableTiming));
+    CU(ctx, own.event(&f->ev_sv[i]));
   }
-  CU(ctx, cudaHostAlloc((void**)&f->h_sv, 2 * sizeof(StreamVerdict), cudaHostAllocDefault));
+  CU(ctx, own.host(&f->h_sv, 2));
   const int tsm = f->p.ts_from_value ? f->p.ts_from_value : 0;
   const int vb_in = (tsm == 1) ? 8 : (sb.val_bytes ? f->val_bytes : 0);
   f->scatter_kernel = pick_scatter_kernel(tsm, vb_in, sb.val_bytes);
   sb.tiles_cap = (u32)((rows + BW_SC_TILE - 1) / BW_SC_TILE + 1);  // one lateness triple per scatter tile
   // (one set per side: the tile triples of activation b are read again when it turns out to have late rows, after the
   // scatter of b + 1 has run)
-  CU(ctx, dmalloc(&sb.tile_min, 2 * (size_t)sb.tiles_cap));
-  CU(ctx, dmalloc(&sb.tile_max, 2 * (size_t)sb.tiles_cap));
-  CU(ctx, dmalloc(&sb.tile_bad, 2 * (size_t)sb.tiles_cap));
-  CU(ctx, dmalloc(&sb.chunk_max, 2 * (size_t)sb.tiles_cap * BW_SC_WARPS));
+  CU(ctx, own.dev(&sb.tile_min, 2 * (size_t)sb.tiles_cap));
+  CU(ctx, own.dev(&sb.tile_max, 2 * (size_t)sb.tiles_cap));
+  CU(ctx, own.dev(&sb.tile_bad, 2 * (size_t)sb.tiles_cap));
+  CU(ctx, own.dev(&sb.chunk_max, 2 * (size_t)sb.tiles_cap * BW_SC_WARPS));
   if (const char* e = getenv("BW_LATE_SPLIT")) f->late_split = atoi(e) != 0;
   if (const char* e = getenv("BW_FLUSH")) f->flush_on = atoi(e) != 0;
   if (const char* e = getenv("BW_TIMER_STRIDE")) f->timer_stride = (u32)std::max(1, atoi(e));
@@ -720,21 +822,21 @@ static bw_status stream_alloc(bw_fold* f) {
       f->precv_cnt_off[sd] = take(sizeof(u32) * (size_t)W * f->nb_local);
       f->precv_rec_off[sd] = take(sizeof(Partial) * (size_t)W * f->nb_local * f->part_cap);
     }
-    CU(ctx, cudaMalloc(&f->precv_base, off));
+    CU(ctx, own.dev(&f->precv_base, off));
     CU(ctx, cudaMemset(f->precv_base, 0, off));
     {
       bw_status cst = coll_share_base(ctx, f->precv_base, f->precv_peer, f->s_compute);
       if (cst != BW_OK) return cst;
     }
-    CU(ctx, dmalloc(&f->d_vg_local, 2));
-    CU(ctx, dmalloc(&f->d_vg_all, 2 * (size_t)W));
-    CU(ctx, cudaHostAlloc((void**)&f->h_vg, sizeof(VerdictGather) * 2 * W, cudaHostAllocDefault));
-    CU(ctx, dmalloc(&f->d_barrier_word, 1));
+    CU(ctx, own.dev(&f->d_vg_local, 2));
+    CU(ctx, own.dev(&f->d_vg_all, 2 * (size_t)W));
+    CU(ctx, own.host(&f->h_vg, 2 * (size_t)W));
+    CU(ctx, own.dev(&f->d_barrier_word, 1));
     CU(ctx, cudaMemset(f->d_barrier_word, 0, 4));
     // the legacy path is now the fallback of single activations: it runs in line with the rest (its own stream only
     // bought overlap between consecutive legacy activations, and its lateness pass must see the maximum set here)
     if (f->s_x && f->s_x != f->s_compute) {
-      cudaStreamDestroy(f->s_x);
+      own.release(f->s_x);
       f->s_x = f->s_compute;
     }
   }
@@ -774,57 +876,54 @@ static bw_status fold_alloc(bw_fold* f) {
     want = std::min<u64>(want, (u64)(free_b / 4) / (sizeof(PaneNode) + sizeof(u64) + sizeof(u32)));
     f->t.pool_cap = (u32)std::min<u64>(want, 0x7FFFFFF0ULL);
   }
-  CU(ctx, dmalloc(&f->t.hot, cap + 1));
-  CU(ctx, dmalloc(&f->t.p1, cap + 1));
-  CU(ctx, dmalloc(&f->t.closed_upto, cap + 1));
-  CU(ctx, dmalloc(&f->t.aux, cap + 1));
-  CU(ctx, dmalloc(&f->t.nodes, f->t.pool_cap));
-  CU(ctx, dmalloc(&f->t.node_acc2, f->t.pool_cap));
-  CU(ctx, dmalloc(&f->t.free_stack, f->t.pool_cap));
-  CU(ctx, dmalloc(&f->t.dirty, cap + 2));
-  CU(ctx, dmalloc(&f->d_ctr, 1));
+  Owner& own = f->own;
+  CU(ctx, own.dev(&f->t.hot, cap + 1));
+  CU(ctx, own.dev(&f->t.p1, cap + 1));
+  CU(ctx, own.dev(&f->t.closed_upto, cap + 1));
+  CU(ctx, own.dev(&f->t.aux, cap + 1));
+  CU(ctx, own.dev(&f->t.nodes, f->t.pool_cap));
+  CU(ctx, own.dev(&f->t.node_acc2, f->t.pool_cap));
+  CU(ctx, own.dev(&f->t.free_stack, f->t.pool_cap));
+  CU(ctx, own.dev(&f->t.dirty, cap + 2));
+  CU(ctx, own.dev(&f->d_ctr, 1));
   f->t.ctr = f->d_ctr;
-  CU(ctx, cudaHostAlloc((void**)&f->h_ctr, sizeof(Counters), cudaHostAllocDefault));
+  CU(ctx, own.host(&f->h_ctr, 1));
   // emit buffers
   f->e.max_closed = s.max_emit_rows;
   f->e.max_late = s.max_late_rows;
-  CU(ctx, dmalloc(&f->e.c_key, s.max_emit_rows));
-  CU(ctx, dmalloc(&f->e.c_wid, s.max_emit_rows));
-  CU(ctx, dmalloc(&f->e.c_acc, s.max_emit_rows));
-  CU(ctx, dmalloc(&f->e.c_count, s.max_emit_rows));
-  CU(ctx, dmalloc(&f->e.c_seq, s.max_emit_rows));
-  CU(ctx, dmalloc(&f->e.c_epoch, s.max_emit_rows));
-  CU(ctx, dmalloc(&f->e.l_key, s.max_late_rows));
-  CU(ctx, dmalloc(&f->e.l_wid, s.max_late_rows));
-  CU(ctx, dmalloc(&f->e.l_val, s.max_late_rows));
-  CU(ctx, dmalloc(&f->e.l_ts, s.max_late_rows));
-  CU(ctx, dmalloc(&f->e.l_seq, s.max_late_rows));
-  CU(ctx, dmalloc(&f->e.l_epoch, s.max_late_rows));
+  CU(ctx, own.dev(&f->e.c_key, s.max_emit_rows));
+  CU(ctx, own.dev(&f->e.c_wid, s.max_emit_rows));
+  CU(ctx, own.dev(&f->e.c_acc, s.max_emit_rows));
+  CU(ctx, own.dev(&f->e.c_count, s.max_emit_rows));
+  CU(ctx, own.dev(&f->e.c_seq, s.max_emit_rows));
+  CU(ctx, own.dev(&f->e.c_epoch, s.max_emit_rows));
+  CU(ctx, own.dev(&f->e.l_key, s.max_late_rows));
+  CU(ctx, own.dev(&f->e.l_wid, s.max_late_rows));
+  CU(ctx, own.dev(&f->e.l_val, s.max_late_rows));
+  CU(ctx, own.dev(&f->e.l_ts, s.max_late_rows));
+  CU(ctx, own.dev(&f->e.l_seq, s.max_late_rows));
+  CU(ctx, own.dev(&f->e.l_epoch, s.max_late_rows));
   // prepass
   f->max_recv_rows = s.max_batch_rows * (u64)ctx->world;
   u64 nranges = (f->max_recv_rows + BW_RANGE_ROWS - 1) / BW_RANGE_ROWS + 1;
-  CU(ctx, dmalloc(&f->d_rmin, nranges));
-  CU(ctx, dmalloc(&f->d_rmax, nranges));
-  CU(ctx, dmalloc(&f->d_rbad, nranges));
-  CU(ctx, dmalloc(&f->d_verdict, 1));
-  CU(ctx, dmalloc(&f->d_span, 2));
-  CU(ctx, cudaHostAlloc((void**)&f->h_verdict, 64, cudaHostAllocDefault));
-  CU(ctx, cudaStreamCreateWithFlags(&f->s_compute, cudaStreamNonBlocking));
-  CU(ctx, cudaStreamCreateWithFlags(&f->s_copy, cudaStreamNonBlocking));
+  CU(ctx, own.dev(&f->d_rmin, nranges));
+  CU(ctx, own.dev(&f->d_rmax, nranges));
+  CU(ctx, own.dev(&f->d_rbad, nranges));
+  CU(ctx, own.dev(&f->d_verdict, 1));
+  CU(ctx, own.dev(&f->d_span, 2));
+  CU(ctx, own.host(&f->h_verdict, 64 / sizeof(u32)));
+  CU(ctx, own.stream(&f->s_compute));
+  CU(ctx, own.stream(&f->s_copy));
   {
     // the verdict pass gates the next fold: let its blocks be placed first whenever an SM has room
     int prio_lo = 0, prio_hi = 0;
     CU(ctx, cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi));
-    CU(ctx, cudaStreamCreateWithPriority(&f->s_pre, cudaStreamNonBlocking, prio_hi));
+    CU(ctx, own.stream(&f->s_pre, prio_hi));
   }
   if (getenv("BW_NO_OVERLAP")) f->s_x = f->s_compute;  // diagnostic: serialise exchange and fold
-  else CU(ctx, cudaStreamCreateWithFlags(&f->s_x, cudaStreamNonBlocking));
-  CU(ctx, cudaEventCreateWithFlags(&f->ev_fold_done, cudaEventDisableTiming));
-  CU(ctx, cudaEventCreateWithFlags(&f->ev_xchg_done, cudaEventDisableTiming));
-  CU(ctx, cudaEventCreateWithFlags(&f->ev_src_ready, cudaEventDisableTiming));
-  CU(ctx, cudaEventCreateWithFlags(&f->ev_in, cudaEventDisableTiming));
-  CU(ctx, cudaEventCreateWithFlags(&f->ev_pre, cudaEventDisableTiming));
-  CU(ctx, cudaEventCreateWithFlags(&f->ev_h2d, cudaEventDisableTiming));
+  else CU(ctx, own.stream(&f->s_x));
+  for (cudaEvent_t* e : {&f->ev_fold_done, &f->ev_xchg_done, &f->ev_src_ready, &f->ev_in, &f->ev_pre, &f->ev_h2d})
+    CU(ctx, own.event(e));
   // No persisting-L2 carve-out: a persisting window on the hot slots would leave too little normal
   // L2 for the second-pane array at window boundaries; plain LRU + evict_first input loads instead.
   int occ = 0;
@@ -882,23 +981,24 @@ static bw_status xchg_setup(bw_fold* f) {
   f->region_cap = f->spec.max_batch_rows;  // worst case: every row of a source goes to one rank
   XLayout L = xlayout(f);
   f->xchg_bytes = L.total;
-  CU(ctx, cudaMalloc(&f->xchg_base, L.total));
+  Owner& own = f->own;
+  CU(ctx, own.dev(&f->xchg_base, L.total));
   CU(ctx, cudaMemset(f->xchg_base, 0, L.total));
   CU(ctx, cudaFuncSetAttribute(k_part_scatter, cudaFuncAttributeMaxDynamicSharedMemorySize, BW_PART_TILE * 24));
   u64 ntiles = (f->spec.max_batch_rows + BW_PART_TILE - 1) / BW_PART_TILE + 1;
-  CU(ctx, dmalloc(&f->d_tile_counts, ntiles * BW_MAX_WORLD));
+  CU(ctx, own.dev(&f->d_tile_counts, ntiles * BW_MAX_WORLD));
   if (f->spec.exchange == BW_XCHG_P2P) {
     // every peer's receive buffer as seen from here (CUDA IPC mappings exchanged through NCCL)
     bw_status cst = coll_share_base(ctx, f->xchg_base, f->peer_base, f->s_compute);
     if (cst != BW_OK) return cst;
   } else {
     const size_t rows = (size_t)f->region_cap * W;
-    CU(ctx, dmalloc(&f->send_keys, rows));
-    if (f->has_vals) CU(ctx, cudaMalloc(&f->send_vals, rows * (size_t)f->val_bytes));
-    if (f->has_ts) CU(ctx, dmalloc(&f->send_ts, rows));
-    CU(ctx, dmalloc(&f->d_send_counts, BW_MAX_WORLD));
-    CU(ctx, dmalloc(&f->d_all_counts, (size_t)BW_MAX_WORLD * BW_MAX_WORLD));
-    CU(ctx, cudaHostAlloc((void**)&f->h_all_counts, sizeof(u64) * BW_MAX_WORLD * BW_MAX_WORLD, cudaHostAllocDefault));
+    CU(ctx, own.dev(&f->send_keys, rows));
+    if (f->has_vals) CU(ctx, own.dev(&f->send_vals, rows * (size_t)f->val_bytes));
+    if (f->has_ts) CU(ctx, own.dev(&f->send_ts, rows));
+    CU(ctx, own.dev(&f->d_send_counts, BW_MAX_WORLD));
+    CU(ctx, own.dev(&f->d_all_counts, (size_t)BW_MAX_WORLD * BW_MAX_WORLD));
+    CU(ctx, own.host(&f->h_all_counts, (size_t)BW_MAX_WORLD * BW_MAX_WORLD));
     for (int r = 0; r < W; ++r) f->peer_base[r] = nullptr;
     f->peer_base[ctx->rank] = f->xchg_base;
   }
@@ -923,9 +1023,11 @@ bw_status bw_fold_create(bw_ctx* ctx, const bw_fold_spec* spec, bw_fold** out) {
   if (spec->max_batch_rows == 0 || spec->max_batch_rows >= (1ULL << 32) / (u64)ctx->world)
     CTX_FAIL(ctx, BW_ERR_SPEC, "max_batch_rows * world must be in [1, 2^32)");
   CU(ctx, cudaSetDevice(ctx->device));
-  bw_fold* f = new bw_fold();
+  std::unique_ptr<bw_fold, void (*)(bw_fold*)> fp(new bw_fold(), bw_fold_destroy);  // torn down on every failure
+  bw_fold* f = fp.get();
   f->ctx = ctx;
   f->spec = *spec;
+  f->pt.own = &f->own;
   FoldParams& p = f->p;
   p.length_us = spec->length_us;
   p.offset_us = spec->offset_us;
@@ -993,12 +1095,12 @@ bw_status bw_fold_create(bw_ctx* ctx, const bw_fold_spec* spec, bw_fold** out) {
     if (st != BW_OK) return st;
   }
   // emission staging is sized once: no allocation on the advance path
-  st = ensure_sort_cap(f, std::max<u64>(spec->max_emit_rows, spec->max_late_rows));
-  if (st != BW_OK) return st;
-  st = grow_host(f, spec->max_emit_rows, spec->max_late_rows);
-  if (st != BW_OK) return st;
+  const u64 n_emit = std::max<u64>(spec->max_emit_rows, spec->max_late_rows);
+  CU(ctx, f->srt.reserve(f->own, n_emit, std::max<u64>(n_emit, 4096), f->s_compute));
+  CU(ctx, f->ho_c.reserve(f->own, spec->max_emit_rows, std::max<u64>(spec->max_emit_rows, 4096)));
+  CU(ctx, f->ho_l.reserve(f->own, spec->max_late_rows, std::max<u64>(spec->max_late_rows, 4096)));
   CU(ctx, cudaStreamSynchronize(f->s_compute));
-  *out = f;
+  *out = fp.release();
   return BW_OK;
 }
 
@@ -1015,68 +1117,7 @@ void bw_fold_destroy(bw_fold* f) {
       if (f->peer_base[r] && f->spec.exchange == BW_XCHG_P2P) cudaIpcCloseMemHandle(f->peer_base[r]);
       if (f->precv_peer[r]) cudaIpcCloseMemHandle(f->precv_peer[r]);
     }
-  void* dev[] = {f->t.hot, f->t.p1, f->t.closed_upto, f->t.aux, f->t.nodes, f->t.node_acc2, f->t.free_stack, f->t.dirty, f->d_ctr, f->e.c_key,
-                 f->e.c_wid, f->e.c_acc, f->e.c_count, f->e.c_seq, f->e.c_epoch, f->e.l_key, f->e.l_wid, f->e.l_val,
-                 f->e.l_ts, f->e.l_seq, f->e.l_epoch, f->d_rmin, f->d_rmax, f->d_rbad, f->d_verdict, f->d_kflat,
-                 f->d_ksorted, f->d_tsflat, f->d_tssorted, f->d_prefmax, f->d_idx, f->d_idxsorted, f->d_late, f->d_cub,
-                 f->d_sk, f->d_sk2, f->d_gather, f->d_perm, f->d_perm2, f->xchg_base, f->d_tile_counts,
-                 f->d_send_counts, f->d_all_counts, f->send_keys, f->send_vals, f->send_ts, f->d_span, f->snap_dev, f->d_snap_ctr};
-  for (void* p : dev)
-    if (p) cudaFree(p);
-  for (int i = 0; i < 2; ++i) {
-    void* sp[] = {f->sb.side[i].rec, f->sb.side[i].val, f->sb.side[i].cnt, f->sb.side[i].spill, f->sb.side[i].sv};
-    for (void* q : sp)
-      if (q) cudaFree(q);
-    if (f->ev_sv[i]) cudaEventDestroy(f->ev_sv[i]);
-  }
-  {
-    void* sp[] = {f->sb.tile_min, f->sb.tile_max, f->sb.tile_bad, f->sb.chunk_max};
-    for (void* q : sp)
-      if (q) cudaFree(q);
-    if (f->h_sv) cudaFreeHost(f->h_sv);
-    void* lp[] = {f->late.key_bits, f->late.late_bits, f->late.ent, f->late.counters, f->late.gpre, f->late_chunk_pre, f->late.s_key, f->late.s_ts, f->late.s_idx, f->late.s_slot};
-    for (void* q : lp)
-      if (q) cudaFree(q);
-    if (f->h_late_ctr) cudaFreeHost(f->h_late_ctr);
-  }
-  for (auto& s : f->stages) {
-    if (s.d_keys) cudaFree(s.d_keys);
-    if (s.d_vals) cudaFree(s.d_vals);
-    if (s.d_ts) cudaFree(s.d_ts);
-    if (s.consumed) cudaEventDestroy(s.consumed);
-  }
-  for (auto& s : f->slots) {
-    if (s.h_keys) cudaFreeHost(s.h_keys);
-    if (s.h_vals) cudaFreeHost(s.h_vals);
-    if (s.h_ts) cudaFreeHost(s.h_ts);
-  }
-  void* host[] = {f->snap_host, f->h_ctr, f->h_verdict, f->h_all_counts, f->ho_ckey, f->ho_cacc, f->ho_ccount, f->ho_cepoch,
-                  f->ho_cwid, f->ho_lkey, f->ho_lval, f->ho_lepoch, f->ho_lwid, f->ho_lts};
-  for (void* p : host)
-    if (p) cudaFreeHost(p);
-  for (auto& t : f->timers) {
-    cudaEventDestroy(t.a);
-    cudaEventDestroy(t.b);
-  }
-  if (f->s_out) {
-    cudaStreamSynchronize(f->s_out);
-    cudaStreamDestroy(f->s_out);
-    void* q[] = {f->fl.sk, f->fl.sk2, f->fl.gather, f->fl.perm, f->fl.perm2, f->fl.cub};
-    for (void* x : q)
-      if (x) cudaFree(x);
-    for (auto& m : f->marks)
-      if (m.ev) cudaEventDestroy(m.ev);
-    if (f->h_marks) cudaFreeHost(f->h_marks);
-  }
-  if (f->s_compute) cudaStreamDestroy(f->s_compute);
-  if (f->s_copy) cudaStreamDestroy(f->s_copy);
-  if (f->s_pre) cudaStreamDestroy(f->s_pre);
-  if (f->s_x && f->s_x != f->s_compute) cudaStreamDestroy(f->s_x);
-  if (f->ev_in) cudaEventDestroy(f->ev_in);
-  if (f->ev_gen) cudaEventDestroy(f->ev_gen);
-  if (f->ev_pre) cudaEventDestroy(f->ev_pre);
-  if (f->ev_h2d) cudaEventDestroy(f->ev_h2d);
-  delete f;
+  delete f;  // f->own releases every buffer, event and stream
 }
 
 // ---------------------------------------------------------------------------
@@ -1098,9 +1139,9 @@ bw_status bw_ingest_acquire(bw_fold* f, uint64_t max_rows, bw_batch* out) {
     if (f->slots.size() >= nslots) FAIL(f, BW_ERR_STATE, "all %u ingest slots are acquired; commit one first", nslots);
     Slot s;
     const size_t rows = f->spec.max_batch_rows;
-    CU(ctx, cudaHostAlloc((void**)&s.h_keys, rows * 8, cudaHostAllocDefault));
-    if (f->has_vals) CU(ctx, cudaHostAlloc(&s.h_vals, rows * (size_t)f->val_bytes, cudaHostAllocDefault));
-    if (f->has_ts) CU(ctx, cudaHostAlloc((void**)&s.h_ts, rows * 8, cudaHostAllocDefault));
+    CU(ctx, f->own.host(&s.h_keys, rows));
+    if (f->has_vals) CU(ctx, f->own.host(&s.h_vals, rows * (size_t)f->val_bytes));
+    if (f->has_ts) CU(ctx, f->own.host(&s.h_ts, rows));
     f->slots.push_back(s);
     pick = (u32)f->slots.size() - 1;
   }
@@ -1123,7 +1164,7 @@ static EventPair* next_timer(bw_fold* f, u32 batch_no) {
   if (f->timers_used == f->timers.size()) {
     if (f->timers.size() >= 4096) return nullptr;
     EventPair ep;
-    if (cudaEventCreate(&ep.a) != cudaSuccess || cudaEventCreate(&ep.b) != cudaSuccess) return nullptr;
+    if (f->own.event(&ep.a, cudaEventDefault) != cudaSuccess || f->own.event(&ep.b, cudaEventDefault) != cudaSuccess) return nullptr;
     ep.rows = 0;
     ep.kind = 0;
     f->timers.push_back(ep);
@@ -1382,8 +1423,6 @@ static bw_status stream_front(bw_fold* f, const u64* d_keys, const void* d_vals,
 
 static bw_status slow_path(bw_fold* f, const BatchView& bv, u64 total, u64 epoch_ord, u32 batch_no);
 
-static bw_status slow_path(bw_fold* f, const BatchView& bv, u64 total, u64 epoch_ord, u32 batch_no);
-
 // The direct path of one activation, start to finish: (world > 1: partition + exchange of the rows) -> lateness pass ->
 // k_fold or the exact path -> K4.
 static bw_status legacy_batch(bw_fold* f, const u64* d_keys, const void* d_vals, const i64* d_ts, u64 rows, u32 batch_no, u64 ord, Stage* stage) {
@@ -1479,7 +1518,7 @@ static bw_status gather_verdict(bw_fold* f, int side) {
     if (cst != BW_OK) return cst;
   }
   CU(ctx, cudaMemcpyAsync(f->h_vg + (size_t)side * W, all, sizeof(VerdictGather) * W, cudaMemcpyDeviceToHost, s));
-  if (!f->ev_vg[side]) CU(ctx, cudaEventCreateWithFlags(&f->ev_vg[side], cudaEventDisableTiming));
+  if (!f->ev_vg[side]) CU(ctx, f->own.event(&f->ev_vg[side]));
   CU(ctx, cudaEventRecord(f->ev_vg[side], s));
   f->vg_pending[side] = false;
   return BW_OK;
@@ -1632,18 +1671,19 @@ static bw_status late_split(bw_fold* f, const Deferred& d, const BatchView& bv, 
     u32 kb = 1u << 16;
     while (kb < 16 * L.cap && kb < (1u << 27)) kb <<= 1;
     L.kb_mask = kb - 1;
-    CU(ctx, dmalloc(&L.key_bits, kb / 32));
-    CU(ctx, dmalloc(&L.late_bits, maxr / 32 + 2));
-    CU(ctx, dmalloc(&L.ent, M));
+    Owner& own = f->own;
+    CU(ctx, own.dev(&L.key_bits, kb / 32));
+    CU(ctx, own.dev(&L.late_bits, maxr / 32 + 2));
+    CU(ctx, own.dev(&L.ent, M));
     CU(ctx, cudaMemsetAsync(L.ent, 0, (size_t)M * sizeof(LateEnt), s));  // generation 0: every entry free, once
-    CU(ctx, dmalloc(&L.counters, 2));
-    CU(ctx, dmalloc(&L.s_key, L.cap));
-    CU(ctx, dmalloc(&L.s_ts, L.cap));
-    CU(ctx, dmalloc(&L.s_idx, L.cap));
-    CU(ctx, dmalloc(&L.s_slot, L.cap));
-    CU(ctx, dmalloc(&L.gpre, sb.tiles_cap));
-    CU(ctx, dmalloc(&f->late_chunk_pre, (size_t)sb.tiles_cap * BW_SC_WARPS));
-    CU(ctx, cudaHostAlloc((void**)&f->h_late_ctr, 2 * sizeof(u32), cudaHostAllocDefault));
+    CU(ctx, own.dev(&L.counters, 2));
+    CU(ctx, own.dev(&L.s_key, L.cap));
+    CU(ctx, own.dev(&L.s_ts, L.cap));
+    CU(ctx, own.dev(&L.s_idx, L.cap));
+    CU(ctx, own.dev(&L.s_slot, L.cap));
+    CU(ctx, own.dev(&L.gpre, sb.tiles_cap));
+    CU(ctx, own.dev(&f->late_chunk_pre, (size_t)sb.tiles_cap * BW_SC_WARPS));
+    CU(ctx, own.host(&f->h_late_ctr, 2));
     f->late_ready = true;
   }
   const u64 rows = d.rows;
@@ -1847,12 +1887,12 @@ bw_status bw_ingest_commit(bw_fold* f, const bw_batch* batch, uint64_t rows, uin
   if (f->stages.empty()) f->stages.resize(3);
   Stage& sg = f->stages[f->stage_next];
   f->stage_next = (f->stage_next + 1) % (u32)f->stages.size();
-  if (!sg.d_keys) {
+  if (!sg.consumed) {  // (made last: a stage is complete once it has its event)
     const size_t cap = f->spec.max_batch_rows;
-    CU(ctx, dmalloc(&sg.d_keys, cap));
-    if (f->has_vals) CU(ctx, cudaMalloc(&sg.d_vals, cap * (size_t)f->val_bytes));
-    if (f->has_ts) CU(ctx, dmalloc(&sg.d_ts, cap));
-    CU(ctx, cudaEventCreateWithFlags(&sg.consumed, cudaEventDisableTiming));
+    CU(ctx, f->own.dev(&sg.d_keys, cap));
+    if (f->has_vals) CU(ctx, f->own.dev(&sg.d_vals, cap * (size_t)f->val_bytes));
+    if (f->has_ts) CU(ctx, f->own.dev(&sg.d_ts, cap));
+    CU(ctx, f->own.event(&sg.consumed));
   }
   if (sg.used) CU(ctx, cudaStreamWaitEvent(f->s_copy, sg.consumed, 0));
   if (rows) {
@@ -1908,37 +1948,32 @@ static bw_status slow_path(bw_fold* f, const BatchView& bv, u64 total, u64 epoch
   cudaStream_t s = f->s_compute;
   if (total == 0) return BW_OK;
   if (total > f->slow_cap) {
-    void* old[] = {f->d_kflat, f->d_ksorted, f->d_tsflat, f->d_tssorted, f->d_prefmax, f->d_idx, f->d_idxsorted, f->d_late};
     CU(ctx, cudaStreamSynchronize(s));
-    for (void* p : old)
-      if (p) cudaFree(p);
-    u64 cap = std::max<u64>(total, 1024);
-    CU(ctx, dmalloc(&f->d_kflat, cap));
-    CU(ctx, dmalloc(&f->d_ksorted, cap));
-    CU(ctx, dmalloc(&f->d_tsflat, cap));
-    CU(ctx, dmalloc(&f->d_tssorted, cap));
-    CU(ctx, dmalloc(&f->d_prefmax, cap));
-    CU(ctx, dmalloc(&f->d_idx, cap));
-    CU(ctx, dmalloc(&f->d_idxsorted, cap));
-    CU(ctx, dmalloc(&f->d_late, cap));
+    const u64 cap = std::max<u64>(total, 1024);
+    Owner& own = f->own;
+    f->slow_cap = 0;
+    CU(ctx, own.regrow(Owner::DEV, &f->d_kflat, cap));
+    CU(ctx, own.regrow(Owner::DEV, &f->d_ksorted, cap));
+    CU(ctx, own.regrow(Owner::DEV, &f->d_tsflat, cap));
+    CU(ctx, own.regrow(Owner::DEV, &f->d_tssorted, cap));
+    CU(ctx, own.regrow(Owner::DEV, &f->d_prefmax, cap));
+    CU(ctx, own.regrow(Owner::DEV, &f->d_idx, cap));
+    CU(ctx, own.regrow(Owner::DEV, &f->d_idxsorted, cap));
+    CU(ctx, own.regrow(Owner::DEV, &f->d_late, cap));
     size_t b1 = 0, b2 = 0;
     cub::DeviceRadixSort::SortPairs(nullptr, b1, f->d_kflat, f->d_ksorted, f->d_idx, f->d_idxsorted, (int)cap, 0, 64, s);
     cub::DeviceScan::ExclusiveScanByKey(nullptr, b2, f->d_ksorted, f->d_tssorted, f->d_prefmax, MaxI64(), (i64)INT64_MIN,
                                         (int)cap, ::cuda::std::equal_to<>(), s);
-    if (std::max(b1, b2) + 256 > f->cub_bytes) {  // the scratch is shared with the emission sort: only ever grow it
-      if (f->d_cub) cudaFree(f->d_cub);
-      f->cub_bytes = std::max(b1, b2) + 256;
-      CU(ctx, cudaMalloc(&f->d_cub, f->cub_bytes));
-    }
+    CU(ctx, f->srt.grow_cub(own, std::max(b1, b2) + 256));  // (the emission sort's CUB storage)
     f->slow_cap = cap;
   }
   const int grid = ctx->sm_count * 8;
   k_slow_flatten<<<grid, 256, 0, s>>>(bv, f->p, f->d_kflat, f->d_tsflat, f->d_idx);
-  size_t tb = f->cub_bytes;
-  CU(ctx, cub::DeviceRadixSort::SortPairs(f->d_cub, tb, f->d_kflat, f->d_ksorted, f->d_idx, f->d_idxsorted, (int)total, 0, 64, s));
+  size_t tb = f->srt.cub_bytes;
+  CU(ctx, cub::DeviceRadixSort::SortPairs(f->srt.cub, tb, f->d_kflat, f->d_ksorted, f->d_idx, f->d_idxsorted, (int)total, 0, 64, s));
   k_gather_i64<<<grid, 256, 0, s>>>(f->d_tsflat, f->d_idxsorted, f->d_tssorted, total);
-  tb = f->cub_bytes;
-  CU(ctx, cub::DeviceScan::ExclusiveScanByKey(f->d_cub, tb, f->d_ksorted, f->d_tssorted, f->d_prefmax, MaxI64(),
+  tb = f->srt.cub_bytes;
+  CU(ctx, cub::DeviceScan::ExclusiveScanByKey(f->srt.cub, tb, f->d_ksorted, f->d_tssorted, f->d_prefmax, MaxI64(),
                                               (i64)INT64_MIN, (int)total, ::cuda::std::equal_to<>(), s));
   k_slow_classify<<<grid, 256, 0, s>>>(f->t, f->p, f->d_ksorted, f->d_idxsorted, f->d_tssorted, f->d_prefmax, f->d_late, total);
   k_slow_fold<<<f->fold_grid, BW_FOLD_THREADS, 0, s>>>(bv, f->t, f->p, f->e, f->d_late, batch_no, epoch_ord);
@@ -1950,90 +1985,31 @@ static bw_status slow_path(bw_fold* f, const BatchView& bv, u64 total, u64 epoch
 // ---------------------------------------------------------------------------
 // advance / eof
 // ---------------------------------------------------------------------------
-static bw_status ensure_sort_cap(bw_fold* f, u64 n) {
-  bw_ctx* ctx = f->ctx;
-  if (n <= f->sort_cap) return BW_OK;
-  void* old[] = {f->d_sk, f->d_sk2, f->d_gather, f->d_perm, f->d_perm2};
-  for (void* p : old)
-    if (p) cudaFree(p);
-  u64 cap = std::max<u64>(n, 4096);
-  CU(ctx, dmalloc(&f->d_sk, cap));
-  CU(ctx, dmalloc(&f->d_sk2, cap));
-  CU(ctx, dmalloc(&f->d_gather, cap));
-  CU(ctx, dmalloc(&f->d_perm, cap));
-  CU(ctx, dmalloc(&f->d_perm2, cap));
-  size_t b = 0;
-  cub::DeviceRadixSort::SortPairs(nullptr, b, f->d_sk, f->d_sk2, f->d_perm, f->d_perm2, (int)cap, 0, 64, f->s_compute);
-  if (b + 256 > f->cub_bytes) {
-    if (f->d_cub) cudaFree(f->d_cub);
-    f->cub_bytes = b + 256;
-    CU(ctx, cudaMalloc(&f->d_cub, f->cub_bytes));
-  }
-  f->sort_cap = cap;
-  return BW_OK;
-}
-
-// Build the reference-order permutation of n rows (LSD passes of stable radix sorts).
-static bw_status order_rows(bw_fold* f, u64 n, const u64* key, const u64* seq, const u64* epoch, const i64* wid,
-                            bool wid_pass, u64 n_ordinals, bool side = false) {
-  bw_ctx* ctx = f->ctx;
-  cudaStream_t s = side ? f->s_out : f->s_compute;
-  // (the side stream sorts in its own scratch: the main one is shared with the sort path of not-clean activations)
-  u64 *&d_sk = side ? f->fl.sk : f->d_sk, *&d_sk2 = side ? f->fl.sk2 : f->d_sk2;
-  u32 *&d_perm = side ? f->fl.perm : f->d_perm, *&d_perm2 = side ? f->fl.perm2 : f->d_perm2;
-  void* d_cub = side ? f->fl.cub : f->d_cub;
-  const size_t cub_bytes = side ? f->fl.cub_bytes : f->cub_bytes;
+// Build the reference-order permutation of n rows into x.perm (LSD passes of stable radix sorts).  A null `wid` skips
+// the window-id pass.  The kernels this library launches are added to *launches, if given (CUB's are not counted).
+static bw_status order_perm(bw_ctx* ctx, SortScratch& x, cudaStream_t s, u64 n, const u64* key, const u64* seq,
+                            const u64* epoch, const i64* wid, u64 n_ordinals, u64 min_epoch, uint64_t* launches) {
   const int grid = ctx->sm_count * 4;
-  k_iota<<<grid, 256, 0, s>>>(d_perm, n);
-  f->st.kernel_launches++;
+  k_iota<<<grid, 256, 0, s>>>(x.perm, n);
   struct Pass {
     int kind, bits;
   };
   int ebits = 1;
   while ((1ULL << ebits) < n_ordinals + 1) ++ebits;
   std::vector<Pass> passes;
-  if (wid_pass) passes.push_back({BW_SK_WID, 64});
+  if (wid) passes.push_back({BW_SK_WID, 64});
   passes.push_back({BW_SK_SEQ, 64});
   passes.push_back({BW_SK_DIGITS, 16});
   passes.push_back({BW_SK_ALIGNED, 64});
   if (n_ordinals > 1) passes.push_back({BW_SK_EPOCH, ebits});
+  if (launches) *launches += 1 + passes.size();
   for (const Pass& ps : passes) {
-    k_sortkey<<<grid, 256, 0, s>>>(ps.kind, key, seq, epoch, wid, d_perm, d_sk, n, f->min_epoch);
-    size_t tb = cub_bytes;
-    CU(ctx, cub::DeviceRadixSort::SortPairs(d_cub, tb, d_sk, d_sk2, d_perm, d_perm2, (int)n, 0, ps.bits, s));
-    std::swap(d_perm, d_perm2);
-    f->st.kernel_launches++;
+    k_sortkey<<<grid, 256, 0, s>>>(ps.kind, key, seq, epoch, wid, x.perm, x.sk, n, min_epoch);
+    size_t tb = x.cub_bytes;
+    CU(ctx, cub::DeviceRadixSort::SortPairs(x.cub, tb, x.sk, x.sk2, x.perm, x.perm2, (int)n, 0, ps.bits, s));
+    std::swap(x.perm, x.perm2);
   }
   CU(ctx, cudaGetLastError());
-  return BW_OK;
-}
-
-static bw_status grow_host(bw_fold* f, u64 nc, u64 nl) {
-  bw_ctx* ctx = f->ctx;
-  if (nc > f->hout_cap_c) {
-    void* old[] = {f->ho_ckey, f->ho_cacc, f->ho_ccount, f->ho_cepoch, f->ho_cwid};
-    for (void* p : old)
-      if (p) cudaFreeHost(p);
-    u64 cap = std::max<u64>(nc, 4096);
-    CU(ctx, cudaHostAlloc((void**)&f->ho_ckey, cap * 8, cudaHostAllocDefault));
-    CU(ctx, cudaHostAlloc((void**)&f->ho_cacc, cap * 8, cudaHostAllocDefault));
-    CU(ctx, cudaHostAlloc((void**)&f->ho_ccount, cap * 8, cudaHostAllocDefault));
-    CU(ctx, cudaHostAlloc((void**)&f->ho_cepoch, cap * 8, cudaHostAllocDefault));
-    CU(ctx, cudaHostAlloc((void**)&f->ho_cwid, cap * 8, cudaHostAllocDefault));
-    f->hout_cap_c = cap;
-  }
-  if (nl > f->hout_cap_l) {
-    void* old[] = {f->ho_lkey, f->ho_lval, f->ho_lepoch, f->ho_lwid, f->ho_lts};
-    for (void* p : old)
-      if (p) cudaFreeHost(p);
-    u64 cap = std::max<u64>(nl, 4096);
-    CU(ctx, cudaHostAlloc((void**)&f->ho_lkey, cap * 8, cudaHostAllocDefault));
-    CU(ctx, cudaHostAlloc((void**)&f->ho_lval, cap * 8, cudaHostAllocDefault));
-    CU(ctx, cudaHostAlloc((void**)&f->ho_lepoch, cap * 8, cudaHostAllocDefault));
-    CU(ctx, cudaHostAlloc((void**)&f->ho_lwid, cap * 8, cudaHostAllocDefault));
-    CU(ctx, cudaHostAlloc((void**)&f->ho_lts, cap * 8, cudaHostAllocDefault));
-    f->hout_cap_l = cap;
-  }
   return BW_OK;
 }
 
@@ -2058,55 +2034,30 @@ static bw_status ship_rows(bw_fold* f, bool late, u64 lo, u64 hi, bool side) {
   // pane, and folds whose sequence is just the closing activation (FoldParams::seq_by_id)
   const bool sliding = f->p.panes_per_window > 1 || f->p.panes_per_offset > 1 || f->p.seq_by_id;
   const EmitBufs& e = f->e;
+  // (the side stream sorts in its own scratch: the main one is shared with the sort path of not-clean activations)
+  SortScratch& x = side ? f->fl : f->srt;
   if (ordered) {
-    if (side && n > f->fl.cap) {  // (grow the side scratch: nothing is in flight on it once the stream is idle)
-      CU(ctx, cudaStreamSynchronize(s));
-      void* old[] = {f->fl.sk, f->fl.sk2, f->fl.gather, f->fl.perm, f->fl.perm2, f->fl.cub};
-      for (void* q : old)
-        if (q) cudaFree(q);
-      const u64 cap = std::max<u64>(2 * n, 1 << 16);
-      CU(ctx, dmalloc(&f->fl.sk, cap));
-      CU(ctx, dmalloc(&f->fl.sk2, cap));
-      CU(ctx, dmalloc(&f->fl.gather, cap));
-      CU(ctx, dmalloc(&f->fl.perm, cap));
-      CU(ctx, dmalloc(&f->fl.perm2, cap));
-      size_t b = 0;
-      cub::DeviceRadixSort::SortPairs(nullptr, b, f->fl.sk, f->fl.sk2, f->fl.perm, f->fl.perm2, (int)cap, 0, 64, s);
-      f->fl.cub_bytes = b + 256;
-      CU(ctx, cudaMalloc(&f->fl.cub, f->fl.cub_bytes));
-      f->fl.cap = cap;
-    }
+    if (side) CU(ctx, x.reserve(f->own, n, std::max<u64>(2 * n, 1 << 16), s));
     bw_status st;
-    if (!late) st = order_rows(f, n, e.c_key + lo, e.c_seq + lo, e.c_epoch + lo, e.c_wid + lo, sliding, n_ord, side);
+    if (!late) st = order_perm(ctx, x, s, n, e.c_key + lo, e.c_seq + lo, e.c_epoch + lo, sliding ? e.c_wid + lo : nullptr, n_ord,
+                               f->min_epoch, &f->st.kernel_launches);
     else  // rows of one late item were reserved contiguously in ascending window id; stable sorts keep that
-      st = order_rows(f, n, e.l_key + lo, e.l_seq + lo, e.l_epoch + lo, e.l_wid + lo, false, n_ord, side);
+      st = order_perm(ctx, x, s, n, e.l_key + lo, e.l_seq + lo, e.l_epoch + lo, nullptr, n_ord, f->min_epoch, &f->st.kernel_launches);
     if (st != BW_OK) return st;
   }
-  const u32* perm = side ? f->fl.perm : f->d_perm;
-  u64* gather = side ? f->fl.gather : f->d_gather;
-  auto ship = [&](const u64* src, u64* dst) -> bw_status {
+  // in the order of the host columns (bw_fold::ho_c, ho_l)
+  const u64* cols[2][5] = {{e.c_key, (const u64*)e.c_wid, e.c_acc, e.c_count, e.c_epoch},
+                           {e.l_key, (const u64*)e.l_wid, e.l_val, (const u64*)e.l_ts, e.l_epoch}};
+  const u64* const* src = cols[late];
+  u64* const* dst = late ? f->ho_l.col : f->ho_c.col;
+  for (int c = 0; c < 5; ++c) {
     if (ordered) {
-      k_gather_u64<<<grid, 256, 0, s>>>(src + lo, perm, gather, n);
+      k_gather_u64<<<grid, 256, 0, s>>>(src[c] + lo, x.perm, x.gather, n);
       f->st.kernel_launches++;
-      CU(ctx, cudaMemcpyAsync(dst + lo, gather, n * 8, cudaMemcpyDeviceToHost, s));
+      CU(ctx, cudaMemcpyAsync(dst[c] + lo, x.gather, n * 8, cudaMemcpyDeviceToHost, s));
     } else {
-      CU(ctx, cudaMemcpyAsync(dst + lo, src + lo, n * 8, cudaMemcpyDeviceToHost, s));
+      CU(ctx, cudaMemcpyAsync(dst[c] + lo, src[c] + lo, n * 8, cudaMemcpyDeviceToHost, s));
     }
-    return BW_OK;
-  };
-  bw_status st;
-  if (!late) {
-    if ((st = ship(e.c_key, f->ho_ckey))) return st;
-    if ((st = ship((const u64*)e.c_wid, (u64*)f->ho_cwid))) return st;
-    if ((st = ship(e.c_acc, f->ho_cacc))) return st;
-    if ((st = ship(e.c_count, f->ho_ccount))) return st;
-    if ((st = ship(e.c_epoch, f->ho_cepoch))) return st;
-  } else {
-    if ((st = ship(e.l_key, f->ho_lkey))) return st;
-    if ((st = ship((const u64*)e.l_wid, (u64*)f->ho_lwid))) return st;
-    if ((st = ship(e.l_val, f->ho_lval))) return st;
-    if ((st = ship((const u64*)e.l_ts, (u64*)f->ho_lts))) return st;
-    if ((st = ship(e.l_epoch, f->ho_lepoch))) return st;
   }
   return BW_OK;
 }
@@ -2115,10 +2066,10 @@ static bw_status ship_rows(bw_fold* f, bool late, u64 lo, u64 hi, bool side) {
 static bw_status mark_rows(bw_fold* f, u64 epoch) {
   bw_ctx* ctx = f->ctx;
   if (!f->flush_on || ctx->world > 1 || !f->host_ingest) return BW_OK;
-  if (!f->s_out) {
-    CU(ctx, cudaStreamCreateWithFlags(&f->s_out, cudaStreamNonBlocking));
-    CU(ctx, cudaHostAlloc((void**)&f->h_marks, 4 * 2 * sizeof(unsigned long long), cudaHostAllocDefault));
-    for (auto& m : f->marks) CU(ctx, cudaEventCreateWithFlags(&m.ev, cudaEventDisableTiming));
+  if (!f->s_out) {  // (the stream is made last: the side flush is ready once it exists)
+    CU(ctx, f->own.host(&f->h_marks, 4 * 2));
+    for (auto& m : f->marks) CU(ctx, f->own.event(&m.ev));
+    CU(ctx, f->own.stream(&f->s_out));
   }
   if (f->mark_head) f->marks[(f->mark_head - 1) & 3].next_epoch = epoch + 1;  // (+1: 0 means "none yet")
   bw_fold::RowMark& m = f->marks[f->mark_head & 3];
@@ -2171,8 +2122,9 @@ static bw_status collect(bw_fold* f, bw_emit* out) {
   const u64 nl = std::min<u64>(f->h_ctr->n_late, f->e.max_late);
   f->st.live_keys = f->h_ctr->live_keys;
   f->st.pane_nodes_used = f->h_ctr->pool_next - 1;
-  bw_status st = grow_host(f, nc, nl);
-  if (st != BW_OK) return st;
+  CU(ctx, f->ho_c.reserve(f->own, nc, std::max<u64>(nc, 4096)));
+  CU(ctx, f->ho_l.reserve(f->own, nl, std::max<u64>(nl, 4096)));
+  bw_status st;
   // what the side stream has not already ordered and copied (everything, when nothing was flushed early)
   if ((st = ship_rows(f, false, std::min(f->done_c, nc), nc, false))) return st;
   if ((st = ship_rows(f, true, std::min(f->done_l, nl), nl, false))) return st;
@@ -2183,17 +2135,17 @@ static bw_status collect(bw_fold* f, bw_emit* out) {
   CU(ctx, cudaStreamSynchronize(s));
   f->have_pending = false;
   out->n_closed = nc;
-  out->closed_key = f->ho_ckey;
-  out->closed_window_id = f->ho_cwid;
-  out->closed_acc = f->ho_cacc;
-  out->closed_count = f->ho_ccount;
-  out->closed_epoch = f->ho_cepoch;
+  out->closed_key = f->ho_c.col[0];
+  out->closed_window_id = (i64*)f->ho_c.col[1];
+  out->closed_acc = f->ho_c.col[2];
+  out->closed_count = f->ho_c.col[3];
+  out->closed_epoch = f->ho_c.col[4];
   out->n_late = nl;
-  out->late_key = f->ho_lkey;
-  out->late_window_id = f->ho_lwid;
-  out->late_val = f->ho_lval;
-  out->late_ts_us = f->ho_lts;
-  out->late_epoch = f->ho_lepoch;
+  out->late_key = f->ho_l.col[0];
+  out->late_window_id = (i64*)f->ho_l.col[1];
+  out->late_val = f->ho_l.col[2];
+  out->late_ts_us = (i64*)f->ho_l.col[3];
+  out->late_epoch = f->ho_l.col[4];
   return BW_OK;
 }
 
@@ -2275,7 +2227,7 @@ bw_status bw_snapshot_take(bw_fold* f, bw_snapshot* out) {
   }
   cudaStream_t s = f->s_compute;
   if (f->s_x) CU(ctx, cudaStreamSynchronize(f->s_x));
-  if (!f->d_snap_ctr) CU(ctx, dmalloc(&f->d_snap_ctr, 2));
+  if (!f->d_snap_ctr) CU(ctx, f->own.dev(&f->d_snap_ctr, 2));
   CU(ctx, cudaMemsetAsync(f->d_snap_ctr, 0, 2 * sizeof(unsigned long long), s));
   k_snap_count<<<f->close_grid, 256, 0, s>>>(f->t, f->d_snap_ctr);
   unsigned long long n = 0;
@@ -2283,11 +2235,9 @@ bw_status bw_snapshot_take(bw_fold* f, bw_snapshot* out) {
   CU(ctx, cudaMemcpyAsync(f->h_ctr, f->d_ctr, sizeof(Counters), cudaMemcpyDeviceToHost, s));
   CU(ctx, cudaStreamSynchronize(s));
   if (f->h_ctr->err) FAIL(f, (bw_status)f->h_ctr->err, "a kernel reported status %u before the snapshot", f->h_ctr->err);
-  if (f->snap_dev) { cudaFree(f->snap_dev); f->snap_dev = nullptr; }
-  if (f->snap_host) { cudaFreeHost(f->snap_host); f->snap_host = nullptr; }
   const u64 rows = n ? n : 1;
-  CU(ctx, cudaMalloc(&f->snap_dev, rows * 7 * 8));
-  CU(ctx, cudaHostAlloc(&f->snap_host, rows * 7 * 8, cudaHostAllocDefault));
+  CU(ctx, f->own.regrow(Owner::DEV, &f->snap_dev, rows * 7 * 8));
+  CU(ctx, f->own.regrow(Owner::HOST, &f->snap_host, rows * 7 * 8));
   SnapCols dc = snap_cols(f->snap_dev, rows), hc = snap_cols(f->snap_host, rows);
   if (n) {
     k_snap_fill<<<f->close_grid, 256, 0, s>>>(f->t, dc, f->d_snap_ctr + 1);
@@ -2424,8 +2374,8 @@ bw_status bw_fold_time_begin(bw_fold* f) {
   bw_ctx* ctx = f->ctx;
   CU(ctx, cudaSetDevice(ctx->device));
   if (!f->ev_t0) {
-    CU(ctx, cudaEventCreate(&f->ev_t0));
-    CU(ctx, cudaEventCreate(&f->ev_t1));
+    CU(ctx, f->own.event(&f->ev_t0, cudaEventDefault));
+    CU(ctx, f->own.event(&f->ev_t1, cudaEventDefault));
   }
   // everything submitted so far (copies, prepass) must be done before the clock starts
   {
@@ -2461,7 +2411,7 @@ bw_status bw_gen_c1(bw_fold* f, uint64_t* d_keys, uint64_t* d_vals, uint64_t sta
   CU(f->ctx, cudaSetDevice(f->ctx->device));
   k_gen_c1<<<f->ctx->sm_count * 8, 256, 0, f->s_compute>>>(d_keys, d_vals, start, rows, n_keys);
   CU(f->ctx, cudaGetLastError());
-  if (!f->ev_gen) CU(f->ctx, cudaEventCreateWithFlags(&f->ev_gen, cudaEventDisableTiming));
+  if (!f->ev_gen) CU(f->ctx, f->own.event(&f->ev_gen));
   CU(f->ctx, cudaEventRecord(f->ev_gen, f->s_compute));
   f->st.kernel_launches++;
   return BW_OK;
@@ -2483,25 +2433,20 @@ struct KeyedScratch {  // grouping of one activation by key (stable)
   size_t cub_bytes = 0;
 };
 
-static bw_status keyed_alloc(bw_ctx* ctx, KeyedScratch& k, u64 cap, cudaStream_t s) {
+static bw_status keyed_alloc(bw_ctx* ctx, Owner& own, KeyedScratch& k, u64 cap, cudaStream_t s) {
   k.cap = cap;
-  CU(ctx, dmalloc(&k.d_keys, cap));
-  CU(ctx, dmalloc(&k.d_ksorted, cap));
-  CU(ctx, dmalloc(&k.d_slot, cap));
-  CU(ctx, dmalloc(&k.d_idx, cap));
-  CU(ctx, dmalloc(&k.d_isorted, cap));
-  CU(ctx, dmalloc(&k.d_head, cap));
+  CU(ctx, own.dev(&k.d_keys, cap));
+  CU(ctx, own.dev(&k.d_ksorted, cap));
+  CU(ctx, own.dev(&k.d_slot, cap));
+  CU(ctx, own.dev(&k.d_idx, cap));
+  CU(ctx, own.dev(&k.d_isorted, cap));
+  CU(ctx, own.dev(&k.d_head, cap));
   size_t b1 = 0, b2 = 0;
   cub::DeviceRadixSort::SortPairs(nullptr, b1, k.d_keys, k.d_ksorted, k.d_idx, k.d_isorted, (int)cap, 0, 64, s);
   cub::DeviceScan::InclusiveScan(nullptr, b2, k.d_head, k.d_head, MaxU32(), (int)cap, s);
   k.cub_bytes = std::max(b1, b2) + 256;
-  CU(ctx, cudaMalloc(&k.d_cub, k.cub_bytes));
+  CU(ctx, own.dev(&k.d_cub, k.cub_bytes));
   return BW_OK;
-}
-static void keyed_free(KeyedScratch& k) {
-  void* p[] = {k.d_keys, k.d_ksorted, k.d_slot, k.d_idx, k.d_isorted, k.d_head, k.d_cub};
-  for (void* q : p)
-    if (q) cudaFree(q);
 }
 // stable group-by-key of n device keys: ksorted / isorted / head positions
 static bw_status keyed_group(bw_ctx* ctx, KeyedScratch& k, const u64* d_keys, u64 n, cudaStream_t s) {
@@ -2517,6 +2462,7 @@ static bw_status keyed_group(bw_ctx* ctx, KeyedScratch& k, const u64* d_keys, u6
 }
 
 struct bw_smap {
+  Owner own;  // every buffer and the stream below
   bw_ctx* ctx = nullptr;
   bw_smap_spec spec{};
   SmapTable t{};
@@ -2535,44 +2481,40 @@ bw_status bw_smap_create(bw_ctx* ctx, const bw_smap_spec* spec, bw_smap** out) {
   if (spec->val_dtype != BW_VAL_F32 && spec->val_dtype != BW_VAL_F64) CTX_FAIL(ctx, BW_ERR_SPEC, "val_dtype must be F32 or F64");
   if (spec->max_batch_rows == 0 || spec->max_batch_rows >= (1ULL << 31)) CTX_FAIL(ctx, BW_ERR_SPEC, "bad max_batch_rows");
   CU(ctx, cudaSetDevice(ctx->device));
-  bw_smap* m = new bw_smap();
+  std::unique_ptr<bw_smap, void (*)(bw_smap*)> mp(new bw_smap(), bw_smap_destroy);  // torn down on every failure
+  bw_smap* m = mp.get();
+  Owner& own = m->own;
   m->ctx = ctx;
   m->spec = *spec;
   u64 cap = std::max<u64>(1024, 2 * std::max<u64>(spec->capacity_hint, 1));
   m->t.cap = cap;
   m->t.window = spec->window;
-  CU(ctx, cudaStreamCreateWithFlags(&m->s, cudaStreamNonBlocking));
-  CU(ctx, dmalloc(&m->t.keys, cap + 1));
-  CU(ctx, dmalloc(&m->t.cnt, cap + 1));
-  CU(ctx, dmalloc(&m->t.ring, (cap + 1) * (u64)spec->window));
-  CU(ctx, dmalloc(&m->t.err, 1));
+  CU(ctx, own.stream(&m->s));
+  CU(ctx, own.dev(&m->t.keys, cap + 1));
+  CU(ctx, own.dev(&m->t.cnt, cap + 1));
+  CU(ctx, own.dev(&m->t.ring, (cap + 1) * (u64)spec->window));
+  CU(ctx, own.dev(&m->t.err, 1));
   CU(ctx, cudaMemsetAsync(m->t.err, 0, 4, m->s));
-  CU(ctx, cudaHostAlloc((void**)&m->h_err, 64, cudaHostAllocDefault));
+  CU(ctx, own.host(&m->h_err, 64 / sizeof(u32)));
   const u64 n = spec->max_batch_rows;
-  bw_status st = keyed_alloc(ctx, m->k, n, m->s);
+  bw_status st = keyed_alloc(ctx, own, m->k, n, m->s);
   if (st != BW_OK) return st;
-  CU(ctx, cudaMalloc(&m->d_vals, n * 8));
-  CU(ctx, dmalloc(&m->d_mu, n));
-  CU(ctx, dmalloc(&m->d_sigma, n));
-  CU(ctx, dmalloc(&m->d_flag, n));
+  CU(ctx, own.dev(&m->d_vals, n * 8));
+  CU(ctx, own.dev(&m->d_mu, n));
+  CU(ctx, own.dev(&m->d_sigma, n));
+  CU(ctx, own.dev(&m->d_flag, n));
   k_smap_init<<<ctx->sm_count * 4, 256, 0, m->s>>>(m->t);
   CU(ctx, cudaGetLastError());
   CU(ctx, cudaStreamSynchronize(m->s));
-  *out = m;
+  *out = mp.release();
   return BW_OK;
 }
 
 void bw_smap_destroy(bw_smap* m) {
   if (!m) return;
   cudaSetDevice(m->ctx->device);
-  cudaStreamSynchronize(m->s);
-  void* p[] = {m->t.keys, m->t.cnt, m->t.ring, m->t.err, m->d_vals, m->d_mu, m->d_sigma, m->d_flag};
-  for (void* q : p)
-    if (q) cudaFree(q);
-  keyed_free(m->k);
-  if (m->h_err) cudaFreeHost(m->h_err);
-  cudaStreamDestroy(m->s);
-  delete m;
+  if (m->s) cudaStreamSynchronize(m->s);
+  delete m;  // m->own releases every buffer and the stream
 }
 
 bw_status bw_smap_apply_device(bw_smap* m, const uint64_t* d_keys, const void* d_vals, uint64_t rows, double* d_mu,
@@ -2622,6 +2564,7 @@ bw_status bw_smap_apply(bw_smap* m, const uint64_t* keys, const void* vals, uint
 }
 
 struct bw_join {
+  Owner own;  // every buffer and the stream below
   bw_ctx* ctx = nullptr;
   bw_join_spec spec{};
   JoinSlot* slots = nullptr;
@@ -2633,12 +2576,8 @@ struct bw_join {
   unsigned char* d_side = nullptr;
   u64* d_vals = nullptr;
   JoinEmit e{};
-  // ordering scratch + host output
-  u64 *d_sk = nullptr, *d_sk2 = nullptr, *d_gather = nullptr;
-  u32 *d_perm = nullptr, *d_perm2 = nullptr;
-  void* d_cub = nullptr;
-  size_t cub_bytes = 0;
-  u64 *h_key = nullptr, *h_l = nullptr, *h_r = nullptr, *h_mask = nullptr, *h_epoch = nullptr;
+  SortScratch srt;  // ordering scratch
+  HostCols h;       // host output: key, left, right, mask, epoch
   u32 batch_no = 0;
   u64 min_epoch = 0, last_epoch = 0;
   bool pending = false;
@@ -2651,56 +2590,42 @@ bw_status bw_join_create(bw_ctx* ctx, const bw_join_spec* spec, bw_join** out) {
   if (spec->emit_mode < 0 || spec->emit_mode > 2) CTX_FAIL(ctx, BW_ERR_SPEC, "bad emit_mode");
   if (spec->max_batch_rows == 0 || spec->max_batch_rows >= (1ULL << 31)) CTX_FAIL(ctx, BW_ERR_SPEC, "bad max_batch_rows");
   CU(ctx, cudaSetDevice(ctx->device));
-  bw_join* j = new bw_join();
+  std::unique_ptr<bw_join, void (*)(bw_join*)> jp(new bw_join(), bw_join_destroy);  // torn down on every failure
+  bw_join* j = jp.get();
+  Owner& own = j->own;
   j->ctx = ctx;
   j->spec = *spec;
   j->cap = std::max<u64>(1024, 2 * std::max<u64>(spec->capacity_hint, 1));
-  CU(ctx, cudaStreamCreateWithFlags(&j->s, cudaStreamNonBlocking));
-  CU(ctx, dmalloc(&j->slots, j->cap + 1));
-  CU(ctx, dmalloc(&j->d_err, 1));
-  CU(ctx, dmalloc(&j->d_nrows, 1));
+  CU(ctx, own.stream(&j->s));
+  CU(ctx, own.dev(&j->slots, j->cap + 1));
+  CU(ctx, own.dev(&j->d_err, 1));
+  CU(ctx, own.dev(&j->d_nrows, 1));
   CU(ctx, cudaMemsetAsync(j->d_err, 0, 4, j->s));
   CU(ctx, cudaMemsetAsync(j->d_nrows, 0, 8, j->s));
-  CU(ctx, cudaHostAlloc((void**)&j->h_err, 64, cudaHostAllocDefault));
-  CU(ctx, cudaHostAlloc((void**)&j->h_nrows, 64, cudaHostAllocDefault));
+  CU(ctx, own.host(&j->h_err, 64 / sizeof(u32)));
+  CU(ctx, own.host(&j->h_nrows, 64 / sizeof(unsigned long long)));
   const u64 n = spec->max_batch_rows, m = std::max<u64>(spec->max_emit_rows, 1024);
-  bw_status st = keyed_alloc(ctx, j->k, n, j->s);
+  bw_status st = keyed_alloc(ctx, own, j->k, n, j->s);
   if (st != BW_OK) return st;
-  CU(ctx, dmalloc(&j->d_side, n));
-  CU(ctx, dmalloc(&j->d_vals, n));
-  u64** cols[] = {&j->e.key, &j->e.l, &j->e.r, &j->e.mask, &j->e.seq, &j->e.epoch, &j->d_sk, &j->d_sk2, &j->d_gather};
-  for (u64** c : cols) CU(ctx, dmalloc(c, m));
-  CU(ctx, dmalloc(&j->d_perm, m));
-  CU(ctx, dmalloc(&j->d_perm2, m));
+  CU(ctx, own.dev(&j->d_side, n));
+  CU(ctx, own.dev(&j->d_vals, n));
+  for (u64** c : {&j->e.key, &j->e.l, &j->e.r, &j->e.mask, &j->e.seq, &j->e.epoch}) CU(ctx, own.dev(c, m));
   j->e.max_rows = spec->max_emit_rows;
   j->e.n_rows = j->d_nrows;
-  size_t b = 0;
-  cub::DeviceRadixSort::SortPairs(nullptr, b, j->d_sk, j->d_sk2, j->d_perm, j->d_perm2, (int)m, 0, 64, j->s);
-  j->cub_bytes = b + 256;
-  CU(ctx, cudaMalloc(&j->d_cub, j->cub_bytes));
-  u64** hcols[] = {&j->h_key, &j->h_l, &j->h_r, &j->h_mask, &j->h_epoch};
-  for (u64** c : hcols) CU(ctx, cudaHostAlloc((void**)c, m * 8, cudaHostAllocDefault));
+  CU(ctx, j->srt.reserve(own, m, m, j->s));
+  CU(ctx, j->h.reserve(own, m, m));
   k_join_init<<<ctx->sm_count * 4, 256, 0, j->s>>>(j->slots, j->cap);
   CU(ctx, cudaGetLastError());
   CU(ctx, cudaStreamSynchronize(j->s));
-  *out = j;
+  *out = jp.release();
   return BW_OK;
 }
 
 void bw_join_destroy(bw_join* j) {
   if (!j) return;
   cudaSetDevice(j->ctx->device);
-  cudaStreamSynchronize(j->s);
-  void* p[] = {j->slots, j->d_err, j->d_nrows, j->d_side, j->d_vals, j->e.key, j->e.l, j->e.r, j->e.mask, j->e.seq, j->e.epoch,
-               j->d_sk, j->d_sk2, j->d_gather, j->d_perm, j->d_perm2, j->d_cub};
-  for (void* q : p)
-    if (q) cudaFree(q);
-  keyed_free(j->k);
-  void* h[] = {j->h_err, j->h_nrows, j->h_key, j->h_l, j->h_r, j->h_mask, j->h_epoch};
-  for (void* q : h)
-    if (q) cudaFreeHost(q);
-  cudaStreamDestroy(j->s);
-  delete j;
+  if (j->s) cudaStreamSynchronize(j->s);
+  delete j;  // j->own releases every buffer and the stream
 }
 
 bw_status bw_join_apply(bw_join* j, const uint64_t* keys, const uint8_t* side, const uint64_t* vals, uint64_t rows, uint64_t epoch) {
@@ -2738,25 +2663,14 @@ static bw_status join_collect(bw_join* j, bw_join_rows* out) {
   if (*j->h_err) CTX_FAIL(ctx, (bw_status)*j->h_err, "join kernel raised status %u: key table or emit buffer full", *j->h_err);
   const u64 n = std::min<u64>(*j->h_nrows, j->e.max_rows);
   if (n) {
-    const int grid = ctx->sm_count * 4;
-    k_iota<<<grid, 256, 0, s>>>(j->d_perm, n);
-    const u64 n_ord = j->last_epoch - j->min_epoch + 1;
-    int ebits = 1;
-    while ((1ULL << ebits) < n_ord + 1) ++ebits;
-    struct Pass { int kind, bits; };
-    std::vector<Pass> passes = {{BW_SK_SEQ, 64}, {BW_SK_DIGITS, 16}, {BW_SK_ALIGNED, 64}};
-    if (n_ord > 1) passes.push_back({BW_SK_EPOCH, ebits});
-    for (const Pass& ps : passes) {
-      k_sortkey<<<grid, 256, 0, s>>>(ps.kind, j->e.key, j->e.seq, j->e.epoch, nullptr, j->d_perm, j->d_sk, n, j->min_epoch);
-      size_t tb = j->cub_bytes;
-      CU(ctx, cub::DeviceRadixSort::SortPairs(j->d_cub, tb, j->d_sk, j->d_sk2, j->d_perm, j->d_perm2, (int)n, 0, ps.bits, s));
-      std::swap(j->d_perm, j->d_perm2);
-    }
+    SortScratch& x = j->srt;
+    bw_status st = order_perm(ctx, x, s, n, j->e.key, j->e.seq, j->e.epoch, nullptr, j->last_epoch - j->min_epoch + 1, j->min_epoch,
+                              nullptr);
+    if (st != BW_OK) return st;
     const u64* src[] = {j->e.key, j->e.l, j->e.r, j->e.mask, j->e.epoch};
-    u64* dst[] = {j->h_key, j->h_l, j->h_r, j->h_mask, j->h_epoch};
     for (int c = 0; c < 5; ++c) {
-      k_gather_u64<<<grid, 256, 0, s>>>(src[c], j->d_perm, j->d_gather, n);
-      CU(ctx, cudaMemcpyAsync(dst[c], j->d_gather, n * 8, cudaMemcpyDeviceToHost, s));
+      k_gather_u64<<<ctx->sm_count * 4, 256, 0, s>>>(src[c], x.perm, x.gather, n);
+      CU(ctx, cudaMemcpyAsync(j->h.col[c], x.gather, n * 8, cudaMemcpyDeviceToHost, s));
     }
     CU(ctx, cudaGetLastError());
   }
@@ -2764,11 +2678,11 @@ static bw_status join_collect(bw_join* j, bw_join_rows* out) {
   CU(ctx, cudaStreamSynchronize(s));
   j->pending = false;
   out->n = n;
-  out->key = j->h_key;
-  out->left = j->h_l;
-  out->right = j->h_r;
-  out->mask = j->h_mask;
-  out->epoch = j->h_epoch;
+  out->key = j->h.col[0];
+  out->left = j->h.col[1];
+  out->right = j->h.col[2];
+  out->mask = j->h.col[3];
+  out->epoch = j->h.col[4];
   return BW_OK;
 }
 

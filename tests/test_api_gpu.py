@@ -90,10 +90,13 @@ def test_columnar_source_feeds_the_cuda_fold():
     out = []
     flow = Dataflow("df")
     s = op.input("inp", flow, TestingSource(batches))
+    # A frozen system clock: with wait 0, the watermark would otherwise advance with the wall time between activations, and
+    # a key's next event (100 ms of event time later) would be late whenever the host took longer than that between them.
+    clock = EventClock(lambda v: None, ZERO_TD, now_getter=lambda: FROZEN)
     # already keyed columns: count_window's key_on would call key() per item, so use fold_window's plan via count on keyed input
-    wo = win.fold_window("sum", s, EventClock(lambda v: None, ZERO_TD), TumblingWindower(timedelta(seconds=10), ALIGN), lambda: 0,
+    wo = win.fold_window("sum", s, clock, TumblingWindower(timedelta(seconds=10), ALIGN), lambda: 0,
                          lambda a, _: a + 1, lambda a, b: a + b, ordered=False,
-                         _gpu_plan=win.GpuFoldPlan("count", EventClock(lambda v: None, ZERO_TD), TumblingWindower(timedelta(seconds=10), ALIGN), False, lambda v: v))
+                         _gpu_plan=win.GpuFoldPlan("count", clock, TumblingWindower(timedelta(seconds=10), ALIGN), False, lambda v: v))
     op.output("out", wo.down, TestingSink(out))
     run_main(flow, gpu=True)
     total = sum(c for _k, (_w, c) in out)
