@@ -59,8 +59,8 @@ __device__ __forceinline__ double bw_val_f64(const void* vals, int is_f32, u64 i
   return is_f32 ? (double)((const float*)vals)[i] : ((const double*)vals)[i];
 }
 
-// CPython >= 3.12 `sum()` of floats: Neumaier compensated summation (Python/bltinmodule.c); the
-// oracle runs on 3.12, so the kernel adds the same way to stay bit-identical at the z == threshold edge.
+// CPython >= 3.12 `sum()` of floats: Neumaier compensated summation (Python/bltinmodule.c); the kernel adds the
+// same way, so its sums, and so mu, are bit-identical to the reference mapper's on CPython >= 3.12.
 struct PySum {
   double s = 0.0, c = 0.0;
   __device__ __forceinline__ void add(double x) {
@@ -73,7 +73,10 @@ struct PySum {
 };
 
 // mean / population sigma of `len` values produced by get(0..len-1), newest first
-// (the order Python's sum() walks `last_10`); explicit round-to-nearest ops, no FMA contraction
+// (the order Python's sum() walks `last_10`); explicit round-to-nearest ops, no FMA contraction.
+// mu is bit-identical to CPython >= 3.12.  The square and the sqrt are correctly rounded; the reference's `** 2` and
+// `** 0.5` go through libm `pow`, which is not always, so sigma can differ from it by 1 ulp and a flag can differ
+// only where z is within a few ulp of the threshold.  `po.run_zscore(..., correctly_rounded=True)` is the exact twin.
 template <class Get>
 __device__ __forceinline__ void bw_window_stats(Get get, int len, double& mu, double& sigma) {
   PySum a;

@@ -468,6 +468,51 @@ def main_keyed():
                     emitted, _ = logics[k].on_eof()
                     rows.extend([k, t[0], t[1]] for t in emitted)
             out["join"].append(dict(insert_mode=im, emit_mode=em, items=[list(i) for i in items], rows=rows))
+
+    # edge cases, from their own generator so that the cases above stay as they are
+    rnd = random.Random(78)
+
+    def zscore_case(keys, vals):
+        states, rows = {}, []
+        for k, v in zip(keys, vals):
+            st, emit = ns["mapper"](states.get(k), v)
+            states[k] = st
+            rows.append([emit[1], emit[2], emit[3]])
+        out["zscore"].append(dict(keys=keys, vals=vals, rows=rows))
+
+    # z exactly at the threshold (not anomalous) and one ulp above it; means of exactly 0 (the flag is suppressed);
+    # constant keys (sigma 0); the sequence on which `** 2` / `** 0.5` flag and correctly rounded arithmetic does not
+    seqs = {0: [0.0, 2.0, 3.0], 1: [0.0, 2.0, 3.0000000000000004], 2: [-1.0, 1.0, 5.0, -5.0, 5.0, -1.0, 1.0, 0.0, 40.0],
+            3: [-3.0, 3.0, -3.0, 3.0, 100.0], 4: [4.0] * 12 + [9.0], 5: [-2.5] * 11 + [-2.5], 6: [0.0, -0.0, 0.0, 7.0],
+            9: list(streams.ZSCORE_FLIP)}
+    keys, vals, pos = [], [], {k: 0 for k in seqs}
+    while any(pos[k] < len(s) for k, s in seqs.items()):  # interleave the keys' sequences at random
+        k = rnd.choice([k for k, s in seqs.items() if pos[k] < len(s)])
+        keys.append(k)
+        vals.append(seqs[k][pos[k]])
+        pos[k] += 1
+    zscore_case(keys, vals)
+    keys = [rnd.randrange(5) for _ in range(500)]  # +-1e16 against O(1): the compensation decides the mean
+    zscore_case(keys, [rnd.choice((1e16, -1e16, 1.0, -1.0, 0.5, 3.0, 2.0)) for _ in keys])
+    keys = [rnd.randrange(6) for _ in range(500)]  # negative values
+    zscore_case(keys, [round(rnd.uniform(-10, 0), 3) if rnd.random() < 0.9 else -float(rnd.randrange(50)) for _ in keys])
+    # final mode over keys whose decimal text orders differently from their value: every digit-count boundary,
+    # 10^19 .. 10^19+9 (20 digits), 2^63, the largest u64 and 0; the EOF emits in key-string order
+    jkeys = [0, 9, 10, 2**63, 2**64 - 1] + [10**k - 1 for k in range(2, 20)] + [10**k for k in range(2, 20)] + [10**19 + d for d in range(10)]
+    for im in ("first", "last"):
+        items = [(k, rnd.randrange(2), rnd.randrange(2**64)) for k in jkeys for _ in range(rnd.randint(1, 3))]
+        rnd.shuffle(items)
+        logics, rows = {}, []
+        for k, sd, v in items:
+            lg = logics.get(k)
+            if lg is None:
+                lg = logics[k] = rop._JoinLogic(im, "final", rop._JoinState.for_side_count(2))
+            emitted, _ = lg.on_item((sd, v))
+            assert not emitted
+        for k in sorted(logics, key=str):
+            emitted, _ = logics[k].on_eof()
+            rows.extend([k, t[0], t[1]] for t in emitted)
+        out["join"].append(dict(insert_mode=im, emit_mode="final", items=[list(i) for i in items], rows=rows))
     path = os.path.join(os.path.dirname(HERE), "tests", "golden", "keyed_cases.json")
     with open(path, "w") as f:
         json.dump(out, f, separators=(",", ":"))

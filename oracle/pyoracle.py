@@ -32,6 +32,7 @@ unbounded, so the reference's ``OverflowError`` branches
 
 from __future__ import annotations
 
+import math
 from dataclasses import dataclass, field
 from typing import Any, Callable, Dict, Iterable, List, Optional, Sequence, Tuple
 
@@ -442,10 +443,16 @@ class ZScoreDetector:
     """Per-key state of the reference's example mapper, restated verbatim in behaviour:
     last-N values newest first, ``mu = sum/len``, ``sigma = (sum((v-mu)**2)/len) ** 0.5`` (both
     summed newest -> oldest like Python's ``sum``), anomalous iff ``mu and sigma`` are truthy and
-    ``abs(v - mu) / sigma > threshold`` evaluated BEFORE the push (anomaly_detector.py:33-46)."""
+    ``abs(v - mu) / sigma > threshold`` evaluated BEFORE the push (anomaly_detector.py:33-46).
 
-    def __init__(self, window: int = 10, threshold: float = 2.0):
+    ``correctly_rounded=True`` is the exact twin of the device's arithmetic (``bw_window_stats`` in
+    csrc/bw_keyed.cuh): the square is ``d * d`` and the root ``math.sqrt``, both correctly rounded, where the
+    reference's ``** 2`` / ``** 0.5`` go through libm ``pow``, which may be off by one ulp.  The builtin ``sum``
+    stays: on CPython >= 3.12 it is Neumaier-compensated, as the device's ``PySum`` is."""
+
+    def __init__(self, window: int = 10, threshold: float = 2.0, correctly_rounded: bool = False):
         self.window, self.threshold = window, threshold
+        self.correctly_rounded = correctly_rounded
         self.last: List[float] = []
         self.mu: Optional[float] = None
         self.sigma: Optional[float] = None
@@ -458,12 +465,16 @@ class ZScoreDetector:
         del self.last[self.window:]
         n = len(self.last)
         self.mu = sum(self.last) / n
-        self.sigma = (sum((v - self.mu) ** 2 for v in self.last) / n) ** 0.5
+        if self.correctly_rounded:
+            self.sigma = math.sqrt(sum((v - self.mu) * (v - self.mu) for v in self.last) / n)
+        else:
+            self.sigma = (sum((v - self.mu) ** 2 for v in self.last) / n) ** 0.5
         return (value, self.mu, self.sigma, anomalous)
 
 
-def run_zscore(batches, window: int = 10, threshold: float = 2.0):
-    """``batches`` = [(keys, vals), ...] -> per batch a list of (mu, sigma, anomalous) aligned with the input rows."""
+def run_zscore(batches, window: int = 10, threshold: float = 2.0, correctly_rounded: bool = False):
+    """``batches`` = [(keys, vals), ...] -> per batch a list of (mu, sigma, anomalous) aligned with the input rows.
+    ``correctly_rounded`` selects the device's arithmetic (see ``ZScoreDetector``)."""
     states: Dict[int, ZScoreDetector] = {}
     out = []
     for keys, vals in batches:
@@ -471,7 +482,7 @@ def run_zscore(batches, window: int = 10, threshold: float = 2.0):
         for k, v in zip(keys, vals):
             st = states.get(int(k))
             if st is None:
-                st = states[int(k)] = ZScoreDetector(window, threshold)
+                st = states[int(k)] = ZScoreDetector(window, threshold, correctly_rounded)
             _, mu, sigma, flag = st.on_value(float(v))
             rows.append((mu, sigma, flag))
         out.append(rows)

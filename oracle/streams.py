@@ -3,7 +3,9 @@ ONLY; needs nothing outside the repository (oracle/gen_golden.py, which runs the
 
 import hashlib
 import json
+import math
 import random
+import struct
 
 ALIGN_US = 1_640_995_200_000_000  # 2022-01-01T00:00:00Z
 
@@ -73,6 +75,39 @@ def snapshot_case(red, length, offset, wait):
         t += 5 * S
         batches.append((keys, ts, [rnd.randint(-20, 20) for _ in range(n)]))
     return spec, batches, 6
+
+
+# One key's values, in arrival order, on which the reference's z-score mapper (libm `pow` for `** 2` / `** 0.5`) flags the
+# last value anomalous and correctly rounded squares and root do not: its z is 2.0000000000000004 against 2.0.
+ZSCORE_FLIP = [8.549, 8.125, 1.7, 2.166, 9.289, 3.565, 7.15, 1.678, 5.861, 5.305, 10.891529188426174]
+
+ZSCORE_FAMILIES = ("int", "dec3", "wide", "mix1e16", "subnormal", "zeros")
+
+
+def zscore_value(family, rnd, f32=False):
+    """One value of a z-score input family drawn from `rnd`.  Every family keeps |v - mu| below 1e154, where CPython's
+    `float ** 2` would raise OverflowError; with `f32` the values are exact in float32 (finite, and subnormal there)."""
+    if family == "int":
+        return float(rnd.randint(0, 9))
+    if family == "dec3":
+        return round(rnd.uniform(0, 10), 3)
+    if family == "wide":
+        hi = 38 if f32 else 150
+        lo = -44 if f32 else -300
+        v = rnd.choice((-1.0, 1.0)) * 10.0 ** rnd.uniform(lo, hi)
+        return float(struct.unpack("f", struct.pack("f", v))[0]) if f32 else v
+    if family == "mix1e16":
+        return rnd.choice((1e16, -1e16, 1.0, -1.0, 0.5, 3.0, 2.0))
+    if family == "subnormal":
+        return rnd.choice((-1.0, 1.0)) * rnd.randrange(1 << (23 if f32 else 52)) * (2.0**-149 if f32 else 2.0**-1074)
+    if family == "zeros":
+        return rnd.choice((0.0, -0.0, 0.0, -0.0, 1.0, -1.0))
+    if family == "nonfinite":
+        u = rnd.random()
+        if u < 0.04:
+            return rnd.choice((math.inf, -math.inf, math.nan))
+        return round(rnd.uniform(-10, 10), 3)
+    raise ValueError(family)
 
 
 def key_items(batches, key):

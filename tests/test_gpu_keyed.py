@@ -36,18 +36,25 @@ def test_zscore_map_matches_oracle(ctx, dtype):
         vals = vals + np.array([po.splitmix64(0xAB ^ i) % 1000 for i in range(n * nb)]) / 1000.0
     m = gpu.ZScoreMap(ctx, 10, 2.0, dtype, capacity_hint=1024, max_batch_rows=1 << 14)
     batches = [(keys[b * n:(b + 1) * n], vals[b * n:(b + 1) * n]) for b in range(nb)]
-    want = po.run_zscore([(k.tolist(), v.astype(np.float64).tolist()) for k, v in batches])
+    lists = [(k.tolist(), v.astype(np.float64).tolist()) for k, v in batches]
+    want = po.run_zscore(lists)
+    twin = po.run_zscore(lists, correctly_rounded=True)  # the device's arithmetic: bit for bit
     near_threshold = 0
-    for (k, v), w in zip(batches, want):
+    for (k, v), w, t in zip(batches, want, twin):
         mu, sigma, flag = m.apply(k, v)
+        tm, ts, tf = (np.array([r[i] for r in t]) for i in range(3))
+        assert np.array_equal(mu.view(np.uint64), tm.view(np.uint64))
+        assert np.array_equal(sigma.view(np.uint64), ts.view(np.uint64))
+        assert np.array_equal(flag, tf)
+        # the reference's own arithmetic: the same means, sigma within one ulp (libm pow), the same flags here
         wm = np.array([r[0] for r in w])
         ws = np.array([r[1] for r in w])
         wf = np.array([r[2] for r in w])
-        np.testing.assert_allclose(mu, wm, rtol=1e-6, atol=0)   # north-star tolerance for float folds
-        np.testing.assert_allclose(sigma, ws, rtol=1e-6, atol=1e-12)
+        assert np.array_equal(mu.view(np.uint64), wm.view(np.uint64))
+        assert (np.abs(sigma - ws) <= np.spacing(sigma)).all()
         diff = np.nonzero(flag != wf)[0]
         near_threshold += len(diff)
-    assert near_threshold == 0  # integer-valued inputs: no |z - 2| < 1e-6 ties in this set
+    assert near_threshold == 0  # no z within a few ulp of 2 in this set
     m.close()
 
 
@@ -62,9 +69,11 @@ def test_zscore_single_hot_key_and_sentinel_key(ctx):
         mu, sigma, flag = m.apply(keys[lo:lo + 4096], vals[lo:lo + 4096])
         got += list(zip(mu.tolist(), sigma.tolist(), flag.tolist()))
     want = po.run_zscore([(keys.tolist(), vals.astype(np.float64).tolist())])[0]
-    assert [g[2] for g in got] == [w[2] for w in want]
-    np.testing.assert_allclose([g[0] for g in got], [w[0] for w in want], rtol=1e-6)
-    np.testing.assert_allclose([g[1] for g in got], [w[1] for w in want], rtol=1e-6, atol=1e-12)
+    twin = po.run_zscore([(keys.tolist(), vals.astype(np.float64).tolist())], correctly_rounded=True)[0]
+    assert [g[2] for g in got] == [w[2] for w in want] == [t[2] for t in twin]
+    assert np.array_equal(np.array([g[0] for g in got]).view(np.uint64), np.array([t[0] for t in twin]).view(np.uint64))
+    assert np.array_equal(np.array([g[1] for g in got]).view(np.uint64), np.array([t[1] for t in twin]).view(np.uint64))
+    assert [g[0] for g in got] == [w[0] for w in want]
     m.close()
 
 
