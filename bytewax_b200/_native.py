@@ -90,6 +90,21 @@ class BwJoinRows(C.Structure):
                 ("mask", C.POINTER(C.c_uint64)), ("epoch", C.POINTER(C.c_uint64))]
 
 
+class BwSessionSpec(C.Structure):
+    _fields_ = [("struct_size", C.c_uint32), ("reduction", C.c_int32), ("val_dtype", C.c_int32), ("max_sessions_per_key", C.c_int32),
+                ("gap_us", C.c_int64), ("wait_us", C.c_int64), ("capacity_hint", C.c_uint64), ("max_batch_rows", C.c_uint64),
+                ("max_emit_rows", C.c_uint64), ("max_late_rows", C.c_uint64)]
+
+
+class BwSessionRows(C.Structure):
+    _fields_ = [("n_closed", C.c_uint64), ("closed_key", C.POINTER(C.c_uint64)), ("closed_window_id", C.POINTER(C.c_int64)),
+                ("closed_acc", C.POINTER(C.c_uint64)), ("closed_open_us", C.POINTER(C.c_int64)),
+                ("closed_close_us", C.POINTER(C.c_int64)), ("closed_epoch", C.POINTER(C.c_uint64)),
+                ("merged_off", C.POINTER(C.c_uint64)), ("merged_ids", C.POINTER(C.c_int64)),
+                ("n_late", C.c_uint64), ("late_key", C.POINTER(C.c_uint64)), ("late_epoch", C.POINTER(C.c_uint64)),
+                ("late_activation", C.POINTER(C.c_uint64)), ("late_row", C.POINTER(C.c_uint64))]
+
+
 # every symbol include/bwgpu.h declares: (restype, argtypes)
 _P = C.c_void_p
 SYMBOLS = {
@@ -131,6 +146,12 @@ SYMBOLS = {
     "bw_join_apply": (C.c_int32, [_P, _P, _P, _P, C.c_uint64, C.c_uint64]),
     "bw_join_advance": (C.c_int32, [_P, C.POINTER(BwJoinRows)]),
     "bw_join_eof": (C.c_int32, [_P, C.POINTER(BwJoinRows)]),
+    "bw_session_create": (C.c_int32, [_P, C.POINTER(BwSessionSpec), C.POINTER(_P)]),
+    "bw_session_destroy": (None, [_P]),
+    "bw_session_apply": (C.c_int32, [_P, _P, _P, _P, C.c_uint64, C.c_uint64, C.c_int64]),
+    "bw_session_apply_device": (C.c_int32, [_P, _P, _P, _P, C.c_uint64, C.c_uint64, C.c_int64]),
+    "bw_session_advance": (C.c_int32, [_P, C.c_int64, C.POINTER(BwSessionRows)]),
+    "bw_session_eof": (C.c_int32, [_P, C.POINTER(BwSessionRows)]),
     "bw_dev_alloc": (C.c_int32, [_P, C.c_uint64, C.POINTER(_P)]),
     "bw_dev_free": (C.c_int32, [_P, _P]),
     "bw_host_alloc": (C.c_int32, [_P, C.c_uint64, C.POINTER(_P)]),

@@ -34,6 +34,7 @@
 #include "bw_snapshot.cuh"
 #include "bw_fold.cuh"
 #include "bw_keyed.cuh"
+#include "bw_session.cuh"
 #include "bw_prepass.cuh"
 #include "bw_slow.cuh"
 #include "bw_late.cuh"
@@ -2703,4 +2704,257 @@ bw_status bw_join_eof(bw_join* j, bw_join_rows* out) {
   k_join_eof<<<ctx->sm_count * 8, 256, 0, j->s>>>(j->slots, j->cap, j->d_err, j->spec.emit_mode, j->e, j->last_epoch);
   CU(ctx, cudaGetLastError());
   return join_collect(j, out);
+}
+
+// ===========================================================================
+// K7 host side: session-window folds (bw_session.cuh)
+// ===========================================================================
+struct bw_session {
+  Owner own;  // every buffer and the stream below
+  bw_ctx* ctx = nullptr;
+  bw_session_spec spec{};
+  SessTable t{};
+  KeyedScratch k;
+  cudaStream_t s = nullptr;
+  u32* h_err = nullptr;                    // err, why
+  unsigned long long* d_cnt = nullptr;     // closed rows, merged ids, late rows
+  unsigned long long* h_cnt = nullptr;
+  u64* d_vals = nullptr;
+  i64* d_ts = nullptr;
+  SessEmit e{};
+  SortScratch srt;  // ordering scratch
+  HostCols hc[2];   // closed: key, window id, acc, open, close | epoch, merged count, merged offset
+  HostCols hl;      // late: key, epoch, activation, row
+  i64* h_mids = nullptr;
+  std::vector<u64> merged_off;
+  std::vector<i64> merged_ids;
+  u32 batch_no = 0;
+  u64 calls = 0, first_call = 0;  // calls (activations, notify phases, EOF) so far; the first not yet collected
+  u64 last_epoch = 0;
+  i64 now = INT64_MIN;
+  bool failed = false;
+};
+
+bw_status bw_session_create(bw_ctx* ctx, const bw_session_spec* spec, bw_session** out) {
+  if (!ctx || !spec || !out) CTX_FAIL(ctx, BW_ERR_SPEC, "bw_session_create: NULL argument");
+  if (spec->struct_size != sizeof(bw_session_spec)) CTX_FAIL(ctx, BW_ERR_SPEC, "bw_session_spec.struct_size mismatch");
+  if (ctx->world != 1) CTX_FAIL(ctx, BW_ERR_SPEC, "session folds run on one GPU (world == 1)");
+  if (spec->reduction < BW_RED_COUNT || spec->reduction > BW_RED_MAX) CTX_FAIL(ctx, BW_ERR_SPEC, "reduction must be count, sum, min or max");
+  if (spec->val_dtype != BW_VAL_I64 && spec->val_dtype != BW_VAL_F64) CTX_FAIL(ctx, BW_ERR_SPEC, "val_dtype must be I64 or F64");
+  if (spec->gap_us < 0 || spec->gap_us > BW_UTC_MAX_US - BW_UTC_MIN_US) CTX_FAIL(ctx, BW_ERR_SPEC, "gap_us must be in 0..UTC_MAX - UTC_MIN");
+  if (spec->wait_us < 0) CTX_FAIL(ctx, BW_ERR_SPEC, "wait_us must not be negative");
+  if (spec->max_sessions_per_key < 1 || spec->max_sessions_per_key > BW_SESS_MAXM)
+    CTX_FAIL(ctx, BW_ERR_SPEC, "max_sessions_per_key must be in 1..%d", BW_SESS_MAXM);
+  if (spec->max_batch_rows == 0 || spec->max_batch_rows >= (1ULL << 31)) CTX_FAIL(ctx, BW_ERR_SPEC, "bad max_batch_rows");
+  CU(ctx, cudaSetDevice(ctx->device));
+  std::unique_ptr<bw_session, void (*)(bw_session*)> sp(new bw_session(), bw_session_destroy);  // torn down on every failure
+  bw_session* f = sp.get();
+  Owner& own = f->own;
+  f->ctx = ctx;
+  f->spec = *spec;
+  const u64 cap = std::max<u64>(1024, 2 * std::max<u64>(spec->capacity_hint, 1));
+  const int M = spec->max_sessions_per_key;
+  SessTable& t = f->t;
+  t.cap = cap;
+  t.M = M;
+  CU(ctx, own.stream(&f->s));
+  CU(ctx, own.dev(&t.keys, cap + 1));
+  CU(ctx, own.dev(&t.st, cap + 1));
+  CU(ctx, own.dev(&t.rec, (cap + 1) * (u64)M));
+  CU(ctx, own.dev(&t.mrg, (cap + 1) * (u64)(2 * M)));
+  CU(ctx, own.dev(&t.err, 2));
+  t.why = t.err + 1;
+  CU(ctx, own.dev(&f->d_cnt, 3));
+  CU(ctx, cudaMemsetAsync(t.err, 0, 8, f->s));
+  CU(ctx, cudaMemsetAsync(f->d_cnt, 0, 24, f->s));
+  CU(ctx, own.host(&f->h_err, 64 / sizeof(u32)));
+  CU(ctx, own.host(&f->h_cnt, 64 / sizeof(unsigned long long)));
+  const u64 n = spec->max_batch_rows, m = std::max<u64>(spec->max_emit_rows, 1), l = std::max<u64>(spec->max_late_rows, 1);
+  bw_status st = keyed_alloc(ctx, own, f->k, n, f->s);
+  if (st != BW_OK) return st;
+  CU(ctx, own.dev(&f->d_vals, n));
+  CU(ctx, own.dev(&f->d_ts, n));
+  SessEmit& e = f->e;
+  for (u64** c : {&e.key, &e.acc, &e.epoch, &e.ord, &e.moff, &e.mcnt}) CU(ctx, own.dev(c, m));
+  for (i64** c : {&e.wid, &e.open, &e.close, &e.mids}) CU(ctx, own.dev(c, m));
+  for (u64** c : {&e.l_key, &e.l_epoch, &e.l_ord, &e.l_act, &e.l_row}) CU(ctx, own.dev(c, l));
+  e.max_rows = spec->max_emit_rows;
+  e.max_late = spec->max_late_rows;
+  e.n_rows = f->d_cnt;
+  e.n_mids = f->d_cnt + 1;
+  e.n_late = f->d_cnt + 2;
+  CU(ctx, f->srt.reserve(own, std::max(m, l), std::max(m, l), f->s));
+  CU(ctx, f->hc[0].reserve(own, m, m));
+  CU(ctx, f->hc[1].reserve(own, m, m));
+  CU(ctx, f->hl.reserve(own, l, l));
+  CU(ctx, own.host(&f->h_mids, m));
+  k_session_init<<<ctx->sm_count * 4, 256, 0, f->s>>>(t);
+  CU(ctx, cudaGetLastError());
+  CU(ctx, cudaStreamSynchronize(f->s));
+  *out = sp.release();
+  return BW_OK;
+}
+
+void bw_session_destroy(bw_session* f) {
+  if (!f) return;
+  cudaSetDevice(f->ctx->device);
+  if (f->s) cudaStreamSynchronize(f->s);
+  delete f;  // f->own releases every buffer and the stream
+}
+
+static SessParams session_params(bw_session* f, u64 epoch) {
+  SessParams p;
+  p.red = f->spec.reduction;
+  p.is_f64 = f->spec.val_dtype == BW_VAL_F64;
+  p.gap = f->spec.gap_us;
+  p.wait = f->spec.wait_us;
+  p.now = f->now;
+  p.epoch = epoch;
+  p.ord = f->calls++;
+  p.batch_no = f->batch_no;
+  return p;
+}
+
+// `now_getter()` of the call: never goes backwards (windowing.py:250-261)
+static void session_now(bw_session* f, int64_t system_now_us) {
+  if (system_now_us > f->now) f->now = system_now_us;
+}
+
+static bw_status session_check(bw_session* f) {
+  bw_ctx* ctx = f->ctx;
+  if (f->failed) CTX_FAIL(ctx, BW_ERR_STATE, "session fold: an earlier call ran out of capacity; the fold is unusable");
+  CU(ctx, cudaMemcpyAsync(f->h_err, f->t.err, 8, cudaMemcpyDeviceToHost, f->s));
+  CU(ctx, cudaStreamSynchronize(f->s));
+  if (f->h_err[0]) {
+    f->failed = true;
+    const u32 w = f->h_err[1];
+    CTX_FAIL(ctx, (bw_status)f->h_err[0], "session kernel ran out of capacity:%s%s%s%s%s", w & BW_SESS_FULL_TABLE ? " key table full (raise capacity_hint);" : "",
+             w & BW_SESS_FULL_SESSIONS ? " a key needs more than max_sessions_per_key sessions or merged ids;" : "",
+             w & BW_SESS_FULL_EMIT ? " more than max_emit_rows closed sessions or merged ids since the last advance;" : "",
+             w & BW_SESS_FULL_LATE ? " more than max_late_rows late rows since the last advance;" : "", w ? "" : " (no reason recorded)");
+  }
+  return BW_OK;
+}
+
+bw_status bw_session_apply_device(bw_session* f, const uint64_t* d_keys, const void* d_vals, const int64_t* d_ts_us, uint64_t rows,
+                                  uint64_t epoch, int64_t system_now_us) {
+  if (!f) return BW_ERR_SPEC;
+  bw_ctx* ctx = f->ctx;
+  if (f->failed) CTX_FAIL(ctx, BW_ERR_STATE, "session fold: an earlier call ran out of capacity; the fold is unusable");
+  if (rows > f->spec.max_batch_rows) CTX_FAIL(ctx, BW_ERR_SPEC, "session: rows > max_batch_rows");
+  if (rows && (!d_keys || !d_ts_us || (!d_vals && f->spec.reduction != BW_RED_COUNT))) CTX_FAIL(ctx, BW_ERR_SPEC, "session: NULL column");
+  if (f->batch_no && epoch < f->last_epoch) CTX_FAIL(ctx, BW_ERR_STATE, "session: epochs must not decrease");
+  f->last_epoch = epoch;
+  session_now(f, system_now_us);
+  CU(ctx, cudaSetDevice(ctx->device));
+  const SessParams p = session_params(f, epoch);
+  f->batch_no++;
+  if (rows == 0) return BW_OK;
+  bw_status st = keyed_group(ctx, f->k, d_keys, rows, f->s);
+  if (st != BW_OK) return st;
+  k_session_apply<<<ctx->sm_count * 8, 256, 0, f->s>>>(f->t, f->e, p, f->k.d_ksorted, f->k.d_isorted, f->k.d_head, (const u64*)d_vals,
+                                                       d_ts_us, rows);
+  CU(ctx, cudaGetLastError());
+  return BW_OK;
+}
+
+bw_status bw_session_apply(bw_session* f, const uint64_t* keys, const void* vals, const int64_t* ts_us, uint64_t rows, uint64_t epoch,
+                           int64_t system_now_us) {
+  if (!f) return BW_ERR_SPEC;
+  bw_ctx* ctx = f->ctx;
+  if (rows > f->spec.max_batch_rows) CTX_FAIL(ctx, BW_ERR_SPEC, "session: rows > max_batch_rows");
+  CU(ctx, cudaSetDevice(ctx->device));
+  const bool has_vals = vals != nullptr;
+  if (rows) {
+    CU(ctx, cudaMemcpyAsync(f->k.d_keys, keys, rows * 8, cudaMemcpyHostToDevice, f->s));
+    CU(ctx, cudaMemcpyAsync(f->d_ts, ts_us, rows * 8, cudaMemcpyHostToDevice, f->s));
+    if (has_vals) CU(ctx, cudaMemcpyAsync(f->d_vals, vals, rows * 8, cudaMemcpyHostToDevice, f->s));
+  }
+  bw_status st = bw_session_apply_device(f, f->k.d_keys, has_vals ? f->d_vals : nullptr, f->d_ts, rows, epoch, system_now_us);
+  if (st != BW_OK) return st;
+  // the host columns may be reused by the caller once this returns
+  return session_check(f);
+}
+
+static bw_status session_collect(bw_session* f, bw_session_rows* out) {
+  bw_ctx* ctx = f->ctx;
+  cudaStream_t s = f->s;
+  bw_status st = session_check(f);
+  if (st != BW_OK) return st;
+  CU(ctx, cudaMemcpyAsync(f->h_cnt, f->d_cnt, 24, cudaMemcpyDeviceToHost, s));
+  CU(ctx, cudaStreamSynchronize(s));
+  const u64 nc = f->h_cnt[0], nmid = f->h_cnt[1], nl = f->h_cnt[2];  // all within bounds: session_check passed
+  const u64 n_ord = std::max<u64>(f->calls - f->first_call, 1);
+  const int grid = ctx->sm_count * 4;
+  SortScratch& x = f->srt;
+  const SessEmit& e = f->e;
+  if (nc) {  // per call, key string, then session id (the id column doubles as the sequence)
+    st = order_perm(ctx, x, s, nc, e.key, (const u64*)e.wid, e.ord, nullptr, n_ord, f->first_call, nullptr);
+    if (st != BW_OK) return st;
+    const u64* src[] = {e.key, (const u64*)e.wid, e.acc, (const u64*)e.open, (const u64*)e.close, e.epoch, e.mcnt, e.moff};
+    for (int c = 0; c < 8; ++c) {
+      k_gather_u64<<<grid, 256, 0, s>>>(src[c], x.perm, x.gather, nc);
+      CU(ctx, cudaMemcpyAsync(f->hc[c / 5].col[c % 5], x.gather, nc * 8, cudaMemcpyDeviceToHost, s));
+    }
+    if (nmid) CU(ctx, cudaMemcpyAsync(f->h_mids, e.mids, nmid * 8, cudaMemcpyDeviceToHost, s));
+  }
+  if (nl) {  // per call, key string, then arrival order
+    st = order_perm(ctx, x, s, nl, e.l_key, e.l_row, e.l_ord, nullptr, n_ord, f->first_call, nullptr);
+    if (st != BW_OK) return st;
+    const u64* src[] = {e.l_key, e.l_epoch, e.l_act, e.l_row};
+    for (int c = 0; c < 4; ++c) {
+      k_gather_u64<<<grid, 256, 0, s>>>(src[c], x.perm, x.gather, nl);
+      CU(ctx, cudaMemcpyAsync(f->hl.col[c], x.gather, nl * 8, cudaMemcpyDeviceToHost, s));
+    }
+  }
+  CU(ctx, cudaGetLastError());
+  CU(ctx, cudaMemsetAsync(f->d_cnt, 0, 24, s));
+  CU(ctx, cudaStreamSynchronize(s));
+  // merged ids in row order
+  f->merged_off.assign(nc + 1, 0);
+  f->merged_ids.resize(nmid);
+  const u64 *cnt = f->hc[1].col[1], *off = f->hc[1].col[2];
+  for (u64 r = 0; r < nc; ++r) {
+    f->merged_off[r + 1] = f->merged_off[r] + cnt[r];
+    std::copy(f->h_mids + off[r], f->h_mids + off[r] + cnt[r], f->merged_ids.begin() + f->merged_off[r]);
+  }
+  f->first_call = f->calls;
+  out->n_closed = nc;
+  out->closed_key = f->hc[0].col[0];
+  out->closed_window_id = (const int64_t*)f->hc[0].col[1];
+  out->closed_acc = f->hc[0].col[2];
+  out->closed_open_us = (const int64_t*)f->hc[0].col[3];
+  out->closed_close_us = (const int64_t*)f->hc[0].col[4];
+  out->closed_epoch = f->hc[1].col[0];
+  out->merged_off = f->merged_off.data();
+  out->merged_ids = f->merged_ids.data();
+  out->n_late = nl;
+  out->late_key = f->hl.col[0];
+  out->late_epoch = f->hl.col[1];
+  out->late_activation = f->hl.col[2];
+  out->late_row = f->hl.col[3];
+  return BW_OK;
+}
+
+bw_status bw_session_advance(bw_session* f, int64_t system_now_us, bw_session_rows* out) {
+  if (!f || !out) return BW_ERR_SPEC;
+  bw_ctx* ctx = f->ctx;
+  if (f->failed) CTX_FAIL(ctx, BW_ERR_STATE, "session fold: an earlier call ran out of capacity; the fold is unusable");
+  CU(ctx, cudaSetDevice(ctx->device));
+  if (system_now_us > 0) {
+    session_now(f, system_now_us);
+    k_session_close_all<<<ctx->sm_count * 8, 256, 0, f->s>>>(f->t, f->e, session_params(f, f->last_epoch), 0);
+    CU(ctx, cudaGetLastError());
+  }
+  return session_collect(f, out);
+}
+
+bw_status bw_session_eof(bw_session* f, bw_session_rows* out) {
+  if (!f || !out) return BW_ERR_SPEC;
+  bw_ctx* ctx = f->ctx;
+  if (f->failed) CTX_FAIL(ctx, BW_ERR_STATE, "session fold: an earlier call ran out of capacity; the fold is unusable");
+  CU(ctx, cudaSetDevice(ctx->device));
+  k_session_close_all<<<ctx->sm_count * 8, 256, 0, f->s>>>(f->t, f->e, session_params(f, f->last_epoch), 1);
+  CU(ctx, cudaGetLastError());
+  return session_collect(f, out);
 }

@@ -269,9 +269,107 @@ class _NoClock:
         return []
 
 
+class _GpuSessionStep(_GpuWindowStep):
+    """One worker's ``stateful_batch`` of a numeric fold over a ``SessionWindower`` (``GpuFoldPlan``) on ``bw_session_*``
+    (K7): `_WindowLogic` over `_SessionWindowerLogic` (windowing.py:671-810, 1046-1190), one call per activation.  Late
+    rows name their input row, so they carry the original item value; ``M`` rows carry the merged session ids."""
+
+    def __init__(self, step_id: str, plan):
+        import numpy as np
+
+        self.np, self.plan, self.step_id = np, plan, step_id
+        wait = getattr(plan.clock, "wait_for_system_duration", timedelta(0))  # (SystemClock: stamped with the system time, wait 0)
+        self.wait_us = None if wait >= timedelta(days=365 * 200) else _td_us(wait)
+        self.gap_us = _td_us(plan.windower.gap)
+        self.key_ids: Dict[str, int] = {}
+        self.id_keys: Dict[int, str] = {}
+        self.resort = False
+        self.last_epoch = 0
+        self.sess = None
+
+    def on_epoch(self, epoch: int, items: list) -> list:
+        from bytewax_b200 import gpu
+
+        np, plan = self.np, self.plan
+        getter = getattr(plan.clock, "ts_getter", None)
+        now = self._now_us()
+        if getter is None:  # SystemClock (windowing.py:196-222): an item's timestamp is the system time of its batch
+            now_dt = _dt(now)
+            getter = lambda _v: now_dt  # noqa: E731
+        keys, ts, vals, orig = [], [], [], []
+        for item in items:
+            key, value = _split_item(self.step_id, item)
+            keys.append(self._key_id(key))
+            ts.append(_us(getter(value)))
+            orig.append(value)
+            if plan.reduction != "count":
+                num = plan.value_of(value)
+                if isinstance(num, bool) or not isinstance(num, (int, float)) or (isinstance(num, int) and not -(1 << 63) <= num < (1 << 63)):
+                    if self.sess is None:  # nothing folded yet: this step runs on the host logic instead
+                        raise _GpuPlanUnfit(f"value {num!r} of type {type(num)!r}")
+                    raise TypeError(f"step {self.step_id!r}: the CUDA session fold needs numeric values in the int64 / float64 range; got {num!r}")
+                vals.append(num)
+        v = None
+        if plan.reduction != "count":
+            v = np.array(vals)
+            if self.sess is not None and v.dtype.kind == "f" and self.sess.val_dtype != "f64":
+                raise TypeError(f"step {self.step_id!r}: value type changed from integer to float mid-stream")
+        if self.sess is None:
+            self.sess = gpu.SessionFold(
+                _get_gpu_ctx(), plan.reduction, self.gap_us, self.wait_us, val_dtype="f64" if v is not None and v.dtype.kind == "f" else "i64",
+                capacity_hint=int(os.environ.get("BYTEWAX_B200_KEYS", 1 << 20)), max_batch_rows=int(os.environ.get("BYTEWAX_B200_BATCH", 1 << 22)),
+                max_emit_rows=1 << 22, max_late_rows=1 << 22, max_sessions_per_key=int(os.environ.get("BYTEWAX_B200_SESSIONS", 64)))
+        self.last_epoch = max(epoch, self.last_epoch)
+        self.sess.apply(np.array(keys, dtype=np.uint64), v, np.array(ts, dtype=np.int64), self.last_epoch, now or 0)
+        return self._session_rows(self.sess.advance(), orig)
+
+    def on_notify(self) -> list:
+        if self.sess is None:
+            return []
+        now = self._now_us()
+        if now is None or now <= 0:
+            return []
+        return self._session_rows(self.sess.advance(system_now_us=now), [])
+
+    def on_eof(self) -> list:
+        if self.sess is None:
+            return []
+        out = self._session_rows(self.sess.eof(), [])
+        self.release()
+        return out
+
+    def release(self):
+        if self.sess is not None:
+            self.sess.close()
+            self.sess = None
+
+    def _session_rows(self, out, orig) -> list:
+        from bytewax_b200.operators.windowing import WindowMetadata
+
+        lates = [(self._key_str(k), orig[r]) for k, r in zip(out.late_key.tolist(), out.late_row.tolist())]
+        closed = [(self._key_str(k), i) for i, k in enumerate(out.closed_key.tolist())]
+        if self.resort:  # interned (non-numeric) keys: restore ascending key-string order; stable
+            lates.sort(key=lambda r: r[0])
+            closed.sort(key=lambda r: r[0])
+        rows = [(ks, (-1, "L", val)) for ks, val in lates]
+        wid, acc = out.closed_window_id.tolist(), out.closed_acc.tolist()
+        o, c = out.closed_open_us.tolist(), out.closed_close_us.tolist()
+        for ks, i in closed:
+            rows.append((ks, (wid[i], "E", acc[i])))
+            rows.append((ks, (wid[i], "M", WindowMetadata(_dt(o[i]), _dt(c[i]), set(out.merged(i))))))
+        return rows
+
+
+def _td_us(td: timedelta) -> int:
+    return (td.days * 86400 + td.seconds) * 1_000_000 + td.microseconds
+
+
 def _gpu_step_for(step_id: str, plan):
     from bytewax_b200.operators import GpuFinalPlan, GpuJoinPlan, GpuSmapPlan
+    from bytewax_b200.operators.windowing import SessionWindower
 
+    if isinstance(getattr(plan, "windower", None), SessionWindower):
+        return _GpuSessionStep(step_id, plan)
     if isinstance(plan, GpuSmapPlan):
         return _GpuSmapStep(step_id, plan)
     if isinstance(plan, GpuJoinPlan):

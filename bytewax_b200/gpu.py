@@ -410,3 +410,110 @@ class KeyedJoin:
         if self.h:
             self.lib.bw_join_destroy(self.h)
             self.h = None
+
+
+@dataclass
+class SessionRows:
+    """Rows of one ``SessionFold.advance`` / ``eof`` in the reference's downstream order."""
+
+    closed_key: np.ndarray
+    closed_window_id: np.ndarray
+    closed_acc: np.ndarray  # uint64 (count), int64 or float64
+    closed_open_us: np.ndarray
+    closed_close_us: np.ndarray
+    closed_epoch: np.ndarray
+    merged_off: np.ndarray  # [n_closed + 1] into merged_ids
+    merged_ids: np.ndarray
+    late_key: np.ndarray
+    late_epoch: np.ndarray
+    late_activation: np.ndarray
+    late_row: np.ndarray
+
+    def merged(self, i: int) -> List[int]:
+        return self.merged_ids[self.merged_off[i] : self.merged_off[i + 1]].tolist()
+
+    def rows(self) -> list:
+        """``[key, window_id, tag, payload]`` rows like the reference's window events: per closed session ``E`` (the
+        accumulator) then ``M`` (``[open_us, close_us, merged ids]``); late rows (``L``, window -1) carry the input
+        position ``(activation, row)`` as payload."""
+        out = []
+        for i, (k, w, a, o, c) in enumerate(zip(self.closed_key.tolist(), self.closed_window_id.tolist(), self.closed_acc.tolist(),
+                                               self.closed_open_us.tolist(), self.closed_close_us.tolist())):
+            out.append([k, w, "E", a])
+            out.append([k, w, "M", [o, c, self.merged(i)]])
+        out.extend([k, -1, "L", (a, r)] for k, a, r in zip(self.late_key.tolist(), self.late_activation.tolist(), self.late_row.tolist()))
+        return out
+
+
+class SessionFold:
+    """Session-window count / sum / min / max by key (``bw_session``, K7; windowing.py:671-810, 1046-1190)."""
+
+    def __init__(self, ctx: Context, reduction: str = "count", gap_us: int = 10_000_000, wait_us: Optional[int] = 0,
+                 val_dtype: str = "i64", capacity_hint: int = 1 << 16, max_batch_rows: int = 1 << 20, max_emit_rows: int = 1 << 20,
+                 max_late_rows: int = 1 << 20, max_sessions_per_key: int = 16):
+        """``wait_us=None``: the watermark never advances on data (``BW_WAIT_FOREVER``)."""
+        self.ctx, self.lib = ctx, ctx.lib
+        self.reduction, self.val_dtype = reduction, val_dtype
+        s = N.BwSessionSpec()
+        s.struct_size = C.sizeof(N.BwSessionSpec)
+        s.reduction, s.val_dtype = N.RED[reduction], N.VAL[val_dtype]
+        s.gap_us, s.wait_us = gap_us, N.BW_WAIT_FOREVER if wait_us is None else wait_us
+        s.capacity_hint, s.max_batch_rows, s.max_emit_rows, s.max_late_rows = capacity_hint, max_batch_rows, max_emit_rows, max_late_rows
+        s.max_sessions_per_key = max_sessions_per_key
+        self.spec = s
+        h = C.c_void_p()
+        N.check(self.lib.bw_session_create(ctx.h, C.byref(s), C.byref(h)), ctx.h)
+        self.h = h
+        self._epoch = 0
+
+    def apply(self, keys, vals, ts_us, epoch: Optional[int] = None, system_now_us: int = 0):
+        """One activation from host arrays (``vals`` may be None for count).  ``system_now_us``: ``now_getter()``."""
+        keys = np.ascontiguousarray(keys, dtype=np.uint64)
+        ts = np.ascontiguousarray(ts_us, dtype=np.int64)
+        v = None if vals is None else np.ascontiguousarray(vals, dtype=_NP_VAL[self.val_dtype])
+        if epoch is None:
+            self._epoch += 1
+            epoch = self._epoch
+        vp = lambda a: a.ctypes.data_as(C.c_void_p)  # noqa: E731
+        N.check(self.lib.bw_session_apply(self.h, vp(keys), None if v is None else vp(v), vp(ts), keys.shape[0], epoch,
+                                          int(system_now_us)), self.ctx.h)
+
+    def apply_device(self, d_keys: int, d_vals: Optional[int], d_ts: int, rows: int, epoch: Optional[int] = None, system_now_us: int = 0):
+        if epoch is None:
+            self._epoch += 1
+            epoch = self._epoch
+        N.check(self.lib.bw_session_apply_device(self.h, C.c_void_p(d_keys), C.c_void_p(d_vals or 0), C.c_void_p(d_ts), rows, epoch,
+                                                 int(system_now_us)), self.ctx.h)
+
+    def _wrap(self, r: N.BwSessionRows) -> SessionRows:
+        nc, nl = int(r.n_closed), int(r.n_late)
+
+        def arr(ptr, n, dt):
+            return np.ctypeslib.as_array(ptr, shape=(n,)).view(dt).copy() if n else np.zeros(0, dt)
+
+        if self.reduction == "count":
+            acc_dt = np.uint64
+        else:
+            acc_dt = np.float64 if self.val_dtype == "f64" else np.int64
+        off = arr(r.merged_off, nc + 1, np.uint64).astype(np.int64)
+        return SessionRows(arr(r.closed_key, nc, np.uint64), arr(r.closed_window_id, nc, np.int64), arr(r.closed_acc, nc, acc_dt),
+                           arr(r.closed_open_us, nc, np.int64), arr(r.closed_close_us, nc, np.int64), arr(r.closed_epoch, nc, np.uint64),
+                           off, arr(r.merged_ids, int(off[-1]), np.int64),
+                           arr(r.late_key, nl, np.uint64), arr(r.late_epoch, nl, np.uint64), arr(r.late_activation, nl, np.uint64),
+                           arr(r.late_row, nl, np.uint64))
+
+    def advance(self, system_now_us: int = 0) -> SessionRows:
+        """Rows since the last call; ``system_now_us`` > 0 first runs the notify phase at that system time."""
+        r = N.BwSessionRows()
+        N.check(self.lib.bw_session_advance(self.h, int(system_now_us), C.byref(r)), self.ctx.h)
+        return self._wrap(r)
+
+    def eof(self) -> SessionRows:
+        r = N.BwSessionRows()
+        N.check(self.lib.bw_session_eof(self.h, C.byref(r)), self.ctx.h)
+        return self._wrap(r)
+
+    def close(self):
+        if self.h:
+            self.lib.bw_session_destroy(self.h)
+            self.h = None

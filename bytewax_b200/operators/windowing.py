@@ -620,6 +620,11 @@ def _plan_for(reduction: str, clock, windower, ordered, value_of=_identity) -> O
     # (SystemClock == an event clock whose timestamps are the arrival times, wait 0: every item is at the watermark)
     if isinstance(clock, (EventClock, SystemClock)) and isinstance(windower, (SlidingWindower, TumblingWindower)):
         return GpuFoldPlan(reduction, clock, windower, ordered, value_of)
+    # session windows (K7): unordered only, and an identity `to_system_utc` (the device's notify phase compares event
+    # time with the system clock directly, windowing.py:1177-1178)
+    if isinstance(windower, SessionWindower) and not ordered and (
+            isinstance(clock, SystemClock) or (isinstance(clock, EventClock) and clock.to_system_utc is _identity)):
+        return GpuFoldPlan(reduction, clock, windower, ordered, value_of)
     return None
 
 

@@ -371,6 +371,74 @@ bw_status bw_join_apply(bw_join* j, const uint64_t* keys, const uint8_t* side, c
 bw_status bw_join_advance(bw_join* j, bw_join_rows* out);
 bw_status bw_join_eof(bw_join* j, bw_join_rows* out);
 
+/* Session-window fold (K7): `_WindowLogic` (unordered) over `_SessionWindowerLogic` with a numeric fold,
+ * pysrc/bytewax/operators/windowing.py:1046-1190 and :671-810, built by `SessionWindower` :928-950.  Per key, in
+ * arrival order: the EventClock's late test (:263-287, :1125-1127; a late item gives one row with window id
+ * LATE_SESSION_ID = -1, :671, :764-766); `open_for` (:731-762): the FIRST live session by id that contains the
+ * timestamp, or whose open is 0 < open - ts <= gap ahead (open := ts), or whose close is 0 < ts - close <= gap
+ * behind (close := ts), else a new session with id max_key + 1 (max_key starts at -1 and never resets: session
+ * state is never discarded, :798-806); after an extension `_session_find_merges` (:688-715) merges, in open order,
+ * every session that opens within gap of the running survivor's close into the EARLIEST-OPENED one, which gains the
+ * merged id (direct merges only).  Then the activation's inserts are folded (:1064-1077) into the accumulator of the
+ * id `open_for` returned, then the merge queue in discovery order (`into = merger(into, orig)`, :1079-1085), then
+ * `close_for` (:774-788): sessions with close < watermark - gap (UTC_MIN if that is below it), in id order.
+ * Accumulators: count_window :1679-1689; reduce_window(operator.add) :2268-2285 (i64 sums wrap past 2^63);
+ * max_window / min_window :2189 / :2236 with `by` = identity (the accumulator is replaced only if the new value is
+ * strictly greater / less, so signed zeros and NaN come out exactly as in Python).  One GPU only. */
+typedef struct bw_session bw_session;
+typedef struct bw_session_spec {
+  uint32_t struct_size;
+  int32_t reduction;            /* BW_RED_COUNT / SUM / MIN / MAX */
+  int32_t val_dtype;            /* BW_VAL_I64 or BW_VAL_F64 (values are ignored by count) */
+  int32_t max_sessions_per_key; /* 1..64: sessions a key holds during an activation (live ones, plus those merged away
+                                   in it, which keep their accumulator until the activation's merge pass), and also the
+                                   merged ids its live sessions hold */
+  int64_t gap_us;               /* SessionWindower.gap, >= 0 (windowing.py:938-943) */
+  int64_t wait_us;              /* EventClock.wait_for_system_duration, or BW_WAIT_FOREVER */
+  uint64_t capacity_hint;       /* keys ever seen: session state is never freed (windowing.py:798-806) */
+  uint64_t max_batch_rows;
+  uint64_t max_emit_rows;       /* closed sessions, and their merged ids, retained between bw_session_advance calls */
+  uint64_t max_late_rows;       /* late rows retained between bw_session_advance calls */
+} bw_session_spec;
+/* Rows handed downstream since the last advance / eof, in the reference's order: per call (activation, notify phase
+ * or EOF), ascending key string (src/operators.rs:758-767, :862-894); within a key late rows in arrival order and
+ * closed sessions in id order.  Host pointers into memory owned by the library, valid until the next advance / eof /
+ * destroy. */
+typedef struct bw_session_rows {
+  /* `down` + `meta` streams: one row per closed session, WindowMetadata(open, close, merged_ids) (:1087-1093) */
+  uint64_t n_closed;
+  const uint64_t* closed_key;
+  const int64_t* closed_window_id;
+  const uint64_t* closed_acc;     /* count: u64; sum / min / max: i64 or f64 bits */
+  const int64_t* closed_open_us;
+  const int64_t* closed_close_us;
+  const uint64_t* closed_epoch;   /* the epoch of the activation, or of the last one before a notify / EOF */
+  const uint64_t* merged_off;     /* [n_closed + 1]: row i merged ids are merged_ids[merged_off[i] .. merged_off[i+1]) */
+  const int64_t* merged_ids;      /* ascending per row */
+  /* `late` stream: one row per late item; (activation, row) name the input row (activations counted from 0) */
+  uint64_t n_late;
+  const uint64_t* late_key;
+  const uint64_t* late_epoch;
+  const uint64_t* late_activation;
+  const uint64_t* late_row;
+} bw_session_rows;
+bw_status bw_session_create(bw_ctx* ctx, const bw_session_spec* spec, bw_session** out);
+void bw_session_destroy(bw_session* s);
+/* One activation from HOST columns (vals may be NULL for count); blocks.  `system_now_us` is `now_getter()` for this
+ * activation (windowing.py:250-261; it must not go backwards; 0 throughout = a frozen clock).  The key's watermark is
+ * then max_j(ts_j - wait - now_j) + now, as bw_fold_set_system_now describes. */
+bw_status bw_session_apply(bw_session* s, const uint64_t* keys, const void* vals, const int64_t* ts_us, uint64_t rows,
+                           uint64_t epoch, int64_t system_now_us);
+/* Same with DEVICE columns; returns once the work is enqueued (the columns must stay valid until the next call). */
+bw_status bw_session_apply_device(bw_session* s, const uint64_t* d_keys, const void* d_vals, const int64_t* d_ts_us,
+                                  uint64_t rows, uint64_t epoch, int64_t system_now_us);
+/* Rows since the last call.  `system_now_us` > 0 first runs the notify phase at that system time
+ * (src/operators.rs:808-858, windowing.py:1135-1142, 1153-1180 with an identity `to_system_utc`): every key with a
+ * live session whose earliest close + gap has been reached closes what its watermark at that time allows. */
+bw_status bw_session_advance(bw_session* s, int64_t system_now_us, bw_session_rows* out);
+/* End of input: watermark := UTC_MAX (:300-302), so sessions with close >= UTC_MAX - gap stay open. */
+bw_status bw_session_eof(bw_session* s, bw_session_rows* out);
+
 /* ---- plain device-memory helpers (tests / bench / host bindings without torch) ---- */
 bw_status bw_dev_alloc(bw_ctx* ctx, uint64_t bytes, void** out);
 bw_status bw_dev_free(bw_ctx* ctx, void* ptr);
