@@ -105,6 +105,23 @@ class BwSessionRows(C.Structure):
                 ("late_activation", C.POINTER(C.c_uint64)), ("late_row", C.POINTER(C.c_uint64))]
 
 
+class BwJwinSpec(C.Structure):
+    _fields_ = [("struct_size", C.c_uint32), ("insert_mode", C.c_int32), ("emit_mode", C.c_int32), ("ordered", C.c_int32),
+                ("sides", C.c_int32), ("max_windows_per_key", C.c_int32), ("length_us", C.c_int64), ("offset_us", C.c_int64),
+                ("align_us", C.c_int64), ("wait_us", C.c_int64), ("capacity_hint", C.c_uint64), ("max_queued_rows", C.c_uint64),
+                ("max_batch_rows", C.c_uint64), ("max_emit_rows", C.c_uint64), ("max_late_rows", C.c_uint64)]
+
+
+class BwJwinRows(C.Structure):
+    _fields_ = [("n_down", C.c_uint64), ("down_key", C.POINTER(C.c_uint64)), ("down_window_id", C.POINTER(C.c_int64)),
+                ("down_handle", C.POINTER(C.c_uint64) * 4), ("down_mask", C.POINTER(C.c_uint64)), ("down_epoch", C.POINTER(C.c_uint64)),
+                ("n_meta", C.c_uint64), ("meta_key", C.POINTER(C.c_uint64)), ("meta_window_id", C.POINTER(C.c_int64)),
+                ("meta_epoch", C.POINTER(C.c_uint64)),
+                ("n_late", C.c_uint64), ("late_key", C.POINTER(C.c_uint64)), ("late_window_id", C.POINTER(C.c_int64)),
+                ("late_epoch", C.POINTER(C.c_uint64)), ("late_activation", C.POINTER(C.c_uint64)), ("late_row", C.POINTER(C.c_uint64)),
+                ("n_released", C.c_uint64), ("released", C.POINTER(C.c_uint64))]
+
+
 # every symbol include/bwgpu.h declares: (restype, argtypes)
 _P = C.c_void_p
 SYMBOLS = {
@@ -152,6 +169,12 @@ SYMBOLS = {
     "bw_session_apply_device": (C.c_int32, [_P, _P, _P, _P, C.c_uint64, C.c_uint64, C.c_int64]),
     "bw_session_advance": (C.c_int32, [_P, C.c_int64, C.POINTER(BwSessionRows)]),
     "bw_session_eof": (C.c_int32, [_P, C.POINTER(BwSessionRows)]),
+    "bw_jwin_create": (C.c_int32, [_P, C.POINTER(BwJwinSpec), C.POINTER(_P)]),
+    "bw_jwin_destroy": (None, [_P]),
+    "bw_jwin_apply": (C.c_int32, [_P, _P, _P, _P, _P, C.c_uint64, C.c_uint64, C.c_int64]),
+    "bw_jwin_apply_device": (C.c_int32, [_P, _P, _P, _P, _P, C.c_uint64, C.c_uint64, C.c_int64]),
+    "bw_jwin_advance": (C.c_int32, [_P, C.c_int64, C.POINTER(BwJwinRows)]),
+    "bw_jwin_eof": (C.c_int32, [_P, C.POINTER(BwJwinRows)]),
     "bw_dev_alloc": (C.c_int32, [_P, C.c_uint64, C.POINTER(_P)]),
     "bw_dev_free": (C.c_int32, [_P, _P]),
     "bw_host_alloc": (C.c_int32, [_P, C.c_uint64, C.POINTER(_P)]),

@@ -35,6 +35,7 @@
 #include "bw_fold.cuh"
 #include "bw_keyed.cuh"
 #include "bw_session.cuh"
+#include "bw_jwin.cuh"
 #include "bw_prepass.cuh"
 #include "bw_slow.cuh"
 #include "bw_late.cuh"
@@ -2957,4 +2958,373 @@ bw_status bw_session_eof(bw_session* f, bw_session_rows* out) {
   k_session_close_all<<<ctx->sm_count * 8, 256, 0, f->s>>>(f->t, f->e, session_params(f, f->last_epoch), 1);
   CU(ctx, cudaGetLastError());
   return session_collect(f, out);
+}
+
+// ===========================================================================
+// K8 host side: windowed join (bw_jwin.cuh)
+// ===========================================================================
+struct bw_jwin {
+  Owner own;  // every buffer and the stream below
+  bw_ctx* ctx = nullptr;
+  bw_jwin_spec spec{};
+  JwTable t{};
+  KeyedScratch k;
+  cudaStream_t s = nullptr;
+  u32* h_err = nullptr;                 // err, why
+  unsigned long long* d_cnt = nullptr;  // down, meta, late, released, carried-over queue entries
+  unsigned long long* h_cnt = nullptr;
+  unsigned char *d_side = nullptr, *d_late = nullptr;
+  u64* d_handles = nullptr;
+  i64* d_ts = nullptr;
+  JwEmit e{};
+  JwPool pool{}, pool2{};  // ordered mode: the queue, and the one the next flush writes
+  u64 nq = 0;              // entries in `pool`
+  int slot_bits = 1;
+  SortScratch srt;       // pool sort and ordering scratch
+  HostCols hd[2];        // down: key, window id, h0, h1, h2 | h3, mask, epoch
+  HostCols hm, hl;       // meta: key, window id, epoch; late: key, window id, epoch, activation, row
+  std::vector<u64> released;      // since the last advance / eof
+  std::vector<u64> released_out;  // what the last advance / eof handed out
+  bool undrained = false;     // a call whose released handles and queue count are not read back yet
+  u64 outstanding = 0;        // handles passed in and not released yet: what the next call can release, besides its own
+  u32 batch_no = 0;
+  u64 calls = 0, first_call = 0;  // calls (activations, notify phases, EOF) so far; the first not yet collected
+  u64 last_epoch = 0;
+  i64 now = INT64_MIN;
+  bool failed = false;
+};
+
+static bw_status jwin_pool_alloc(bw_ctx* ctx, Owner& own, JwPool& p, u64 n) {
+  CU(ctx, own.dev(&p.slot, n));
+  CU(ctx, own.dev(&p.ts, n));
+  CU(ctx, own.dev(&p.h, n));
+  CU(ctx, own.dev(&p.side, n));
+  return BW_OK;
+}
+
+bw_status bw_jwin_create(bw_ctx* ctx, const bw_jwin_spec* spec, bw_jwin** out) {
+  if (!ctx || !spec || !out) CTX_FAIL(ctx, BW_ERR_SPEC, "bw_jwin_create: NULL argument");
+  if (spec->struct_size != sizeof(bw_jwin_spec)) CTX_FAIL(ctx, BW_ERR_SPEC, "bw_jwin_spec.struct_size mismatch");
+  if (ctx->world != 1) CTX_FAIL(ctx, BW_ERR_SPEC, "windowed joins run on one GPU (world == 1)");
+  if (spec->insert_mode != BW_JOIN_INSERT_FIRST && spec->insert_mode != BW_JOIN_INSERT_LAST)
+    CTX_FAIL(ctx, BW_ERR_SPEC, "insert_mode must be first or last (product: host engine)");
+  if (spec->emit_mode < BW_JOIN_EMIT_COMPLETE || spec->emit_mode > BW_JOIN_EMIT_RUNNING) CTX_FAIL(ctx, BW_ERR_SPEC, "bad emit_mode");
+  if (spec->ordered != 0 && spec->ordered != 1) CTX_FAIL(ctx, BW_ERR_SPEC, "ordered must be 0 or 1");
+  if (spec->sides < 1 || spec->sides > BW_JW_MAXSIDES) CTX_FAIL(ctx, BW_ERR_SPEC, "sides must be in 1..%d", BW_JW_MAXSIDES);
+  if (spec->max_windows_per_key < 1 || spec->max_windows_per_key > BW_JW_MAXM)
+    CTX_FAIL(ctx, BW_ERR_SPEC, "max_windows_per_key must be in 1..%d", BW_JW_MAXM);
+  if (spec->length_us <= 0 || spec->length_us > BW_UTC_MAX_US - BW_UTC_MIN_US) CTX_FAIL(ctx, BW_ERR_SPEC, "length_us must be in 1..UTC_MAX - UTC_MIN");
+  if (spec->offset_us <= 0 || spec->offset_us > spec->length_us) CTX_FAIL(ctx, BW_ERR_SPEC, "offset_us must be in 1..length_us");
+  if (spec->align_us < BW_UTC_MIN_US || spec->align_us > BW_UTC_MAX_US) CTX_FAIL(ctx, BW_ERR_SPEC, "align_us out of range");
+  if (spec->wait_us < 0) CTX_FAIL(ctx, BW_ERR_SPEC, "wait_us must not be negative");
+  if (spec->max_batch_rows == 0 || spec->max_batch_rows >= (1ULL << 31)) CTX_FAIL(ctx, BW_ERR_SPEC, "bad max_batch_rows");
+  if (spec->max_queued_rows >= (1ULL << 31) - spec->max_batch_rows) CTX_FAIL(ctx, BW_ERR_SPEC, "max_queued_rows + max_batch_rows must stay below 2^31");
+  if (spec->capacity_hint >= (1ULL << 30)) CTX_FAIL(ctx, BW_ERR_SPEC, "capacity_hint must be below 2^30");
+  CU(ctx, cudaSetDevice(ctx->device));
+  std::unique_ptr<bw_jwin, void (*)(bw_jwin*)> jp(new bw_jwin(), bw_jwin_destroy);  // torn down on every failure
+  bw_jwin* j = jp.get();
+  Owner& own = j->own;
+  j->ctx = ctx;
+  j->spec = *spec;
+  const u64 cap = std::max<u64>(1024, 2 * std::max<u64>(spec->capacity_hint, 1));
+  const int M = spec->max_windows_per_key;
+  JwTable& t = j->t;
+  t.cap = cap;
+  t.M = M;
+  t.sides = spec->sides;
+  while ((1ULL << j->slot_bits) < cap + 1) ++j->slot_bits;
+  CU(ctx, own.stream(&j->s));
+  CU(ctx, own.dev(&t.keys, cap + 1));
+  CU(ctx, own.dev(&t.st, cap + 1));
+  CU(ctx, own.dev(&t.win, (cap + 1) * (u64)M));
+  CU(ctx, own.dev(&t.err, 2));
+  t.why = t.err + 1;
+  CU(ctx, own.dev(&j->d_cnt, 5));
+  CU(ctx, cudaMemsetAsync(t.err, 0, 8, j->s));
+  CU(ctx, cudaMemsetAsync(j->d_cnt, 0, 40, j->s));
+  CU(ctx, own.host(&j->h_err, 64 / sizeof(u32)));
+  CU(ctx, own.host(&j->h_cnt, 64 / sizeof(unsigned long long)));
+  const u64 n = spec->max_batch_rows, m = std::max<u64>(spec->max_emit_rows, 1), l = std::max<u64>(spec->max_late_rows, 1);
+  const u64 q = spec->ordered ? spec->max_queued_rows : 0;
+  bw_status st = keyed_alloc(ctx, own, j->k, n, j->s);
+  if (st != BW_OK) return st;
+  CU(ctx, own.dev(&j->d_side, n));
+  CU(ctx, own.dev(&j->d_late, n));
+  CU(ctx, own.dev(&j->d_handles, n));
+  CU(ctx, own.dev(&j->d_ts, n));
+  if (spec->ordered) {
+    if ((st = jwin_pool_alloc(ctx, own, j->pool, q + n)) != BW_OK) return st;
+    if ((st = jwin_pool_alloc(ctx, own, j->pool2, q + n)) != BW_OK) return st;
+  }
+  JwEmit& e = j->e;
+  for (u64** c : {&e.key, &e.wid, &e.h0, &e.h1, &e.h2, &e.h3, &e.mask, &e.epoch, &e.ord, &e.seq}) CU(ctx, own.dev(c, m));
+  for (u64** c : {&e.m_key, &e.m_wid, &e.m_epoch, &e.m_ord, &e.m_seq}) CU(ctx, own.dev(c, m));
+  for (u64** c : {&e.l_key, &e.l_wid, &e.l_epoch, &e.l_act, &e.l_row, &e.l_ord, &e.l_seq}) CU(ctx, own.dev(c, l));
+  // the release buffer grows with the handles held (jwin_room); it starts at one batch
+  e.max_rel = n;
+  CU(ctx, own.dev(&e.rel, e.max_rel));
+  e.max_rows = spec->max_emit_rows;
+  e.max_late = spec->max_late_rows;
+  e.max_queue = q;
+  e.n_rows = j->d_cnt;
+  e.n_meta = j->d_cnt + 1;
+  e.n_late = j->d_cnt + 2;
+  e.n_rel = j->d_cnt + 3;
+  e.n_next = j->d_cnt + 4;
+  const u64 ns = std::max(std::max(m, l), q + n);
+  CU(ctx, j->srt.reserve(own, ns, ns, j->s));
+  CU(ctx, j->hd[0].reserve(own, m, m));
+  CU(ctx, j->hd[1].reserve(own, m, m));
+  CU(ctx, j->hm.reserve(own, m, m));
+  CU(ctx, j->hl.reserve(own, l, l));
+  k_jwin_init<<<ctx->sm_count * 4, 256, 0, j->s>>>(t);
+  CU(ctx, cudaGetLastError());
+  CU(ctx, cudaStreamSynchronize(j->s));
+  *out = jp.release();
+  return BW_OK;
+}
+
+void bw_jwin_destroy(bw_jwin* j) {
+  if (!j) return;
+  cudaSetDevice(j->ctx->device);
+  if (j->s) cudaStreamSynchronize(j->s);
+  delete j;  // j->own releases every buffer and the stream
+}
+
+static JwParams jwin_params(bw_jwin* j, u64 epoch) {
+  JwParams p;
+  p.insert_last = j->spec.insert_mode == BW_JOIN_INSERT_LAST;
+  p.emit_mode = j->spec.emit_mode;
+  p.ordered = j->spec.ordered;
+  p.length = j->spec.length_us;
+  p.offset = j->spec.offset_us;
+  p.align = j->spec.align_us;
+  p.wait = j->spec.wait_us;
+  p.now = j->now;
+  p.epoch = epoch;
+  p.ord = j->calls++;
+  p.batch_no = j->batch_no;
+  return p;
+}
+
+#define JWIN_REFUSE_FAILED(j) \
+  if ((j)->failed) CTX_FAIL((j)->ctx, BW_ERR_STATE, "windowed join: an earlier call failed on the device; the join is unusable")
+
+// wait for the last call; fail on a device-side overflow; then take its released handles and its queue count, so the
+// device buffer only ever holds one call's releases
+static bw_status jwin_drain(bw_jwin* j) {
+  bw_ctx* ctx = j->ctx;
+  JWIN_REFUSE_FAILED(j);
+  if (!j->undrained) return BW_OK;
+  CU(ctx, cudaMemcpyAsync(j->h_err, j->t.err, 8, cudaMemcpyDeviceToHost, j->s));
+  CU(ctx, cudaMemcpyAsync(j->h_cnt, j->d_cnt, 40, cudaMemcpyDeviceToHost, j->s));
+  CU(ctx, cudaStreamSynchronize(j->s));
+  if (j->h_err[0]) {
+    j->failed = true;
+    const u32 w = j->h_err[1];
+    CTX_FAIL(ctx, (bw_status)j->h_err[0], "windowed join kernel %s:%s%s%s%s%s%s%s",
+             j->h_err[0] == BW_ERR_SPEC ? "rejected its input" : "ran out of capacity",
+             w & BW_JW_BAD_SIDE ? " a side column value is not below sides;" : "", w & BW_JW_FULL_TABLE ? " key table full (raise capacity_hint);" : "",
+             w & BW_JW_FULL_WINDOWS ? " a key needs more than max_windows_per_key open windows;" : "",
+             w & BW_JW_FULL_EMIT ? " more than max_emit_rows down or meta rows since the last advance;" : "",
+             w & BW_JW_FULL_LATE ? " more than max_late_rows late rows since the last advance;" : "",
+             w & BW_JW_FULL_QUEUE ? " more than max_queued_rows queued entries;" : "", w ? "" : " (no reason recorded)");
+  }
+  const u64 nr = j->h_cnt[3];
+  j->outstanding -= std::min(nr, j->outstanding);
+  if (nr) {
+    const size_t at = j->released.size();
+    j->released.resize(at + nr);
+    CU(ctx, cudaMemcpyAsync(j->released.data() + at, j->e.rel, nr * 8, cudaMemcpyDeviceToHost, j->s));
+  }
+  if (j->spec.ordered) j->nq = j->h_cnt[4];
+  CU(ctx, cudaMemsetAsync(j->d_cnt + 3, 0, 16, j->s));
+  CU(ctx, cudaStreamSynchronize(j->s));
+  j->undrained = false;
+  return BW_OK;
+}
+
+// Room in the release buffer for the next call: it can release at most the handles passed in earlier and not released
+// yet, plus its own `rows`.  Called after jwin_drain, so nothing on the stream reads the old buffer and it holds no
+// releases; the buffer then holds what the join actually holds, not what its tables could hold.
+static bw_status jwin_room(bw_jwin* j, u64 rows) {
+  const u64 need = j->outstanding + rows;
+  if (need <= j->e.max_rel) return BW_OK;
+  const u64 grow = std::max<u64>(need, 2 * j->e.max_rel);
+  j->e.max_rel = 0;  // (a failed regrow leaves no buffer: the next call tries again)
+  CU(j->ctx, j->own.regrow(Owner::DEV, &j->e.rel, grow));
+  j->e.max_rel = grow;
+  return BW_OK;
+}
+
+// ordered mode: sort the pool's due entries into play order, then flush every woken key (k_jwin_flush)
+static bw_status jwin_flush_pool(bw_jwin* j, const JwParams& p, u64 n) {
+  bw_ctx* ctx = j->ctx;
+  const int grid = ctx->sm_count * 4;
+  SortScratch& x = j->srt;
+  if (n) {
+    k_jwin_sortkey<<<grid, 256, 0, j->s>>>(j->t, p, j->pool, x.sk, x.perm, n);
+    size_t tb = x.cub_bytes;
+    CU(ctx, cub::DeviceRadixSort::SortPairs(x.cub, tb, x.sk, x.sk2, x.perm, x.perm2, (int)n, 0, 64, j->s));
+    k_jwin_slotkey<<<grid, 256, 0, j->s>>>(j->pool, x.perm2, x.sk, n);
+    tb = x.cub_bytes;
+    CU(ctx, cub::DeviceRadixSort::SortPairs(x.cub, tb, x.sk, x.sk2, x.perm2, x.perm, (int)n, 0, j->slot_bits, j->s));
+    k_jwin_ranges<<<grid, 256, 0, j->s>>>(j->t, p, j->pool, x.perm, n);
+  }
+  JwEmit e = j->e;
+  e.next = j->pool2;
+  k_jwin_flush<<<ctx->sm_count * 8, 256, 0, j->s>>>(j->t, e, p, j->pool, x.perm);
+  CU(ctx, cudaGetLastError());
+  std::swap(j->pool, j->pool2);  // the next call reads what this flush carried over (count: jwin_drain)
+  return BW_OK;
+}
+
+bw_status bw_jwin_apply_device(bw_jwin* j, const uint64_t* d_keys, const uint8_t* d_side, const uint64_t* d_handles, const int64_t* d_ts_us,
+                               uint64_t rows, uint64_t epoch, int64_t system_now_us) {
+  if (!j) return BW_ERR_SPEC;
+  bw_ctx* ctx = j->ctx;
+  JWIN_REFUSE_FAILED(j);
+  if (rows > j->spec.max_batch_rows) CTX_FAIL(ctx, BW_ERR_SPEC, "windowed join: rows > max_batch_rows");
+  if (rows && (!d_keys || !d_side || !d_handles || !d_ts_us)) CTX_FAIL(ctx, BW_ERR_SPEC, "windowed join: NULL column");
+  if (j->batch_no && epoch < j->last_epoch) CTX_FAIL(ctx, BW_ERR_STATE, "windowed join: epochs must not decrease");
+  CU(ctx, cudaSetDevice(ctx->device));
+  bw_status st = jwin_drain(j);
+  if (st != BW_OK) return st;
+  j->last_epoch = epoch;
+  if (system_now_us > j->now) j->now = system_now_us;  // `now_getter()` never goes backwards (windowing.py:250-261)
+  const JwParams p = jwin_params(j, epoch);
+  j->batch_no++;
+  if (rows == 0) return BW_OK;
+  if ((st = jwin_room(j, rows)) != BW_OK) return st;
+  j->outstanding += rows;
+  st = keyed_group(ctx, j->k, d_keys, rows, j->s);
+  if (st != BW_OK) return st;
+  k_jwin_apply<<<ctx->sm_count * 8, 256, 0, j->s>>>(j->t, j->e, p, j->pool, j->nq, j->k.d_ksorted, j->k.d_isorted, j->k.d_head, d_handles,
+                                                    d_side, d_ts_us, j->d_late, rows);
+  CU(ctx, cudaGetLastError());
+  j->undrained = true;
+  if (j->spec.ordered) return jwin_flush_pool(j, p, j->nq + rows);
+  return BW_OK;
+}
+
+bw_status bw_jwin_apply(bw_jwin* j, const uint64_t* keys, const uint8_t* side, const uint64_t* handles, const int64_t* ts_us, uint64_t rows,
+                        uint64_t epoch, int64_t system_now_us) {
+  if (!j) return BW_ERR_SPEC;
+  bw_ctx* ctx = j->ctx;
+  if (rows > j->spec.max_batch_rows) CTX_FAIL(ctx, BW_ERR_SPEC, "windowed join: rows > max_batch_rows");
+  if (rows && (!keys || !side || !handles || !ts_us)) CTX_FAIL(ctx, BW_ERR_SPEC, "windowed join: NULL column");
+  for (u64 i = 0; i < rows; ++i)
+    if (side[i] >= (u32)j->spec.sides) CTX_FAIL(ctx, BW_ERR_SPEC, "windowed join: side %u of row %llu is not below sides", side[i], (unsigned long long)i);
+  CU(ctx, cudaSetDevice(ctx->device));
+  bw_status st = jwin_drain(j);
+  if (st != BW_OK) return st;
+  if (rows) {
+    CU(ctx, cudaMemcpyAsync(j->k.d_keys, keys, rows * 8, cudaMemcpyHostToDevice, j->s));
+    CU(ctx, cudaMemcpyAsync(j->d_side, side, rows, cudaMemcpyHostToDevice, j->s));
+    CU(ctx, cudaMemcpyAsync(j->d_handles, handles, rows * 8, cudaMemcpyHostToDevice, j->s));
+    CU(ctx, cudaMemcpyAsync(j->d_ts, ts_us, rows * 8, cudaMemcpyHostToDevice, j->s));
+  }
+  st = bw_jwin_apply_device(j, j->k.d_keys, j->d_side, j->d_handles, j->d_ts, rows, epoch, system_now_us);
+  if (st != BW_OK) return st;
+  // the host columns may be reused by the caller once this returns
+  return jwin_drain(j);
+}
+
+// order rows [0, n) of one stream by (call, key string, seq) and copy `nc` columns to the host
+static bw_status jwin_ship(bw_jwin* j, u64 n, const u64* key, const u64* seq, const u64* ord, const u64* const* src, int nc, HostCols* dst) {
+  if (!n) return BW_OK;
+  bw_ctx* ctx = j->ctx;
+  SortScratch& x = j->srt;
+  bw_status st = order_perm(ctx, x, j->s, n, key, seq, ord, nullptr, std::max<u64>(j->calls - j->first_call, 1), j->first_call, nullptr);
+  if (st != BW_OK) return st;
+  for (int c = 0; c < nc; ++c) {
+    k_gather_u64<<<ctx->sm_count * 4, 256, 0, j->s>>>(src[c], x.perm, x.gather, n);
+    CU(ctx, cudaMemcpyAsync(dst[c / 5].col[c % 5], x.gather, n * 8, cudaMemcpyDeviceToHost, j->s));
+  }
+  return BW_OK;
+}
+
+static bw_status jwin_collect(bw_jwin* j, bw_jwin_rows* out) {
+  bw_ctx* ctx = j->ctx;
+  bw_status st = jwin_drain(j);
+  if (st != BW_OK) return st;
+  CU(ctx, cudaMemcpyAsync(j->h_cnt, j->d_cnt, 24, cudaMemcpyDeviceToHost, j->s));
+  CU(ctx, cudaStreamSynchronize(j->s));
+  const u64 nd = j->h_cnt[0], nm = j->h_cnt[1], nl = j->h_cnt[2];  // all within bounds: jwin_drain passed
+  const JwEmit& e = j->e;
+  const u64* down[] = {e.key, e.wid, e.h0, e.h1, e.h2, e.h3, e.mask, e.epoch};
+  const u64* meta[] = {e.m_key, e.m_wid, e.m_epoch};
+  const u64* late[] = {e.l_key, e.l_wid, e.l_epoch, e.l_act, e.l_row};
+  if ((st = jwin_ship(j, nd, e.key, e.seq, e.ord, down, 8, j->hd)) != BW_OK) return st;
+  if ((st = jwin_ship(j, nm, e.m_key, e.m_seq, e.m_ord, meta, 3, &j->hm)) != BW_OK) return st;
+  if ((st = jwin_ship(j, nl, e.l_key, e.l_seq, e.l_ord, late, 5, &j->hl)) != BW_OK) return st;
+  CU(ctx, cudaGetLastError());
+  CU(ctx, cudaMemsetAsync(j->d_cnt, 0, 24, j->s));
+  CU(ctx, cudaStreamSynchronize(j->s));
+  j->first_call = j->calls;
+  out->n_down = nd;
+  out->down_key = j->hd[0].col[0];
+  out->down_window_id = (const int64_t*)j->hd[0].col[1];
+  out->down_handle[0] = j->hd[0].col[2];
+  out->down_handle[1] = j->hd[0].col[3];
+  out->down_handle[2] = j->hd[0].col[4];
+  out->down_handle[3] = j->hd[1].col[0];
+  out->down_mask = j->hd[1].col[1];
+  out->down_epoch = j->hd[1].col[2];
+  out->n_meta = nm;
+  out->meta_key = j->hm.col[0];
+  out->meta_window_id = (const int64_t*)j->hm.col[1];
+  out->meta_epoch = j->hm.col[2];
+  out->n_late = nl;
+  out->late_key = j->hl.col[0];
+  out->late_window_id = (const int64_t*)j->hl.col[1];
+  out->late_epoch = j->hl.col[2];
+  out->late_activation = j->hl.col[3];
+  out->late_row = j->hl.col[4];
+  // handed out until the next advance / eof, then cleared
+  j->released.swap(j->released_out);
+  j->released.clear();
+  out->n_released = j->released_out.size();
+  out->released = j->released_out.data();
+  return BW_OK;
+}
+
+// notify phase or EOF: wake the keys, then flush them (ordered: through the pool)
+static bw_status jwin_wake(bw_jwin* j, int eof) {
+  bw_ctx* ctx = j->ctx;
+  bw_status st = jwin_drain(j);
+  if (st != BW_OK) return st;
+  if ((st = jwin_room(j, 0)) != BW_OK) return st;
+  const JwParams p = jwin_params(j, j->last_epoch);
+  k_jwin_mark<<<ctx->sm_count * 8, 256, 0, j->s>>>(j->t, p, eof);
+  CU(ctx, cudaGetLastError());
+  j->undrained = true;
+  if (j->spec.ordered) return jwin_flush_pool(j, p, j->nq);
+  JwEmit e = j->e;
+  k_jwin_flush<<<ctx->sm_count * 8, 256, 0, j->s>>>(j->t, e, p, j->pool, nullptr);
+  CU(ctx, cudaGetLastError());
+  return BW_OK;
+}
+
+bw_status bw_jwin_advance(bw_jwin* j, int64_t system_now_us, bw_jwin_rows* out) {
+  if (!j || !out) return BW_ERR_SPEC;
+  bw_ctx* ctx = j->ctx;
+  JWIN_REFUSE_FAILED(j);
+  CU(ctx, cudaSetDevice(ctx->device));
+  if (system_now_us > 0) {
+    if (system_now_us > j->now) j->now = system_now_us;
+    bw_status st = jwin_wake(j, 0);
+    if (st != BW_OK) return st;
+  }
+  return jwin_collect(j, out);
+}
+
+bw_status bw_jwin_eof(bw_jwin* j, bw_jwin_rows* out) {
+  if (!j || !out) return BW_ERR_SPEC;
+  bw_ctx* ctx = j->ctx;
+  JWIN_REFUSE_FAILED(j);
+  CU(ctx, cudaSetDevice(ctx->device));
+  bw_status st = jwin_wake(j, 1);
+  if (st != BW_OK) return st;
+  return jwin_collect(j, out);
 }

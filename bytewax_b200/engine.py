@@ -360,14 +360,115 @@ class _GpuSessionStep(_GpuWindowStep):
         return rows
 
 
+class _GpuJoinWindowStep(_GpuWindowStep):
+    """One worker's ``join_window`` (``GpuJoinWindowPlan``) on ``bw_jwin_*`` (K8): `_WindowLogic` over a tumbling or
+    sliding windower with `_JoinWindowLogic` per window (windowing.py:1046-1190, 1849-1902), one call per activation.
+    Items are ``(key, (side, value))`` from ``_join_label_merge``; the values stay here, keyed by handle, and each is
+    dropped once the device releases its handle.  Late rows carry the labelled item, as on the host."""
+
+    def __init__(self, step_id: str, plan):
+        import numpy as np
+
+        from bytewax_b200.operators.windowing import SlidingWindower
+
+        self.np, self.plan, self.step_id = np, plan, step_id
+        w = plan.windower
+        self.length_us = _td_us(w.length)
+        self.offset_us = _td_us(w.offset) if isinstance(w, SlidingWindower) else self.length_us
+        self.align_us = _us(w.align_to)
+        wait = getattr(plan.clock, "wait_for_system_duration", timedelta(0))  # (SystemClock: stamped with the system time, wait 0)
+        self.wait_us = None if wait >= timedelta(days=365 * 200) else _td_us(wait)
+        self.key_ids: Dict[str, int] = {}
+        self.id_keys: Dict[int, str] = {}
+        self.resort = False
+        self.last_epoch = 0
+        self.values: Dict[int, Any] = {}  # handle -> value, while the device holds the handle
+        self.next_handle = 0
+        self.jwin = None
+
+    def on_epoch(self, epoch: int, items: list) -> list:
+        from bytewax_b200 import gpu
+
+        np, plan = self.np, self.plan
+        getter = getattr(plan.clock, "ts_getter", None)
+        now = self._now_us()
+        if getter is None:  # SystemClock (windowing.py:196-222): an item's timestamp is the system time of its batch
+            now_dt = _dt(now)
+            getter = lambda _v: now_dt  # noqa: E731
+        keys, sides, handles, ts, labelled = [], [], [], [], []
+        for item in items:
+            key, sv = _split_item(self.step_id, item)
+            side, value = sv
+            keys.append(self._key_id(key))
+            sides.append(side)
+            ts.append(_us(getter(value)))
+            h = self.next_handle
+            self.next_handle += 1
+            handles.append(h)
+            self.values[h] = value
+            labelled.append(sv)
+        if self.jwin is None:
+            self.jwin = gpu.JoinWindow(
+                _get_gpu_ctx(), plan.insert_mode, plan.emit_mode, plan.ordered, plan.sides, self.length_us, self.offset_us, self.align_us,
+                self.wait_us, capacity_hint=int(os.environ.get("BYTEWAX_B200_KEYS", 1 << 20)), max_windows_per_key=64,
+                max_queued_rows=1 << 22 if plan.ordered else 0, max_batch_rows=int(os.environ.get("BYTEWAX_B200_BATCH", 1 << 22)),
+                max_emit_rows=1 << 22, max_late_rows=1 << 22)
+        self.last_epoch = max(epoch, self.last_epoch)
+        self.jwin.apply(np.array(keys, dtype=np.uint64), np.array(sides, dtype=np.uint8), np.array(handles, dtype=np.uint64),
+                        np.array(ts, dtype=np.int64), self.last_epoch, now or 0)
+        return self._jwin_rows(self.jwin.advance(), labelled)
+
+    def on_notify(self) -> list:
+        if self.jwin is None:
+            return []
+        now = self._now_us()
+        if now is None or now <= 0:
+            return []
+        return self._jwin_rows(self.jwin.advance(system_now_us=now), [])
+
+    def on_eof(self) -> list:
+        if self.jwin is None:
+            return []
+        out = self._jwin_rows(self.jwin.eof(), [])
+        self.release()
+        return out
+
+    def release(self):
+        if self.jwin is not None:
+            self.jwin.close()
+            self.jwin = None
+
+    def _jwin_rows(self, out, labelled) -> list:
+        from bytewax_b200.operators.windowing import WindowMetadata
+
+        V = self.values
+        lates = [(self._key_str(k), w, labelled[r]) for k, w, r in zip(out.late_key.tolist(), out.late_window_id.tolist(), out.late_row.tolist())]
+        downs = [(self._key_str(k), w, tuple(None if h is None else V[h] for h in t))
+                 for k, w, t in zip(out.down_key.tolist(), out.down_window_id.tolist(), out.tuples())]
+        metas = [(self._key_str(k), w) for k, w in zip(out.meta_key.tolist(), out.meta_window_id.tolist())]
+        if self.resort:  # interned (non-numeric) keys: restore ascending key-string order; stable
+            for rows in (lates, downs, metas):
+                rows.sort(key=lambda r: r[0])
+        rows = [(ks, (w, "L", sv)) for ks, w, sv in lates]
+        rows.extend((ks, (w, "E", t)) for ks, w, t in downs)
+        for ks, w in metas:
+            o, c = self.jwin.window_bounds(w)
+            rows.append((ks, (w, "M", WindowMetadata(_dt(o), _dt(c)))))
+        for h in out.released.tolist():  # after this call's rows are built: no later row can name these
+            del V[h]
+        return rows
+
+
 def _td_us(td: timedelta) -> int:
     return (td.days * 86400 + td.seconds) * 1_000_000 + td.microseconds
 
 
 def _gpu_step_for(step_id: str, plan):
     from bytewax_b200.operators import GpuFinalPlan, GpuJoinPlan, GpuSmapPlan
-    from bytewax_b200.operators.windowing import SessionWindower
+    from bytewax_b200.operators.windowing import GpuJoinWindowPlan, SessionWindower
 
+    if isinstance(plan, GpuJoinWindowPlan):
+        return _GpuJoinWindowStep(step_id, plan)
     if isinstance(getattr(plan, "windower", None), SessionWindower):
         return _GpuSessionStep(step_id, plan)
     if isinstance(plan, GpuSmapPlan):

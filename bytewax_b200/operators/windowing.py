@@ -794,9 +794,36 @@ def join_window(step_id: str, clock: Clock, windower: Windower, *sides: KeyedStr
         state = resume_state if resume_state is not None else _JoinState.for_side_count(side_count)
         return _JoinWindowLogic(insert_mode, emit_mode, state)
 
+    plan = _join_window_plan(clock, windower, side_count, insert_mode, emit_mode, ordered)
     # items reach the clock as (side, value): unwrap for the user's ts_getter
     if isinstance(clock, EventClock):
         inner = clock.ts_getter
         clock = EventClock(lambda side_v: inner(side_v[1]), clock.wait_for_system_duration, clock.now_getter, clock.to_system_utc)
     merged = op._join_label_merge("add_names", *sides)
-    return window("window", merged, clock, windower, shim_builder, ordered=ordered)
+    return window("window", merged, clock, windower, shim_builder, ordered=ordered, _gpu_plan=plan)
+
+
+@dataclass(frozen=True)
+class GpuJoinWindowPlan:
+    """A ``join_window`` the engine may run with ``bw_jwin_*`` (K8): insert mode first / last, 1 to 4 sides, a tumbling or
+    sliding windower, and an `EventClock` with an identity ``to_system_utc`` or a `SystemClock`.  Values travel as
+    handles into a host-side dict, so they can be any Python object."""
+
+    insert_mode: str
+    emit_mode: str
+    ordered: bool
+    sides: int
+    clock: Any     # the user's clock: its ts_getter sees the bare value
+    windower: Any
+
+
+def _join_window_plan(clock, windower, side_count, insert_mode, emit_mode, ordered) -> Optional[GpuJoinWindowPlan]:
+    # product keeps lists per side and session windows merge: host engine.  A custom `to_system_utc` moves the notify
+    # time away from the event time the device compares with the system clock (windowing.py:1177-1178): host engine.
+    if insert_mode not in ("first", "last") or not 1 <= side_count <= 4:
+        return None
+    if not isinstance(windower, (SlidingWindower, TumblingWindower)):
+        return None
+    if not (isinstance(clock, SystemClock) or (isinstance(clock, EventClock) and clock.to_system_utc is _identity)):
+        return None
+    return GpuJoinWindowPlan(insert_mode, emit_mode, bool(ordered), side_count, clock, windower)

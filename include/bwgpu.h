@@ -439,6 +439,80 @@ bw_status bw_session_advance(bw_session* s, int64_t system_now_us, bw_session_ro
 /* End of input: watermark := UTC_MAX (:300-302), so sessions with close >= UTC_MAX - gap stay open. */
 bw_status bw_session_eof(bw_session* s, bw_session_rows* out);
 
+/* Windowed join (K8): `join_window` (pysrc/bytewax/operators/windowing.py:2056-2140) with insert modes first / last,
+ * i.e. `_WindowLogic` (:1046-1190) over `_SlidingWindowerLogic` (:603-668; tumbling == offset equal to length,
+ * :921-926) with `_JoinWindowLogic` (:1849-1902) per window.  Values travel as u64 handles; the objects stay with the
+ * caller.  Per key, per call, in order: the EventClock's late test per item (:263-287; a late item gives one row per id
+ * of `intersects(ts)`, ascending, :611-618, :636-637, :1125-1127, and is not queued); `_flush_queue` (:1095-1108) at the
+ * watermark after the key's last item: unordered, every queued entry in arrival order; ordered, the entries with
+ * ts <= watermark, stably sorted by ts, the rest kept queued in their order across calls; each due entry goes to every
+ * window of `open_for(ts)` in ascending id (:626-633, :1064-1077; a window is opened on its first value), where "first"
+ * sets its side only if unset, "last" always (:1866-1876, `_JoinState` operators/__init__.py:2076-2120), "complete" emits
+ * the tuple and clears the state once every side is set, "running" emits the tuple after every value; then
+ * `_handle_closed` (:1087-1093): windows with close <= watermark in first-opened order, each giving the `final` tuple
+ * (emit mode final) and then its metadata row.  A key with no open window and an empty queue is discarded, clock state
+ * included (:1110-1113, src/operators.rs:796-799).  One GPU only. */
+typedef struct bw_jwin bw_jwin;
+typedef struct bw_jwin_spec {
+  uint32_t struct_size;
+  int32_t insert_mode;          /* BW_JOIN_INSERT_FIRST / LAST (product keeps lists per side: host engine) */
+  int32_t emit_mode;            /* BW_JOIN_EMIT_COMPLETE / FINAL / RUNNING */
+  int32_t ordered;              /* 1: play values in timestamp order once the watermark passes them (the default) */
+  int32_t sides;                /* 1..4 joined streams */
+  int32_t max_windows_per_key;  /* 1..64 open windows per key */
+  int64_t length_us;            /* window length, > 0 */
+  int64_t offset_us;            /* 0 < offset <= length (TumblingWindower: == length) */
+  int64_t align_us;             /* align_to */
+  int64_t wait_us;              /* EventClock.wait_for_system_duration, or BW_WAIT_FOREVER */
+  uint64_t capacity_hint;       /* live keys; a key's slot is kept once seen */
+  uint64_t max_queued_rows;     /* ordered mode: queued entries over ALL keys (with a long wait one key may hold most) */
+  uint64_t max_batch_rows;
+  uint64_t max_emit_rows;       /* down rows, and meta rows, retained between bw_jwin_advance calls */
+  uint64_t max_late_rows;       /* late rows retained between bw_jwin_advance calls */
+} bw_jwin_spec;
+/* Rows handed downstream since the last advance / eof, in the reference's order: per call (activation, notify phase
+ * or EOF), ascending key string (src/operators.rs:758-767, :862-894); within a key `down` rows in play order with the
+ * close-time (`final`) rows after them, `meta` rows in first-opened order, `late` rows in arrival order (one per window
+ * id, ascending).  Host pointers into memory owned by the library, valid until the next advance / eof / destroy. */
+typedef struct bw_jwin_rows {
+  uint64_t n_down;
+  const uint64_t* down_key;
+  const int64_t* down_window_id;
+  const uint64_t* down_handle[4]; /* [side][row]: valid where bit `side` of down_mask is set (else the reference emits None) */
+  const uint64_t* down_mask;
+  const uint64_t* down_epoch;
+  uint64_t n_meta;                /* closed windows: WindowMetadata(align + id * offset, + length) */
+  const uint64_t* meta_key;
+  const int64_t* meta_window_id;
+  const uint64_t* meta_epoch;
+  uint64_t n_late;
+  const uint64_t* late_key;
+  const int64_t* late_window_id;
+  const uint64_t* late_epoch;
+  const uint64_t* late_activation; /* (activation, row) name the input row (activations counted from 0) */
+  const uint64_t* late_row;
+  /* handles no window and no queue entry holds any more; each handle passed to apply is listed exactly once, in the
+   * rows of the call that let go of it (late items and values never stored: the call that received them) */
+  uint64_t n_released;           /* (the device buffer behind it grows with the handles held, never with the table size) */
+  const uint64_t* released;
+} bw_jwin_rows;
+bw_status bw_jwin_create(bw_ctx* ctx, const bw_jwin_spec* spec, bw_jwin** out);
+void bw_jwin_destroy(bw_jwin* j);
+/* One activation from HOST columns (keys, side 0..sides-1, handle, ts); blocks.  `system_now_us` is `now_getter()`
+ * for this activation (windowing.py:250-261; it must not go backwards; 0 throughout = a frozen clock). */
+bw_status bw_jwin_apply(bw_jwin* j, const uint64_t* keys, const uint8_t* side, const uint64_t* handles, const int64_t* ts_us,
+                        uint64_t rows, uint64_t epoch, int64_t system_now_us);
+/* Same with DEVICE columns; returns once the work is enqueued (the columns must stay valid until the next call).  A side
+ * value >= sides is not played: the next call returns BW_ERR_SPEC and the join refuses further calls. */
+bw_status bw_jwin_apply_device(bw_jwin* j, const uint64_t* d_keys, const uint8_t* d_side, const uint64_t* d_handles,
+                               const int64_t* d_ts_us, uint64_t rows, uint64_t epoch, int64_t system_now_us);
+/* Rows since the last call.  `system_now_us` > 0 first runs the notify phase at that system time
+ * (src/operators.rs:808-858, windowing.py:1135-1142, 1153-1180 with an identity `to_system_utc`): every key whose
+ * earliest window close -- or, ordered, the ts of its FIRST queued entry -- has been reached flushes at its watermark. */
+bw_status bw_jwin_advance(bw_jwin* j, int64_t system_now_us, bw_jwin_rows* out);
+/* End of input: every key flushes at watermark UTC_MAX (:1144-1151). */
+bw_status bw_jwin_eof(bw_jwin* j, bw_jwin_rows* out);
+
 /* ---- plain device-memory helpers (tests / bench / host bindings without torch) ---- */
 bw_status bw_dev_alloc(bw_ctx* ctx, uint64_t bytes, void** out);
 bw_status bw_dev_free(bw_ctx* ctx, void* ptr);
