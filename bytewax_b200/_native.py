@@ -122,6 +122,21 @@ class BwJwinRows(C.Structure):
                 ("n_released", C.c_uint64), ("released", C.POINTER(C.c_uint64))]
 
 
+class BwCollectSpec(C.Structure):
+    _fields_ = [("struct_size", C.c_uint32), ("ordered", C.c_int32), ("max_windows_per_key", C.c_int32), ("pad", C.c_int32),
+                ("length_us", C.c_int64), ("offset_us", C.c_int64), ("align_us", C.c_int64), ("wait_us", C.c_int64),
+                ("capacity_hint", C.c_uint64), ("max_queued_rows", C.c_uint64), ("max_batch_rows", C.c_uint64),
+                ("max_emit_rows", C.c_uint64), ("max_late_rows", C.c_uint64)]
+
+
+class BwCollectRows(C.Structure):
+    _fields_ = [("n_down", C.c_uint64), ("down_key", C.POINTER(C.c_uint64)), ("down_window_id", C.POINTER(C.c_int64)),
+                ("down_epoch", C.POINTER(C.c_uint64)), ("down_offset", C.POINTER(C.c_uint64)), ("handle", C.POINTER(C.c_uint64)),
+                ("n_late", C.c_uint64), ("late_key", C.POINTER(C.c_uint64)), ("late_window_id", C.POINTER(C.c_int64)),
+                ("late_epoch", C.POINTER(C.c_uint64)), ("late_activation", C.POINTER(C.c_uint64)), ("late_row", C.POINTER(C.c_uint64)),
+                ("n_released", C.c_uint64), ("released", C.POINTER(C.c_uint64))]
+
+
 # every symbol include/bwgpu.h declares: (restype, argtypes)
 _P = C.c_void_p
 SYMBOLS = {
@@ -175,6 +190,12 @@ SYMBOLS = {
     "bw_jwin_apply_device": (C.c_int32, [_P, _P, _P, _P, _P, C.c_uint64, C.c_uint64, C.c_int64]),
     "bw_jwin_advance": (C.c_int32, [_P, C.c_int64, C.POINTER(BwJwinRows)]),
     "bw_jwin_eof": (C.c_int32, [_P, C.POINTER(BwJwinRows)]),
+    "bw_collect_create": (C.c_int32, [_P, C.POINTER(BwCollectSpec), C.POINTER(_P)]),
+    "bw_collect_destroy": (None, [_P]),
+    "bw_collect_apply": (C.c_int32, [_P, _P, _P, _P, C.c_uint64, C.c_uint64, C.c_int64]),
+    "bw_collect_apply_device": (C.c_int32, [_P, _P, _P, _P, C.c_uint64, C.c_uint64, C.c_int64]),
+    "bw_collect_advance": (C.c_int32, [_P, C.c_int64, C.POINTER(BwCollectRows)]),
+    "bw_collect_eof": (C.c_int32, [_P, C.POINTER(BwCollectRows)]),
     "bw_dev_alloc": (C.c_int32, [_P, C.c_uint64, C.POINTER(_P)]),
     "bw_dev_free": (C.c_int32, [_P, _P]),
     "bw_host_alloc": (C.c_int32, [_P, C.c_uint64, C.POINTER(_P)]),

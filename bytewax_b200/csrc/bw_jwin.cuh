@@ -51,6 +51,10 @@ struct __align__(16) JwWin {
   i64 id;
   u64 mask;
   u64 h[BW_JW_MAXSIDES];
+  __device__ void open(i64 i) {
+    id = i;
+    mask = 0;
+  }
 };
 struct JwTable {
   u64* keys;
@@ -95,7 +99,9 @@ struct JwParams {
   u32 batch_no;
 };
 
-__device__ __forceinline__ void bw_jw_fail(const JwTable& t, u32 bit) {
+// (T, E: JwTable / JwEmit here, and the tables and emit buffers of the kernels that share these steps, bw_collect.cuh)
+template <class T>
+__device__ __forceinline__ void bw_jw_fail(const T& t, u32 bit) {
   atomicOr(t.why, bit);
   atomicCAS(t.err, 0u, (u32)BW_ERR_CAPACITY);
 }
@@ -118,7 +124,86 @@ __device__ __forceinline__ void bw_jw_ids(const JwParams& p, i64 ts, i64& lo, i6
 }
 __device__ __forceinline__ i64 bw_jw_close(const JwParams& p, i64 id) { return p.align + p.offset * id + p.length; }
 
-__device__ __forceinline__ void bw_jw_release(const JwTable& t, const JwEmit& e, u64 h) {
+// the window `id` among a key's n open windows W (first-opened order), opened at the end when absent (`open_for`: a
+// window is opened on its first value); M when the key already holds M windows
+template <class W>
+__device__ __forceinline__ u32 bw_jw_find_or_open(W* Ws, u32& n, u32 M, i64 id) {
+  u32 i = 0;
+  while (i < n && Ws[i].id != id) ++i;
+  if (i == n) {
+    if (n >= M) return M;
+    Ws[n].open(id);
+    ++n;
+  }
+  return i;
+}
+
+// `_handle_closed` (windowing.py:1087-1093): every window with close <= wm leaves W in first-opened order; `on_close`
+// sees it after it has left (so W[0, n) are the windows still open)
+template <class W, class F>
+__device__ __forceinline__ void bw_jw_close_each(const JwParams& p, W* Ws, u32& n, i64 wm, F&& on_close) {
+  u32 i = 0;
+  while (i < n) {
+    if (bw_jw_close(p, Ws[i].id) > wm) {
+      ++i;
+      continue;
+    }
+    const W w = Ws[i];
+    for (u32 j = i + 1; j < n; ++j) Ws[j - 1] = Ws[j];
+    --n;
+    on_close(w);
+  }
+}
+
+// builder(None) of a key with no logic: _EventClockLogic.__post_init__ (windowing.py:245-248), empty windower and queue
+__device__ __forceinline__ void bw_jw_begin(JwState& st, const JwParams& p) {
+  if (st.init) return;
+  st.init = 1;
+  st.wm_base = BW_UTC_MIN_US;
+  st.sys_max = p.now;
+  st.n = st.nq = 0;
+  st.qord = ~0ULL;
+}
+
+// _EventClockLogic.on_item (windowing.py:263-287; ts - wait below UTC_MIN raises OverflowError: ignored): the watermark
+// after the item goes to wm; true when the item is late
+__device__ __forceinline__ bool bw_jw_on_item(JwState& st, const JwParams& p, i64 ts, i64& wm) {
+  wm = st.wm_base + (p.now - st.sys_max);
+  if (p.wait != BW_WAIT_FOREVER && ts - BW_UTC_MIN_US >= p.wait) {
+    const i64 cand = ts - p.wait;
+    if (cand > wm) {
+      st.wm_base = cand;
+      st.sys_max = p.now;
+      wm = cand;
+    }
+  }
+  return ts < wm;
+}
+
+// a late item: one row per id of intersects(ts), ascending (windowing.py:636-637, :1125-1127), naming input row o
+template <class T, class E>
+__device__ void bw_jw_late_rows(const T& t, const E& e, const JwParams& p, u64 key, i64 ts, u32 o, u64& lseq) {
+  i64 lo, hi;
+  bw_jw_ids(p, ts, lo, hi);
+  const u64 cnt = hi >= lo ? (u64)(hi - lo + 1) : 0;
+  const u64 i0 = cnt > e.max_late ? e.max_late : atomicAdd(e.n_late, (unsigned long long)cnt);
+  if (i0 + cnt > e.max_late) {
+    bw_jw_fail(t, BW_JW_FULL_LATE);
+    return;
+  }
+  for (u64 c = 0; c < cnt; ++c) {
+    e.l_key[i0 + c] = key;
+    e.l_wid[i0 + c] = (u64)(lo + (i64)c);
+    e.l_epoch[i0 + c] = p.epoch;
+    e.l_act[i0 + c] = p.batch_no;
+    e.l_row[i0 + c] = o;
+    e.l_ord[i0 + c] = p.ord;
+    e.l_seq[i0 + c] = lseq++;
+  }
+}
+
+template <class T, class E>
+__device__ __forceinline__ void bw_jw_release(const T& t, const E& e, u64 h) {
   const u64 i = atomicAdd(e.n_rel, 1ULL);
   if (i < e.max_rel) e.rel[i] = h;  // (the host sizes the buffer for every handle the call can release: never reached)
   else bw_jw_fail(t, BW_JW_FULL_EMIT);
@@ -158,14 +243,8 @@ __device__ bool bw_jw_play(const JwTable& t, const JwEmit& e, const JwParams& p,
   i64 lo, hi;
   bw_jw_ids(p, ts, lo, hi);
   for (i64 id = lo; id <= hi; ++id) {
-    u32 i = 0;
-    while (i < n && W[i].id != id) ++i;
-    if (i == n) {  // open_for: opened in first-opened order, state built on the first value
-      if (n >= (u32)t.M) return false;
-      W[n].id = id;
-      W[n].mask = 0;
-      ++n;
-    }
+    const u32 i = bw_jw_find_or_open(W, n, (u32)t.M, id);
+    if (i == (u32)t.M) return false;
     JwWin& w = W[i];
     if (!(w.mask & bit)) {
       w.h[side] = h;
@@ -193,13 +272,7 @@ __device__ bool bw_jw_play(const JwTable& t, const JwEmit& e, const JwParams& p,
 // `_handle_closed` (windowing.py:1087-1093): windows with close <= watermark in first-opened order; `final` row, then meta
 __device__ void bw_jw_close_windows(const JwTable& t, const JwEmit& e, const JwParams& p, u64 key, JwWin* W, u32& n, i64 wm, u64& seq,
                                     u64& mseq) {
-  u32 i = 0;
-  while (i < n) {
-    if (bw_jw_close(p, W[i].id) > wm) {
-      ++i;
-      continue;
-    }
-    const JwWin w = W[i];
+  bw_jw_close_each(p, W, n, wm, [&](const JwWin& w) {
     if (p.emit_mode == BW_JOIN_EMIT_FINAL) bw_jw_emit(t, e, p, key, w, seq);
     const u64 m = atomicAdd(e.n_meta, 1ULL);
     if (m >= e.max_rows) {
@@ -211,18 +284,17 @@ __device__ void bw_jw_close_windows(const JwTable& t, const JwEmit& e, const JwP
       e.m_ord[m] = p.ord;
       e.m_seq[m] = mseq++;
     }
-    for (u32 j = i + 1; j < n; ++j) W[j - 1] = W[j];
-    --n;
     for (int s = 0; s < t.sides; ++s)
       if ((w.mask >> s & 1) && !bw_jw_held(W, n, t.sides, w.h[s])) bw_jw_release(t, e, w.h[s]);
-  }
+  });
 }
 
 // notify_at (windowing.py:1153-1180), identity `to_system_utc`
-__device__ __forceinline__ i64 bw_jw_notify_at(const JwParams& p, const JwState& st, const JwWin* W) {
+template <class W>
+__device__ __forceinline__ i64 bw_jw_notify_at(const JwParams& p, const JwState& st, const W* Ws) {
   i64 at = INT64_MAX;
   for (u32 i = 0; i < st.n; ++i) {
-    const i64 c = bw_jw_close(p, W[i].id);
+    const i64 c = bw_jw_close(p, Ws[i].id);
     at = c < at ? c : at;
   }
   if (p.ordered && st.nq && st.q0ts < at) at = st.q0ts;
@@ -250,13 +322,7 @@ __global__ void k_jwin_apply(JwTable t, JwEmit e, JwParams p, JwPool pool, u64 b
       continue;
     }
     JwState st = t.st[s];
-    if (!st.init) {  // builder(None): _EventClockLogic.__post_init__ (windowing.py:245-248), empty windower and queue
-      st.init = 1;
-      st.wm_base = BW_UTC_MIN_US;
-      st.sys_max = p.now;
-      st.n = st.nq = 0;
-      st.qord = ~0ULL;
-    }
+    bw_jw_begin(st, p);
     u64 end = h;
     while (end < n && ksorted[end] == key) ++end;
     i64 wm = BW_UTC_MIN_US;
@@ -275,35 +341,9 @@ __global__ void k_jwin_apply(JwTable t, JwEmit e, JwParams p, JwPool pool, u64 b
         }
         continue;
       }
-      // _EventClockLogic.on_item (ts - wait below UTC_MIN raises OverflowError: ignored)
-      wm = st.wm_base + (p.now - st.sys_max);
-      if (p.wait != BW_WAIT_FOREVER && ts - BW_UTC_MIN_US >= p.wait) {
-        const i64 cand = ts - p.wait;
-        if (cand > wm) {
-          st.wm_base = cand;
-          st.sys_max = p.now;
-          wm = cand;
-        }
-      }
-      const bool is_late = ts < wm;
-      if (is_late) {  // one row per id of intersects(ts), ascending (windowing.py:636-637); the handle is let go
-        i64 lo, hi;
-        bw_jw_ids(p, ts, lo, hi);
-        const u64 cnt = hi >= lo ? (u64)(hi - lo + 1) : 0;
-        const u64 i0 = cnt > e.max_late ? e.max_late : atomicAdd(e.n_late, (unsigned long long)cnt);
-        if (i0 + cnt > e.max_late) {
-          bw_jw_fail(t, BW_JW_FULL_LATE);
-        } else {
-          for (u64 c = 0; c < cnt; ++c) {
-            e.l_key[i0 + c] = key;
-            e.l_wid[i0 + c] = (u64)(lo + (i64)c);
-            e.l_epoch[i0 + c] = p.epoch;
-            e.l_act[i0 + c] = p.batch_no;
-            e.l_row[i0 + c] = o;
-            e.l_ord[i0 + c] = p.ord;
-            e.l_seq[i0 + c] = lseq++;
-          }
-        }
+      const bool is_late = bw_jw_on_item(st, p, ts, wm);
+      if (is_late) {  // the late rows; the handle is let go
+        bw_jw_late_rows(t, e, p, key, ts, o, lseq);
         bw_jw_release(t, e, handles[o]);
       }
       if (p.ordered) {
@@ -340,14 +380,16 @@ __global__ void k_jwin_apply(JwTable t, JwEmit e, JwParams p, JwPool pool, u64 b
 
 // notify (src/operators.rs:808-858): keys whose notify_at has come, at the watermark `on_notify` sees (:289-298);
 // EOF (:862-894, windowing.py:1144-1151): every key, watermark UTC_MAX
-__global__ void k_jwin_mark(JwTable t, JwParams p, int eof) {
+// (W: the table's window records, JwWin here)
+template <class W>
+__global__ void k_jwin_mark(JwTable t, const W* win, JwParams p, int eof) {
   for (u64 s = (u64)blockIdx.x * blockDim.x + threadIdx.x; s <= t.cap; s += (u64)gridDim.x * blockDim.x) {
     JwState& st = t.st[s];
     if (!st.init) continue;
     if (eof) {
       st.wm = BW_UTC_MAX_US;
     } else {
-      if (bw_jw_notify_at(p, st, t.win + s * (u64)t.M) > p.now) continue;
+      if (bw_jw_notify_at(p, st, win + s * (u64)t.M) > p.now) continue;
       st.wm = st.wm_base + (p.now - st.sys_max);
     }
     st.act = p.ord;
@@ -380,6 +422,30 @@ __global__ void k_jwin_ranges(JwTable t, JwParams p, JwPool pool, const u32* per
   }
 }
 
+// the `keep` entries of slot s's range [qb, qe) of the sorted pool that are not due stay queued, in their order
+// (windowing.py:1098-1100): they go to the next pool; false when it is full
+template <class T, class E>
+__device__ bool bw_jw_carry(const T& t, const E& e, const JwPool& pool, const u32* perm, u32 qb, u32 qe, bool woken, u64 s, u32 keep,
+                            JwState& st) {
+  const u64 b = atomicAdd(e.n_next, (unsigned long long)keep);
+  if (b + keep > e.max_queue) {
+    bw_jw_fail(t, BW_JW_FULL_QUEUE);
+    return false;
+  }
+  u64 w = b;
+  for (u32 i = qb; i < qe; ++i) {
+    const u32 x = perm[i];
+    if (pool.side[x] == BW_JW_DROP || (woken && pool.ts[x] <= st.wm)) continue;
+    if (w == b) st.q0ts = pool.ts[x];
+    e.next.slot[w] = (u32)s;
+    e.next.ts[w] = pool.ts[x];
+    e.next.h[w] = pool.h[x];
+    e.next.side[w] = pool.side[x];
+    ++w;
+  }
+  return true;
+}
+
 // pass B, one thread per slot: a woken key plays its due entries (already in ts order, ties in arrival order), keeps
 // the others queued in arrival order, and closes; an idle key's entries move to the next pool unchanged
 __global__ void k_jwin_flush(JwTable t, JwEmit e, JwParams p, JwPool pool, const u32* perm) {
@@ -407,24 +473,7 @@ __global__ void k_jwin_flush(JwTable t, JwEmit e, JwParams p, JwPool pool, const
       bw_jw_fail(t, BW_JW_FULL_WINDOWS);
       continue;
     }
-    if (keep) {  // the rest of the queue, in its order (windowing.py:1098-1100)
-      const u64 b = atomicAdd(e.n_next, (unsigned long long)keep);
-      if (b + keep > e.max_queue) {
-        bw_jw_fail(t, BW_JW_FULL_QUEUE);
-        continue;
-      }
-      u64 w = b;
-      for (u32 i = qb; i < qe; ++i) {
-        const u32 x = perm[i];
-        if (pool.side[x] == BW_JW_DROP || (woken && pool.ts[x] <= st.wm)) continue;
-        if (w == b) st.q0ts = pool.ts[x];
-        e.next.slot[w] = (u32)s;
-        e.next.ts[w] = pool.ts[x];
-        e.next.h[w] = pool.h[x];
-        e.next.side[w] = pool.side[x];
-        ++w;
-      }
-    }
+    if (keep && !bw_jw_carry(t, e, pool, perm, qb, qe, woken, s, keep, st)) continue;
     st.nq = keep;
     if (woken) {
       bw_jw_close_windows(t, e, p, key, W, nw, st.wm, seq, mseq);

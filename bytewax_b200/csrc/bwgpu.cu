@@ -36,6 +36,7 @@
 #include "bw_keyed.cuh"
 #include "bw_session.cuh"
 #include "bw_jwin.cuh"
+#include "bw_collect.cuh"
 #include "bw_prepass.cuh"
 #include "bw_slow.cuh"
 #include "bw_late.cuh"
@@ -3146,8 +3147,9 @@ static bw_status jwin_drain(bw_jwin* j) {
 
 // Room in the release buffer for the next call: it can release at most the handles passed in earlier and not released
 // yet, plus its own `rows`.  Called after jwin_drain, so nothing on the stream reads the old buffer and it holds no
-// releases; the buffer then holds what the join actually holds, not what its tables could hold.
-static bw_status jwin_room(bw_jwin* j, u64 rows) {
+// releases; the buffer then holds what the join actually holds, not what its tables could hold.  (J: bw_jwin, bw_collect)
+template <class J>
+static bw_status jwin_room(J* j, u64 rows) {
   const u64 need = j->outstanding + rows;
   if (need <= j->e.max_rel) return BW_OK;
   const u64 grow = std::max<u64>(need, 2 * j->e.max_rel);
@@ -3157,20 +3159,31 @@ static bw_status jwin_room(bw_jwin* j, u64 rows) {
   return BW_OK;
 }
 
-// ordered mode: sort the pool's due entries into play order, then flush every woken key (k_jwin_flush)
-static bw_status jwin_flush_pool(bw_jwin* j, const JwParams& p, u64 n) {
+// ordered mode: put the n entries of `pool` in play order -- x.perm: every key's due entries by ts (ties in arrival
+// order), then the rest in arrival order, keys by slot -- and give every key its range (k_jwin_ranges).  (J: bw_jwin,
+// bw_collect)
+template <class J>
+static bw_status jwin_sort_pool(J* j, const JwTable& t, const JwParams& p, u64 n) {
   bw_ctx* ctx = j->ctx;
   const int grid = ctx->sm_count * 4;
   SortScratch& x = j->srt;
-  if (n) {
-    k_jwin_sortkey<<<grid, 256, 0, j->s>>>(j->t, p, j->pool, x.sk, x.perm, n);
-    size_t tb = x.cub_bytes;
-    CU(ctx, cub::DeviceRadixSort::SortPairs(x.cub, tb, x.sk, x.sk2, x.perm, x.perm2, (int)n, 0, 64, j->s));
-    k_jwin_slotkey<<<grid, 256, 0, j->s>>>(j->pool, x.perm2, x.sk, n);
-    tb = x.cub_bytes;
-    CU(ctx, cub::DeviceRadixSort::SortPairs(x.cub, tb, x.sk, x.sk2, x.perm2, x.perm, (int)n, 0, j->slot_bits, j->s));
-    k_jwin_ranges<<<grid, 256, 0, j->s>>>(j->t, p, j->pool, x.perm, n);
-  }
+  if (!n) return BW_OK;
+  k_jwin_sortkey<<<grid, 256, 0, j->s>>>(t, p, j->pool, x.sk, x.perm, n);
+  size_t tb = x.cub_bytes;
+  CU(ctx, cub::DeviceRadixSort::SortPairs(x.cub, tb, x.sk, x.sk2, x.perm, x.perm2, (int)n, 0, 64, j->s));
+  k_jwin_slotkey<<<grid, 256, 0, j->s>>>(j->pool, x.perm2, x.sk, n);
+  tb = x.cub_bytes;
+  CU(ctx, cub::DeviceRadixSort::SortPairs(x.cub, tb, x.sk, x.sk2, x.perm2, x.perm, (int)n, 0, j->slot_bits, j->s));
+  k_jwin_ranges<<<grid, 256, 0, j->s>>>(t, p, j->pool, x.perm, n);
+  return BW_OK;
+}
+
+// ordered mode: sort the pool's due entries into play order, then flush every woken key (k_jwin_flush)
+static bw_status jwin_flush_pool(bw_jwin* j, const JwParams& p, u64 n) {
+  bw_ctx* ctx = j->ctx;
+  SortScratch& x = j->srt;
+  bw_status st = jwin_sort_pool(j, j->t, p, n);
+  if (st != BW_OK) return st;
   JwEmit e = j->e;
   e.next = j->pool2;
   k_jwin_flush<<<ctx->sm_count * 8, 256, 0, j->s>>>(j->t, e, p, j->pool, x.perm);
@@ -3230,8 +3243,9 @@ bw_status bw_jwin_apply(bw_jwin* j, const uint64_t* keys, const uint8_t* side, c
   return jwin_drain(j);
 }
 
-// order rows [0, n) of one stream by (call, key string, seq) and copy `nc` columns to the host
-static bw_status jwin_ship(bw_jwin* j, u64 n, const u64* key, const u64* seq, const u64* ord, const u64* const* src, int nc, HostCols* dst) {
+// order rows [0, n) of one stream by (call, key string, seq) and copy `nc` columns to the host (J: bw_jwin, bw_collect)
+template <class J>
+static bw_status jwin_ship(J* j, u64 n, const u64* key, const u64* seq, const u64* ord, const u64* const* src, int nc, HostCols* dst) {
   if (!n) return BW_OK;
   bw_ctx* ctx = j->ctx;
   SortScratch& x = j->srt;
@@ -3296,7 +3310,7 @@ static bw_status jwin_wake(bw_jwin* j, int eof) {
   if (st != BW_OK) return st;
   if ((st = jwin_room(j, 0)) != BW_OK) return st;
   const JwParams p = jwin_params(j, j->last_epoch);
-  k_jwin_mark<<<ctx->sm_count * 8, 256, 0, j->s>>>(j->t, p, eof);
+  k_jwin_mark<<<ctx->sm_count * 8, 256, 0, j->s>>>(j->t, j->t.win, p, eof);
   CU(ctx, cudaGetLastError());
   j->undrained = true;
   if (j->spec.ordered) return jwin_flush_pool(j, p, j->nq);
@@ -3327,4 +3341,431 @@ bw_status bw_jwin_eof(bw_jwin* j, bw_jwin_rows* out) {
   bw_status st = jwin_wake(j, 1);
   if (st != BW_OK) return st;
   return jwin_collect(j, out);
+}
+
+// ===========================================================================
+// K9 host side: collect_window (bw_collect.cuh)
+// ===========================================================================
+struct bw_collect {
+  Owner own;  // every buffer and the stream below
+  bw_ctx* ctx = nullptr;
+  bw_collect_spec spec{};
+  CwTable t{};
+  CwStore es{};
+  KeyedScratch k;
+  cudaStream_t s = nullptr;
+  u32* h_err = nullptr;                 // err, why
+  unsigned long long* d_cnt = nullptr;  // closed windows, late rows, released, carried-over queue entries, staged, store
+  unsigned long long* h_cnt = nullptr;
+  unsigned char *d_late = nullptr, *d_flag = nullptr;
+  u64* d_handles = nullptr;
+  i64* d_ts = nullptr;
+  CwEmit e{};
+  JwPool pool{}, pool2{};  // ordered mode: the queue, and the one the next flush writes
+  u64 nq = 0;              // entries in `pool`
+  int slot_bits = 1;
+  u64 kmax = 1;            // entries one value can add: min(ceil(length / offset), max_windows_per_key)
+  u64 n_store = 0, dead = 0;      // entries in the store, and how many of them are dead
+  u64 n_rows = 0, n_stage = 0;    // closed windows and staged handles since the last advance / eof
+  SortScratch srt;                // pool sort, ordering and compaction scratch
+  u32* d_inv = nullptr;           // advance / eof: a closed window's place in the reference's order
+  u64 *d_cs = nullptr, *d_off = nullptr;  // its count in that order, and the exclusive scan of them
+  u64* d_out = nullptr;           // the handles in the reference's order
+  u64* h_out = nullptr;
+  u64 out_cap = 0;
+  HostCols hd, hl;                // down: key, window id, epoch, offsets; late: key, window id, epoch, activation, row
+  std::vector<u64> released;      // since the last advance / eof
+  std::vector<u64> released_out;  // what the last advance / eof handed out
+  bool undrained = false;     // a call whose counts are not read back yet
+  u64 outstanding = 0;        // handles passed in and not released yet: what the next call can release, besides its own
+  u32 batch_no = 0;
+  u64 calls = 0, first_call = 0;  // calls (activations, notify phases, EOF) so far; the first not yet collected
+  u64 last_epoch = 0;
+  i64 now = INT64_MIN;
+  bool failed = false;
+};
+
+bw_status bw_collect_create(bw_ctx* ctx, const bw_collect_spec* spec, bw_collect** out) {
+  if (!ctx || !spec || !out) CTX_FAIL(ctx, BW_ERR_SPEC, "bw_collect_create: NULL argument");
+  if (spec->struct_size != sizeof(bw_collect_spec)) CTX_FAIL(ctx, BW_ERR_SPEC, "bw_collect_spec.struct_size mismatch");
+  if (ctx->world != 1) CTX_FAIL(ctx, BW_ERR_SPEC, "windowed collects run on one GPU (world == 1)");
+  if (spec->ordered != 0 && spec->ordered != 1) CTX_FAIL(ctx, BW_ERR_SPEC, "ordered must be 0 or 1");
+  if (spec->max_windows_per_key < 1 || spec->max_windows_per_key > BW_JW_MAXM)
+    CTX_FAIL(ctx, BW_ERR_SPEC, "max_windows_per_key must be in 1..%d", BW_JW_MAXM);
+  if (spec->length_us <= 0 || spec->length_us > BW_UTC_MAX_US - BW_UTC_MIN_US) CTX_FAIL(ctx, BW_ERR_SPEC, "length_us must be in 1..UTC_MAX - UTC_MIN");
+  if (spec->offset_us <= 0 || spec->offset_us > spec->length_us) CTX_FAIL(ctx, BW_ERR_SPEC, "offset_us must be in 1..length_us");
+  if (spec->align_us < BW_UTC_MIN_US || spec->align_us > BW_UTC_MAX_US) CTX_FAIL(ctx, BW_ERR_SPEC, "align_us out of range");
+  if (spec->wait_us < 0) CTX_FAIL(ctx, BW_ERR_SPEC, "wait_us must not be negative");
+  if (spec->max_batch_rows == 0 || spec->max_batch_rows >= (1ULL << 31)) CTX_FAIL(ctx, BW_ERR_SPEC, "bad max_batch_rows");
+  if (spec->max_queued_rows >= (1ULL << 31) - spec->max_batch_rows) CTX_FAIL(ctx, BW_ERR_SPEC, "max_queued_rows + max_batch_rows must stay below 2^31");
+  if (spec->max_emit_rows >= (1ULL << 31)) CTX_FAIL(ctx, BW_ERR_SPEC, "max_emit_rows must be below 2^31");
+  if (spec->capacity_hint >= (1ULL << 30)) CTX_FAIL(ctx, BW_ERR_SPEC, "capacity_hint must be below 2^30");
+  CU(ctx, cudaSetDevice(ctx->device));
+  std::unique_ptr<bw_collect, void (*)(bw_collect*)> cp(new bw_collect(), bw_collect_destroy);  // torn down on every failure
+  bw_collect* j = cp.get();
+  Owner& own = j->own;
+  j->ctx = ctx;
+  j->spec = *spec;
+  const u64 cap = std::max<u64>(1024, 2 * std::max<u64>(spec->capacity_hint, 1));
+  const int M = spec->max_windows_per_key;
+  const u64 per = (u64)((spec->length_us - 1) / spec->offset_us) + 1;
+  j->kmax = std::min<u64>(per, (u64)M);
+  CwTable& t = j->t;
+  t.j.cap = cap;
+  t.j.M = M;
+  t.j.sides = 1;
+  while ((1ULL << j->slot_bits) < cap + 1) ++j->slot_bits;
+  CU(ctx, own.stream(&j->s));
+  CU(ctx, own.dev(&t.j.keys, cap + 1));
+  CU(ctx, own.dev(&t.j.st, cap + 1));
+  CU(ctx, own.dev(&t.win, (cap + 1) * (u64)M));
+  CU(ctx, own.dev(&t.cell_ord, (cap + 1) * (u64)M));
+  CU(ctx, own.dev(&t.cell_c, (cap + 1) * (u64)M));
+  CU(ctx, own.dev(&t.j.err, 2));
+  t.j.why = t.j.err + 1;
+  t.err = t.j.err;
+  t.why = t.j.why;
+  CU(ctx, own.dev(&j->d_cnt, 6));
+  CU(ctx, cudaMemsetAsync(t.err, 0, 8, j->s));
+  CU(ctx, cudaMemsetAsync(j->d_cnt, 0, 48, j->s));
+  CU(ctx, own.host(&j->h_err, 64 / sizeof(u32)));
+  CU(ctx, own.host(&j->h_cnt, 64 / sizeof(unsigned long long)));
+  const u64 n = spec->max_batch_rows, m = std::max<u64>(spec->max_emit_rows, 1), l = std::max<u64>(spec->max_late_rows, 1);
+  const u64 q = spec->ordered ? spec->max_queued_rows : 0;
+  bw_status st = keyed_alloc(ctx, own, j->k, n, j->s);
+  if (st != BW_OK) return st;
+  CU(ctx, own.dev(&j->d_late, n));
+  CU(ctx, own.dev(&j->d_handles, n));
+  CU(ctx, own.dev(&j->d_ts, n));
+  if (spec->ordered) {
+    if ((st = jwin_pool_alloc(ctx, own, j->pool, q + n)) != BW_OK) return st;
+    if ((st = jwin_pool_alloc(ctx, own, j->pool2, q + n)) != BW_OK) return st;
+  }
+  CwEmit& e = j->e;
+  for (u64** c : {&e.key, &e.wid, &e.cnt, &e.soff, &e.epoch, &e.ord, &e.seq}) CU(ctx, own.dev(c, m));
+  for (u64** c : {&e.l_key, &e.l_wid, &e.l_epoch, &e.l_act, &e.l_row, &e.l_ord, &e.l_seq}) CU(ctx, own.dev(c, l));
+  CU(ctx, own.dev(&j->d_inv, m));
+  CU(ctx, own.dev(&j->d_cs, m + 1));
+  CU(ctx, own.dev(&j->d_off, m + 1));
+  // the store, the staging buffer, the output and the release buffer grow with what the collect holds (collect_room);
+  // they start at one batch
+  CwStore& es = j->es;
+  es.cap = n;
+  CU(ctx, own.dev(&es.ref, n));
+  CU(ctx, own.dev(&es.rank, n));
+  CU(ctx, own.dev(&es.h, n));
+  CU(ctx, own.dev(&j->d_flag, n));
+  e.max_stage = n;
+  CU(ctx, own.dev(&e.stage, n));
+  CU(ctx, own.dev(&e.stage_rec, n));
+  j->out_cap = n;
+  CU(ctx, own.dev(&j->d_out, n));
+  CU(ctx, own.host(&j->h_out, n));
+  e.max_rel = n;
+  CU(ctx, own.dev(&e.rel, e.max_rel));
+  e.max_rows = spec->max_emit_rows;
+  e.max_late = spec->max_late_rows;
+  e.max_queue = q;
+  e.n_rows = j->d_cnt;
+  e.n_late = j->d_cnt + 1;
+  e.n_rel = j->d_cnt + 2;
+  e.n_next = j->d_cnt + 3;
+  e.n_stage = j->d_cnt + 4;
+  es.n = j->d_cnt + 5;
+  const u64 ns = std::max(std::max(m, l), q + n);
+  CU(ctx, j->srt.reserve(own, ns, ns, j->s));
+  size_t b = 0;
+  CU(ctx, cub::DeviceScan::ExclusiveSum(nullptr, b, j->d_cs, j->d_off, (int)(m + 1), j->s));
+  CU(ctx, j->srt.grow_cub(own, b + 256));
+  CU(ctx, j->hd.reserve(own, m + 1, m + 1));
+  CU(ctx, j->hl.reserve(own, l, l));
+  k_cwin_init<<<ctx->sm_count * 4, 256, 0, j->s>>>(t);
+  CU(ctx, cudaGetLastError());
+  CU(ctx, cudaStreamSynchronize(j->s));
+  *out = cp.release();
+  return BW_OK;
+}
+
+void bw_collect_destroy(bw_collect* j) {
+  if (!j) return;
+  cudaSetDevice(j->ctx->device);
+  if (j->s) cudaStreamSynchronize(j->s);
+  delete j;  // j->own releases every buffer and the stream
+}
+
+static JwParams collect_params(bw_collect* j, u64 epoch) {
+  JwParams p{};
+  p.ordered = j->spec.ordered;
+  p.length = j->spec.length_us;
+  p.offset = j->spec.offset_us;
+  p.align = j->spec.align_us;
+  p.wait = j->spec.wait_us;
+  p.now = j->now;
+  p.epoch = epoch;
+  p.ord = j->calls++;
+  p.batch_no = j->batch_no;
+  return p;
+}
+
+#define COLLECT_REFUSE_FAILED(j) \
+  if ((j)->failed) CTX_FAIL((j)->ctx, BW_ERR_STATE, "windowed collect: an earlier call failed on the device; the collect is unusable")
+
+// wait for the last call; fail on a device-side overflow; then take its released handles and its counts
+static bw_status collect_drain(bw_collect* j) {
+  bw_ctx* ctx = j->ctx;
+  COLLECT_REFUSE_FAILED(j);
+  if (!j->undrained) return BW_OK;
+  CU(ctx, cudaMemcpyAsync(j->h_err, j->t.err, 8, cudaMemcpyDeviceToHost, j->s));
+  CU(ctx, cudaMemcpyAsync(j->h_cnt, j->d_cnt, 48, cudaMemcpyDeviceToHost, j->s));
+  CU(ctx, cudaStreamSynchronize(j->s));
+  if (j->h_err[0]) {
+    j->failed = true;
+    const u32 w = j->h_err[1];
+    CTX_FAIL(ctx, (bw_status)j->h_err[0], "windowed collect kernel ran out of capacity:%s%s%s%s%s%s%s",
+             w & BW_JW_FULL_TABLE ? " key table full (raise capacity_hint);" : "",
+             w & BW_JW_FULL_WINDOWS ? " a key needs more than max_windows_per_key open windows;" : "",
+             w & BW_JW_FULL_EMIT ? " more than max_emit_rows closed windows since the last advance;" : "",
+             w & BW_JW_FULL_LATE ? " more than max_late_rows late rows since the last advance;" : "",
+             w & BW_JW_FULL_QUEUE ? " more than max_queued_rows queued entries;" : "",
+             w & BW_CW_FULL_STORE ? " entry store or staging buffer full;" : "", w ? "" : " (no reason recorded)");
+  }
+  const u64 nr = j->h_cnt[2];
+  j->outstanding -= std::min(nr, j->outstanding);
+  if (nr) {
+    const size_t at = j->released.size();
+    j->released.resize(at + nr);
+    CU(ctx, cudaMemcpyAsync(j->released.data() + at, j->e.rel, nr * 8, cudaMemcpyDeviceToHost, j->s));
+  }
+  if (j->spec.ordered) j->nq = j->h_cnt[3];
+  j->n_rows = j->h_cnt[0];
+  j->dead += j->h_cnt[4] - j->n_stage;  // every staged handle left a dead entry behind
+  j->n_stage = j->h_cnt[4];
+  j->n_store = j->h_cnt[5];
+  CU(ctx, cudaMemsetAsync(j->d_cnt + 2, 0, 16, j->s));
+  CU(ctx, cudaStreamSynchronize(j->s));
+  j->undrained = false;
+  return BW_OK;
+}
+
+// a device buffer of `cap` elements, the first `used` of them kept, regrown to `grow` (nothing on the stream reads it)
+template <class T>
+static cudaError_t collect_grow_keep(bw_collect* j, T** p, u64 used, u64 grow) {
+  T* q = nullptr;
+  cudaError_t e = j->own.dev(&q, grow);
+  if (!e && used) e = cudaMemcpyAsync(q, *p, used * sizeof(T), cudaMemcpyDeviceToDevice, j->s);
+  if (!e) e = cudaStreamSynchronize(j->s);
+  if (e) {
+    j->own.release(q);
+    return e;
+  }
+  j->own.release(*p);
+  *p = q;
+  return cudaSuccess;
+}
+
+// Before a call that can play `values` values (its rows, and ordered the queued entries): compact the store once dead
+// entries outnumber live ones, then grow the store, the staging buffer and the release buffer so that nothing the call
+// can add or close overflows them.  Called after collect_drain: nothing on the stream reads them.
+static bw_status collect_room(bw_collect* j, u64 rows) {
+  bw_ctx* ctx = j->ctx;
+  CwStore& es = j->es;
+  CwEmit& e = j->e;
+  bw_status st = jwin_room(j, rows);
+  if (st != BW_OK) return st;
+  if (j->dead && j->dead >= j->n_store - j->dead) {  // stream compaction (entry order does not matter: each has its rank)
+    const int grid = ctx->sm_count * 4;
+    k_cwin_live<<<grid, 256, 0, j->s>>>(es.ref, j->d_flag, j->n_store);
+    size_t b = 0;
+    CU(ctx, cub::DeviceSelect::Flagged(nullptr, b, es.ref, j->d_flag, es.n, (int64_t)j->n_store, j->s));
+    CU(ctx, j->srt.grow_cub(j->own, b + 256));
+    for (int c = 0; c < 3; ++c) {
+      size_t tb = j->srt.cub_bytes;
+      if (c == 0) CU(ctx, cub::DeviceSelect::Flagged(j->srt.cub, tb, es.h, j->d_flag, es.n, (int64_t)j->n_store, j->s));
+      if (c == 1) CU(ctx, cub::DeviceSelect::Flagged(j->srt.cub, tb, es.rank, j->d_flag, es.n, (int64_t)j->n_store, j->s));
+      if (c == 2) CU(ctx, cub::DeviceSelect::Flagged(j->srt.cub, tb, es.ref, j->d_flag, es.n, (int64_t)j->n_store, j->s));
+    }
+    CU(ctx, cudaGetLastError());
+    j->n_store -= j->dead;
+    j->dead = 0;
+  }
+  const u64 adds = (rows + (j->spec.ordered ? j->nq : 0)) * j->kmax;
+  const u64 live = j->n_store - j->dead;
+  if (j->n_store + adds > es.cap) {
+    const u64 grow = std::max<u64>(j->n_store + adds, 2 * es.cap);
+    es.cap = 0;  // (a failed regrow leaves the store unusable: the next call fails here again)
+    CU(ctx, collect_grow_keep(j, &es.ref, j->n_store, grow));
+    CU(ctx, collect_grow_keep(j, &es.rank, j->n_store, grow));
+    CU(ctx, collect_grow_keep(j, &es.h, j->n_store, grow));
+    CU(ctx, j->own.regrow(Owner::DEV, &j->d_flag, grow));
+    es.cap = grow;
+  }
+  if (j->n_stage + live + adds > e.max_stage) {
+    const u64 grow = std::max<u64>(j->n_stage + live + adds, 2 * e.max_stage);
+    e.max_stage = 0;
+    CU(ctx, collect_grow_keep(j, &e.stage, j->n_stage, grow));
+    CU(ctx, collect_grow_keep(j, &e.stage_rec, j->n_stage, grow));
+    e.max_stage = grow;
+  }
+  return BW_OK;
+}
+
+// after the per-key kernels of a call: move the closed windows' entries out (k_cwin_gather)
+static bw_status collect_gather(bw_collect* j, const JwParams& p) {
+  k_cwin_gather<<<j->ctx->sm_count * 8, 256, 0, j->s>>>(j->t, j->e, j->es, p, j->n_rows);
+  CU(j->ctx, cudaGetLastError());
+  return BW_OK;
+}
+
+// ordered mode: sort the pool's due entries into play order (K8's sort), then flush every woken key (k_cwin_flush)
+static bw_status collect_flush(bw_collect* j, const JwParams& p, u64 n) {
+  bw_ctx* ctx = j->ctx;
+  bw_status st = j->spec.ordered ? jwin_sort_pool(j, j->t.j, p, n) : BW_OK;
+  if (st != BW_OK) return st;
+  CwEmit e = j->e;
+  e.next = j->pool2;
+  k_cwin_flush<<<ctx->sm_count * 8, 256, 0, j->s>>>(j->t, e, j->es, p, j->pool, j->srt.perm);
+  CU(ctx, cudaGetLastError());
+  if (j->spec.ordered) std::swap(j->pool, j->pool2);  // the next call reads what this flush carried over (count: collect_drain)
+  return collect_gather(j, p);
+}
+
+bw_status bw_collect_apply_device(bw_collect* j, const uint64_t* d_keys, const uint64_t* d_handles, const int64_t* d_ts_us, uint64_t rows,
+                                  uint64_t epoch, int64_t system_now_us) {
+  if (!j) return BW_ERR_SPEC;
+  bw_ctx* ctx = j->ctx;
+  COLLECT_REFUSE_FAILED(j);
+  if (rows > j->spec.max_batch_rows) CTX_FAIL(ctx, BW_ERR_SPEC, "windowed collect: rows > max_batch_rows");
+  if (rows && (!d_keys || !d_handles || !d_ts_us)) CTX_FAIL(ctx, BW_ERR_SPEC, "windowed collect: NULL column");
+  if (j->batch_no && epoch < j->last_epoch) CTX_FAIL(ctx, BW_ERR_STATE, "windowed collect: epochs must not decrease");
+  CU(ctx, cudaSetDevice(ctx->device));
+  bw_status st = collect_drain(j);
+  if (st != BW_OK) return st;
+  j->last_epoch = epoch;
+  if (system_now_us > j->now) j->now = system_now_us;  // `now_getter()` never goes backwards (windowing.py:250-261)
+  const JwParams p = collect_params(j, epoch);
+  j->batch_no++;
+  if (rows == 0) return BW_OK;
+  if ((st = collect_room(j, rows)) != BW_OK) return st;
+  j->outstanding += rows;
+  st = keyed_group(ctx, j->k, d_keys, rows, j->s);
+  if (st != BW_OK) return st;
+  k_cwin_apply<<<ctx->sm_count * 8, 256, 0, j->s>>>(j->t, j->e, j->es, p, j->pool, j->nq, j->k.d_ksorted, j->k.d_isorted, j->k.d_head,
+                                                    d_handles, d_ts_us, j->d_late, rows);
+  CU(ctx, cudaGetLastError());
+  j->undrained = true;
+  if (j->spec.ordered) return collect_flush(j, p, j->nq + rows);
+  return collect_gather(j, p);
+}
+
+bw_status bw_collect_apply(bw_collect* j, const uint64_t* keys, const uint64_t* handles, const int64_t* ts_us, uint64_t rows, uint64_t epoch,
+                           int64_t system_now_us) {
+  if (!j) return BW_ERR_SPEC;
+  bw_ctx* ctx = j->ctx;
+  if (rows > j->spec.max_batch_rows) CTX_FAIL(ctx, BW_ERR_SPEC, "windowed collect: rows > max_batch_rows");
+  if (rows && (!keys || !handles || !ts_us)) CTX_FAIL(ctx, BW_ERR_SPEC, "windowed collect: NULL column");
+  CU(ctx, cudaSetDevice(ctx->device));
+  bw_status st = collect_drain(j);
+  if (st != BW_OK) return st;
+  if (rows) {
+    CU(ctx, cudaMemcpyAsync(j->k.d_keys, keys, rows * 8, cudaMemcpyHostToDevice, j->s));
+    CU(ctx, cudaMemcpyAsync(j->d_handles, handles, rows * 8, cudaMemcpyHostToDevice, j->s));
+    CU(ctx, cudaMemcpyAsync(j->d_ts, ts_us, rows * 8, cudaMemcpyHostToDevice, j->s));
+  }
+  st = bw_collect_apply_device(j, j->k.d_keys, j->d_handles, j->d_ts, rows, epoch, system_now_us);
+  if (st != BW_OK) return st;
+  // the host columns may be reused by the caller once this returns
+  return collect_drain(j);
+}
+
+static bw_status collect_collect(bw_collect* j, bw_collect_rows* out) {
+  bw_ctx* ctx = j->ctx;
+  bw_status st = collect_drain(j);
+  if (st != BW_OK) return st;
+  CU(ctx, cudaMemcpyAsync(j->h_cnt, j->d_cnt, 48, cudaMemcpyDeviceToHost, j->s));
+  CU(ctx, cudaStreamSynchronize(j->s));
+  const u64 nd = j->h_cnt[0], nl = j->h_cnt[1], ns = j->h_cnt[4];  // all within bounds: collect_drain passed
+  const CwEmit& e = j->e;
+  if (ns > j->out_cap) {
+    j->out_cap = 0;
+    CU(ctx, j->own.regrow(Owner::DEV, &j->d_out, ns));
+    CU(ctx, j->own.regrow(Owner::HOST, &j->h_out, ns));
+    j->out_cap = ns;
+  }
+  const u64* down[] = {e.key, e.wid, e.epoch};
+  const u64* late[] = {e.l_key, e.l_wid, e.l_epoch, e.l_act, e.l_row};
+  if ((st = jwin_ship(j, nd, e.key, e.seq, e.ord, down, 3, &j->hd)) != BW_OK) return st;
+  if (nd) {  // the lists in the closed windows' order: offsets by a scan of their counts, then every handle in parallel
+    const int grid = ctx->sm_count * 4;
+    SortScratch& x = j->srt;
+    k_cwin_order<<<grid, 256, 0, j->s>>>(x.perm, e.cnt, j->d_inv, j->d_cs, nd);
+    CU(ctx, cudaMemsetAsync(j->d_cs + nd, 0, 8, j->s));
+    size_t tb = x.cub_bytes;
+    CU(ctx, cub::DeviceScan::ExclusiveSum(x.cub, tb, j->d_cs, j->d_off, (int)(nd + 1), j->s));
+    k_cwin_place<<<ctx->sm_count * 8, 256, 0, j->s>>>(e.stage, e.stage_rec, e.soff, j->d_inv, j->d_off, j->d_out, ns);
+    CU(ctx, cudaMemcpyAsync(j->hd.col[3], j->d_off, (nd + 1) * 8, cudaMemcpyDeviceToHost, j->s));
+    if (ns) CU(ctx, cudaMemcpyAsync(j->h_out, j->d_out, ns * 8, cudaMemcpyDeviceToHost, j->s));
+  } else {
+    j->hd.col[3][0] = 0;
+  }
+  if ((st = jwin_ship(j, nl, e.l_key, e.l_seq, e.l_ord, late, 5, &j->hl)) != BW_OK) return st;
+  CU(ctx, cudaGetLastError());
+  CU(ctx, cudaMemsetAsync(j->d_cnt, 0, 16, j->s));
+  CU(ctx, cudaMemsetAsync(j->d_cnt + 4, 0, 8, j->s));
+  CU(ctx, cudaStreamSynchronize(j->s));
+  j->n_rows = j->n_stage = 0;
+  j->first_call = j->calls;
+  out->n_down = nd;
+  out->down_key = j->hd.col[0];
+  out->down_window_id = (const int64_t*)j->hd.col[1];
+  out->down_epoch = j->hd.col[2];
+  out->down_offset = j->hd.col[3];
+  out->handle = j->h_out;
+  out->n_late = nl;
+  out->late_key = j->hl.col[0];
+  out->late_window_id = (const int64_t*)j->hl.col[1];
+  out->late_epoch = j->hl.col[2];
+  out->late_activation = j->hl.col[3];
+  out->late_row = j->hl.col[4];
+  // handed out until the next advance / eof, then cleared
+  j->released.swap(j->released_out);
+  j->released.clear();
+  out->n_released = j->released_out.size();
+  out->released = j->released_out.data();
+  return BW_OK;
+}
+
+// notify phase or EOF: wake the keys (K8's k_jwin_mark), then flush them (ordered: through the pool)
+static bw_status collect_wake(bw_collect* j, int eof) {
+  bw_ctx* ctx = j->ctx;
+  bw_status st = collect_drain(j);
+  if (st != BW_OK) return st;
+  if ((st = collect_room(j, 0)) != BW_OK) return st;
+  const JwParams p = collect_params(j, j->last_epoch);
+  k_jwin_mark<<<ctx->sm_count * 8, 256, 0, j->s>>>(j->t.j, j->t.win, p, eof);
+  CU(ctx, cudaGetLastError());
+  j->undrained = true;
+  return collect_flush(j, p, j->nq);
+}
+
+bw_status bw_collect_advance(bw_collect* j, int64_t system_now_us, bw_collect_rows* out) {
+  if (!j || !out) return BW_ERR_SPEC;
+  bw_ctx* ctx = j->ctx;
+  COLLECT_REFUSE_FAILED(j);
+  CU(ctx, cudaSetDevice(ctx->device));
+  if (system_now_us > 0) {
+    if (system_now_us > j->now) j->now = system_now_us;
+    bw_status st = collect_wake(j, 0);
+    if (st != BW_OK) return st;
+  }
+  return collect_collect(j, out);
+}
+
+bw_status bw_collect_eof(bw_collect* j, bw_collect_rows* out) {
+  if (!j || !out) return BW_ERR_SPEC;
+  bw_ctx* ctx = j->ctx;
+  COLLECT_REFUSE_FAILED(j);
+  CU(ctx, cudaSetDevice(ctx->device));
+  bw_status st = collect_wake(j, 1);
+  if (st != BW_OK) return st;
+  return collect_collect(j, out);
 }

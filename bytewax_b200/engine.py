@@ -459,16 +459,111 @@ class _GpuJoinWindowStep(_GpuWindowStep):
         return rows
 
 
+class _GpuCollectWindowStep(_GpuJoinWindowStep):
+    """One worker's ``collect_window`` (``GpuCollectWindowPlan``) on ``bw_collect_*`` (K9): `_WindowLogic` over a tumbling
+    or sliding windower with the collect folder per window (windowing.py:1046-1190, 1356-1384, 1436-1576), one call per
+    activation.  Handles, clock sampling, notify, EOF and the key re-sort are the join step's; each window's container is
+    built here from its handles in play order, with the reference's own folder calls (`append`, `add`, ``d[k] = v``)."""
+
+    def on_epoch(self, epoch: int, items: list) -> list:
+        from bytewax_b200 import gpu
+
+        np, plan = self.np, self.plan
+        getter = getattr(plan.clock, "ts_getter", None)
+        now = self._now_us()
+        if getter is None:  # SystemClock (windowing.py:196-222): an item's timestamp is the system time of its batch
+            now_dt = _dt(now)
+            getter = lambda _v: now_dt  # noqa: E731
+        keys, handles, ts, vals = [], [], [], []
+        for item in items:
+            key, value = _split_item(self.step_id, item)
+            self._check_value(value)
+            keys.append(self._key_id(key))
+            ts.append(_us(getter(value)))
+            vals.append(value)
+        if self.jwin is None:
+            self.jwin = gpu.CollectWindow(
+                _get_gpu_ctx(), plan.ordered, self.length_us, self.offset_us, self.align_us, self.wait_us,
+                capacity_hint=int(os.environ.get("BYTEWAX_B200_KEYS", 1 << 20)), max_windows_per_key=64,
+                max_queued_rows=1 << 22 if plan.ordered else 0, max_batch_rows=int(os.environ.get("BYTEWAX_B200_BATCH", 1 << 22)),
+                max_emit_rows=1 << 22, max_late_rows=1 << 22)
+        for value in vals:
+            h = self.next_handle
+            self.next_handle += 1
+            handles.append(h)
+            self.values[h] = value
+        self.last_epoch = max(epoch, self.last_epoch)
+        self.jwin.apply(np.array(keys, dtype=np.uint64), np.array(handles, dtype=np.uint64), np.array(ts, dtype=np.int64),
+                        self.last_epoch, now or 0)
+        return self._jwin_rows(self.jwin.advance(), vals)
+
+    def _check_value(self, value):
+        # what the folder would reject when it plays the value (windowing.py:1365-1376; `set.add` of an unhashable
+        # value): in the first batch the step goes to the host logic, which raises its own error; later, the same error
+        # is raised here, at ingest
+        try:
+            if self.plan.into is dict:
+                k, _v = value
+                hash(k)
+            elif self.plan.into is set:
+                hash(value)
+        except TypeError as ex:
+            if self.jwin is None:
+                raise _GpuPlanUnfit(f"value {value!r} of type {type(value)!r}") from ex
+            if self.plan.into is dict:
+                raise TypeError(f"step {self.plan.step_id!r} collecting into a `dict` requires `(key, value)` 2-tuple as the values in "
+                                f"the stream; got a {type(value)!r} instead") from ex
+            raise
+        except ValueError as ex:
+            if self.jwin is None:
+                raise _GpuPlanUnfit(f"value {value!r} of type {type(value)!r}") from ex
+            raise
+
+    def _container(self, handles):
+        V, into = self.values, self.plan.into
+        if into is list:
+            return [V[h] for h in handles]
+        if into is set:
+            out = set()
+            for h in handles:
+                out.add(V[h])
+            return out
+        d = {}
+        for h in handles:
+            k, v = V[h]
+            d[k] = v
+        return d
+
+    def _jwin_rows(self, out, vals) -> list:
+        from bytewax_b200.operators.windowing import WindowMetadata
+
+        lates = [(self._key_str(k), w, vals[r]) for k, w, r in zip(out.late_key.tolist(), out.late_window_id.tolist(), out.late_row.tolist())]
+        downs = [(self._key_str(k), w, self._container(hs)) for k, w, hs in zip(out.down_key.tolist(), out.down_window_id.tolist(), out.lists())]
+        if self.resort:  # interned (non-numeric) keys: restore ascending key-string order; stable
+            for rows in (lates, downs):
+                rows.sort(key=lambda r: r[0])
+        rows = [(ks, (w, "L", v)) for ks, w, v in lates]
+        rows.extend((ks, (w, "E", c)) for ks, w, c in downs)
+        for ks, w, _c in downs:
+            o, c = self.jwin.window_bounds(w)
+            rows.append((ks, (w, "M", WindowMetadata(_dt(o), _dt(c)))))
+        for h in out.released.tolist():  # after this call's rows are built: no later row can name these
+            del self.values[h]
+        return rows
+
+
 def _td_us(td: timedelta) -> int:
     return (td.days * 86400 + td.seconds) * 1_000_000 + td.microseconds
 
 
 def _gpu_step_for(step_id: str, plan):
     from bytewax_b200.operators import GpuFinalPlan, GpuJoinPlan, GpuSmapPlan
-    from bytewax_b200.operators.windowing import GpuJoinWindowPlan, SessionWindower
+    from bytewax_b200.operators.windowing import GpuCollectWindowPlan, GpuJoinWindowPlan, SessionWindower
 
     if isinstance(plan, GpuJoinWindowPlan):
         return _GpuJoinWindowStep(step_id, plan)
+    if isinstance(plan, GpuCollectWindowPlan):
+        return _GpuCollectWindowStep(step_id, plan)
     if isinstance(getattr(plan, "windower", None), SessionWindower):
         return _GpuSessionStep(step_id, plan)
     if isinstance(plan, GpuSmapPlan):

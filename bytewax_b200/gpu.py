@@ -627,3 +627,102 @@ class JoinWindow:
         if self.h:
             self.lib.bw_jwin_destroy(self.h)
             self.h = None
+
+
+@dataclass
+class CollectWindowRows:
+    """Rows of one ``CollectWindow.advance`` / ``eof``, each stream in the reference's downstream order, and the handles
+    released since the previous one.  Each down row is a closed window: its list is
+    ``handle[down_offset[i]:down_offset[i + 1]]`` in play order, and its metadata row follows it (``window_bounds``)."""
+
+    down_key: np.ndarray
+    down_window_id: np.ndarray
+    down_epoch: np.ndarray
+    down_offset: np.ndarray  # n_down + 1
+    handle: np.ndarray
+    late_key: np.ndarray
+    late_window_id: np.ndarray
+    late_epoch: np.ndarray
+    late_activation: np.ndarray
+    late_row: np.ndarray
+    released: np.ndarray  # uint64, in no particular order
+
+    def lists(self) -> List[List[int]]:
+        """The handles of every down row, in play order."""
+        h, o = self.handle.tolist(), self.down_offset.tolist()
+        return [h[o[i]:o[i + 1]] for i in range(len(o) - 1)]
+
+
+class CollectWindow:
+    """``collect_window`` over tumbling or sliding windows (``bw_collect``, K9; windowing.py:1046-1190, 1436-1576).
+    Values travel as uint64 handles; the caller keeps the objects, builds each window's container from its handles and
+    may drop each object once its handle comes back in ``released``."""
+
+    def __init__(self, ctx: Context, ordered: bool = True, length_us: int = 10_000_000, offset_us: Optional[int] = None,
+                 align_us: int = 0, wait_us: Optional[int] = 0, capacity_hint: int = 1 << 16, max_windows_per_key: int = 16,
+                 max_queued_rows: int = 1 << 20, max_batch_rows: int = 1 << 20, max_emit_rows: int = 1 << 20,
+                 max_late_rows: int = 1 << 20):
+        """``offset_us=None``: tumbling.  ``wait_us=None``: the watermark never advances on data (``BW_WAIT_FOREVER``)."""
+        self.ctx, self.lib = ctx, ctx.lib
+        s = N.BwCollectSpec()
+        s.struct_size = C.sizeof(N.BwCollectSpec)
+        s.ordered, s.max_windows_per_key = int(ordered), max_windows_per_key
+        s.length_us, s.offset_us, s.align_us = length_us, length_us if offset_us is None else offset_us, align_us
+        s.wait_us = N.BW_WAIT_FOREVER if wait_us is None else wait_us
+        s.capacity_hint, s.max_queued_rows, s.max_batch_rows = capacity_hint, max_queued_rows, max_batch_rows
+        s.max_emit_rows, s.max_late_rows = max_emit_rows, max_late_rows
+        self.spec = s
+        h = C.c_void_p()
+        N.check(self.lib.bw_collect_create(ctx.h, C.byref(s), C.byref(h)), ctx.h)
+        self.h = h
+        self._epoch = 0
+
+    def window_bounds(self, window_id: int):
+        """``(open_us, close_us)`` of a window (windowing.py:620-623)."""
+        o = self.spec.align_us + self.spec.offset_us * window_id
+        return o, o + self.spec.length_us
+
+    def apply(self, keys, handles, ts_us, epoch: Optional[int] = None, system_now_us: int = 0):
+        """One activation from host arrays.  ``system_now_us``: ``now_getter()`` of the activation."""
+        keys = np.ascontiguousarray(keys, dtype=np.uint64)
+        handles = np.ascontiguousarray(handles, dtype=np.uint64)
+        ts = np.ascontiguousarray(ts_us, dtype=np.int64)
+        if epoch is None:
+            self._epoch += 1
+            epoch = self._epoch
+        vp = lambda a: a.ctypes.data_as(C.c_void_p)  # noqa: E731
+        N.check(self.lib.bw_collect_apply(self.h, vp(keys), vp(handles), vp(ts), keys.shape[0], epoch, int(system_now_us)), self.ctx.h)
+
+    def apply_device(self, d_keys: int, d_handles: int, d_ts: int, rows: int, epoch: Optional[int] = None, system_now_us: int = 0):
+        if epoch is None:
+            self._epoch += 1
+            epoch = self._epoch
+        N.check(self.lib.bw_collect_apply_device(self.h, C.c_void_p(d_keys), C.c_void_p(d_handles), C.c_void_p(d_ts), rows, epoch,
+                                                 int(system_now_us)), self.ctx.h)
+
+    def _wrap(self, r: N.BwCollectRows) -> CollectWindowRows:
+        nd, nl, nr = int(r.n_down), int(r.n_late), int(r.n_released)
+
+        def arr(ptr, n, dt=np.uint64):
+            return np.ctypeslib.as_array(ptr, shape=(n,)).view(dt).copy() if n else np.zeros(0, dt)
+
+        off = arr(r.down_offset, nd + 1)
+        return CollectWindowRows(arr(r.down_key, nd), arr(r.down_window_id, nd, np.int64), arr(r.down_epoch, nd), off,
+                                 arr(r.handle, int(off[-1])), arr(r.late_key, nl), arr(r.late_window_id, nl, np.int64),
+                                 arr(r.late_epoch, nl), arr(r.late_activation, nl), arr(r.late_row, nl), arr(r.released, nr))
+
+    def advance(self, system_now_us: int = 0) -> CollectWindowRows:
+        """Rows since the last call; ``system_now_us`` > 0 first runs the notify phase at that system time."""
+        r = N.BwCollectRows()
+        N.check(self.lib.bw_collect_advance(self.h, int(system_now_us), C.byref(r)), self.ctx.h)
+        return self._wrap(r)
+
+    def eof(self) -> CollectWindowRows:
+        r = N.BwCollectRows()
+        N.check(self.lib.bw_collect_eof(self.h, C.byref(r)), self.ctx.h)
+        return self._wrap(r)
+
+    def close(self):
+        if self.h:
+            self.lib.bw_collect_destroy(self.h)
+            self.h = None

@@ -733,7 +733,34 @@ def collect_window(step_id: str, up: KeyedStream, clock: Clock, windower: Window
         folder, merger = _collect_dict_folder, _collect_dict_merger
     else:
         raise TypeError(f"`collect_window` doesn't support `{into:!}`; only `set`, `list`, and `dict`; use `fold_window` directly")
-    return fold_window("fold_window", up, clock, windower, into, folder, merger, ordered)
+    return fold_window("fold_window", up, clock, windower, into, folder, merger, ordered,
+                       _gpu_plan=_collect_window_plan(step_id, clock, windower, into, ordered))
+
+
+@dataclass(frozen=True)
+class GpuCollectWindowPlan:
+    """A ``collect_window`` the engine may run with ``bw_collect_*`` (K9): ``into`` exactly `list`, `set` or `dict`, a
+    tumbling or sliding windower, and an `EventClock` with an identity ``to_system_utc`` or a `SystemClock`.  Values travel
+    as handles into a host-side dict; each window's container is built from its handles in play order."""
+
+    into: type
+    ordered: bool
+    clock: Any
+    windower: Any
+    step_id: str = ""  # the `collect_window` step id, for the reference's `dict` error message
+
+
+def _collect_window_plan(step_id, clock, windower, into, ordered) -> Optional[GpuCollectWindowPlan]:
+    # the reference builds the plain type even for a subclass `into` (windowing.py:1356-1384) while this mirror builds
+    # `into` itself: a subclass stays on the host engine.  Session windows merge, and a custom `to_system_utc` moves the
+    # notify time away from the event time the device compares with the system clock (windowing.py:1177-1178).
+    if into not in (list, set, dict):
+        return None
+    if not isinstance(windower, (SlidingWindower, TumblingWindower)):
+        return None
+    if not (isinstance(clock, SystemClock) or (isinstance(clock, EventClock) and clock.to_system_utc is _identity)):
+        return None
+    return GpuCollectWindowPlan(into, bool(ordered), clock, windower, step_id)
 
 
 @dataclass

@@ -513,6 +513,79 @@ bw_status bw_jwin_advance(bw_jwin* j, int64_t system_now_us, bw_jwin_rows* out);
 /* End of input: every key flushes at watermark UTC_MAX (:1144-1151). */
 bw_status bw_jwin_eof(bw_jwin* j, bw_jwin_rows* out);
 
+/* Windowed collect (K9): `collect_window` (pysrc/bytewax/operators/windowing.py:1436-1576) into list / set / dict,
+ * i.e. `_WindowLogic` (:1046-1190) over `_SlidingWindowerLogic` (:603-668; tumbling == offset equal to length,
+ * :921-926) with `_FoldWindowLogic` per window and the collect callbacks (:1356-1384), whose state is the window's
+ * values in play order.  Values travel as u64 handles (any u64: none is reserved); the objects stay with the caller,
+ * which builds each container from the window's handles -- `into()`, then `append` / `add` / `d[k] = v` per handle in
+ * order, exactly the reference's folder calls.  Per key, per call, in order: the EventClock's late test per item
+ * (:263-287; a late item gives one row per id of `intersects(ts)`, ascending, :611-618, :636-637, :1125-1127, and is not
+ * queued); `_flush_queue` (:1095-1108) at the watermark after the key's last item: unordered, every queued entry in
+ * arrival order; ordered, the entries with ts <= watermark, stably sorted by ts, the rest kept queued in their order
+ * across calls; each due value joins every window of `open_for(ts)` in ascending id (:626-633, :1064-1077; a window is
+ * opened on its first value); then `_handle_closed` (:1087-1093): windows with close <= watermark in first-opened order,
+ * each giving its list and then its metadata row.  A key with no open window and an empty queue is discarded, clock
+ * state included (:1110-1113, src/operators.rs:796-799).  One GPU only. */
+typedef struct bw_collect bw_collect;
+typedef struct bw_collect_spec {
+  uint32_t struct_size;
+  int32_t ordered;              /* 1: play values in timestamp order once the watermark passes them (the default) */
+  int32_t max_windows_per_key;  /* 1..64 open windows per key */
+  int32_t pad;
+  int64_t length_us;            /* window length, > 0 */
+  int64_t offset_us;            /* 0 < offset <= length (TumblingWindower: == length) */
+  int64_t align_us;             /* align_to */
+  int64_t wait_us;              /* EventClock.wait_for_system_duration, or BW_WAIT_FOREVER */
+  uint64_t capacity_hint;       /* live keys; a key's slot is kept once seen */
+  uint64_t max_queued_rows;     /* ordered mode: queued entries over ALL keys */
+  uint64_t max_batch_rows;
+  uint64_t max_emit_rows;       /* closed windows retained between bw_collect_advance calls */
+  uint64_t max_late_rows;       /* late rows retained between bw_collect_advance calls */
+} bw_collect_spec;
+/* Rows handed downstream since the last advance / eof, in the reference's order: per call (activation, notify phase
+ * or EOF), ascending key string (src/operators.rs:758-767, :862-894); within a key `down` rows in first-opened order,
+ * `late` rows in arrival order (one per window id, ascending).  Each down row is one closed window: its `E` row is the
+ * list handle[down_offset[i] .. down_offset[i + 1]) (play order), and its `M` row, which follows it, is
+ * WindowMetadata(align + id * offset, + length) -- so no separate meta columns.  Host pointers into memory owned by the
+ * library, valid until the next advance / eof / destroy. */
+typedef struct bw_collect_rows {
+  uint64_t n_down;
+  const uint64_t* down_key;
+  const int64_t* down_window_id;
+  const uint64_t* down_epoch;
+  const uint64_t* down_offset;     /* n_down + 1 entries */
+  const uint64_t* handle;          /* down_offset[n_down] entries */
+  uint64_t n_late;
+  const uint64_t* late_key;
+  const int64_t* late_window_id;
+  const uint64_t* late_epoch;
+  const uint64_t* late_activation; /* (activation, row) name the input row (activations counted from 0) */
+  const uint64_t* late_row;
+  /* handles no window and no queue entry holds any more: each handle passed to apply is listed exactly once, in the
+   * rows of the call that closes the last window holding it (its highest id of `open_for(ts)`: a key's windows close
+   * in id order), a late item's in the call that received it */
+  uint64_t n_released;
+  const uint64_t* released;
+} bw_collect_rows;
+bw_status bw_collect_create(bw_ctx* ctx, const bw_collect_spec* spec, bw_collect** out);
+void bw_collect_destroy(bw_collect* c);
+/* One activation from HOST columns (keys, handle, ts); blocks.  `system_now_us` is `now_getter()` for this activation
+ * (windowing.py:250-261; it must not go backwards; 0 throughout = a frozen clock).  The entry store, the staging and
+ * output buffers and the release buffer grow before each call to what it can add, so no call fails for lack of room
+ * there; a full key table, window list, queue, late buffer or closed-window buffer returns BW_ERR_CAPACITY (reason in
+ * bw_last_error) and the collect refuses further calls. */
+bw_status bw_collect_apply(bw_collect* c, const uint64_t* keys, const uint64_t* handles, const int64_t* ts_us, uint64_t rows,
+                           uint64_t epoch, int64_t system_now_us);
+/* Same with DEVICE columns; returns once the work is enqueued (the columns must stay valid until the next call). */
+bw_status bw_collect_apply_device(bw_collect* c, const uint64_t* d_keys, const uint64_t* d_handles, const int64_t* d_ts_us,
+                                  uint64_t rows, uint64_t epoch, int64_t system_now_us);
+/* Rows since the last call.  `system_now_us` > 0 first runs the notify phase at that system time
+ * (src/operators.rs:808-858, windowing.py:1135-1142, 1153-1180 with an identity `to_system_utc`): every key whose
+ * earliest window close -- or, ordered, the ts of its FIRST queued entry -- has been reached flushes at its watermark. */
+bw_status bw_collect_advance(bw_collect* c, int64_t system_now_us, bw_collect_rows* out);
+/* End of input: every key flushes at watermark UTC_MAX (:1144-1151). */
+bw_status bw_collect_eof(bw_collect* c, bw_collect_rows* out);
+
 /* ---- plain device-memory helpers (tests / bench / host bindings without torch) ---- */
 bw_status bw_dev_alloc(bw_ctx* ctx, uint64_t bytes, void** out);
 bw_status bw_dev_free(bw_ctx* ctx, void* ptr);
