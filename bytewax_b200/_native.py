@@ -137,6 +137,24 @@ class BwCollectRows(C.Structure):
                 ("n_released", C.c_uint64), ("released", C.POINTER(C.c_uint64))]
 
 
+class BwSjwinSpec(C.Structure):
+    _fields_ = [("struct_size", C.c_uint32), ("insert_mode", C.c_int32), ("emit_mode", C.c_int32), ("ordered", C.c_int32),
+                ("sides", C.c_int32), ("max_sessions_per_key", C.c_int32), ("gap_us", C.c_int64), ("wait_us", C.c_int64),
+                ("capacity_hint", C.c_uint64), ("max_queued_rows", C.c_uint64), ("max_batch_rows", C.c_uint64),
+                ("max_emit_rows", C.c_uint64), ("max_late_rows", C.c_uint64)]
+
+
+class BwSjwinRows(C.Structure):
+    _fields_ = [("n_down", C.c_uint64), ("down_key", C.POINTER(C.c_uint64)), ("down_window_id", C.POINTER(C.c_int64)),
+                ("down_handle", C.POINTER(C.c_uint64) * 4), ("down_mask", C.POINTER(C.c_uint64)), ("down_epoch", C.POINTER(C.c_uint64)),
+                ("n_meta", C.c_uint64), ("meta_key", C.POINTER(C.c_uint64)), ("meta_window_id", C.POINTER(C.c_int64)),
+                ("meta_open_us", C.POINTER(C.c_int64)), ("meta_close_us", C.POINTER(C.c_int64)), ("meta_epoch", C.POINTER(C.c_uint64)),
+                ("merged_off", C.POINTER(C.c_uint64)), ("merged_ids", C.POINTER(C.c_int64)),
+                ("n_late", C.c_uint64), ("late_key", C.POINTER(C.c_uint64)), ("late_epoch", C.POINTER(C.c_uint64)),
+                ("late_activation", C.POINTER(C.c_uint64)), ("late_row", C.POINTER(C.c_uint64)),
+                ("n_released", C.c_uint64), ("released", C.POINTER(C.c_uint64))]
+
+
 # every symbol include/bwgpu.h declares: (restype, argtypes)
 _P = C.c_void_p
 SYMBOLS = {
@@ -196,6 +214,12 @@ SYMBOLS = {
     "bw_collect_apply_device": (C.c_int32, [_P, _P, _P, _P, C.c_uint64, C.c_uint64, C.c_int64]),
     "bw_collect_advance": (C.c_int32, [_P, C.c_int64, C.POINTER(BwCollectRows)]),
     "bw_collect_eof": (C.c_int32, [_P, C.POINTER(BwCollectRows)]),
+    "bw_sjwin_create": (C.c_int32, [_P, C.POINTER(BwSjwinSpec), C.POINTER(_P)]),
+    "bw_sjwin_destroy": (None, [_P]),
+    "bw_sjwin_apply": (C.c_int32, [_P, _P, _P, _P, _P, C.c_uint64, C.c_uint64, C.c_int64]),
+    "bw_sjwin_apply_device": (C.c_int32, [_P, _P, _P, _P, _P, C.c_uint64, C.c_uint64, C.c_int64]),
+    "bw_sjwin_advance": (C.c_int32, [_P, C.c_int64, C.POINTER(BwSjwinRows)]),
+    "bw_sjwin_eof": (C.c_int32, [_P, C.POINTER(BwSjwinRows)]),
     "bw_dev_alloc": (C.c_int32, [_P, C.c_uint64, C.POINTER(_P)]),
     "bw_dev_free": (C.c_int32, [_P, _P]),
     "bw_host_alloc": (C.c_int32, [_P, C.c_uint64, C.POINTER(_P)]),

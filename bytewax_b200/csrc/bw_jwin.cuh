@@ -378,18 +378,26 @@ __global__ void k_jwin_apply(JwTable t, JwEmit e, JwParams p, JwPool pool, u64 b
   }
 }
 
+// notify_at of the sliding windower's keys (the default of k_jwin_mark)
+struct JwNotifyAt {
+  template <class W>
+  __device__ __forceinline__ i64 operator()(const JwParams& p, const JwState& st, const W* Ws) const {
+    return bw_jw_notify_at(p, st, Ws);
+  }
+};
+
 // notify (src/operators.rs:808-858): keys whose notify_at has come, at the watermark `on_notify` sees (:289-298);
 // EOF (:862-894, windowing.py:1144-1151): every key, watermark UTC_MAX
-// (W: the table's window records, JwWin here)
-template <class W>
-__global__ void k_jwin_mark(JwTable t, const W* win, JwParams p, int eof) {
+// (W: the table's window records, JwWin here; N: the windower's notify_at, JwNotifyAt here, SjNotifyAt for sessions)
+template <class W, class N = JwNotifyAt>
+__global__ void k_jwin_mark(JwTable t, const W* win, JwParams p, int eof, N notify_at = N()) {
   for (u64 s = (u64)blockIdx.x * blockDim.x + threadIdx.x; s <= t.cap; s += (u64)gridDim.x * blockDim.x) {
     JwState& st = t.st[s];
     if (!st.init) continue;
     if (eof) {
       st.wm = BW_UTC_MAX_US;
     } else {
-      if (bw_jw_notify_at(p, st, win + s * (u64)t.M) > p.now) continue;
+      if (notify_at(p, st, win + s * (u64)t.M) > p.now) continue;
       st.wm = st.wm_base + (p.now - st.sys_max);
     }
     st.act = p.ord;

@@ -96,43 +96,134 @@ __device__ __forceinline__ u64 bw_sess_merge(const SessParams& p, u64 into, u64 
   return p.red == BW_RED_COUNT ? into + orig : bw_sess_combine(p.red, p.is_f64, into, orig);
 }
 
-// close_for (windowing.py:774-788): live sessions with close < close_after, in id order; E + M rows, merged ids ascending
-__device__ void bw_sess_close(const SessTable& t, const SessEmit& e, u64 key, SessRec* R, i64* MG, u32& n, u32& nm, i64 close_after,
-                              u64 epoch, u64 ord) {
+// ---- the per-key session steps: K10 (bw_sjwin.cuh) walks with all of them, K7 closes and notifies with them -----------
+// R: a session record with `id`, `open` and `close` (SessRec here, SjRec there); MG: the key's (owner id, merged id)
+// pairs.  One thread walks a key; the walk of one call's inserts is SessWalk.
+// (scalars only, so they stay in registers; the merge queue, (orig, into) record indices in discovery order, lives in
+// the caller's local arrays qo / qt of BW_SESS_MAXM entries, passed to the steps that use it)
+struct SessWalk {
+  u32 n, nm;  // records held (live, or merged away in this call), held merged ids
+  u32 nq;     // merge queue entries
+  u64 dead;   // records merged away in this call (bit i = R[i])
+};
+__device__ __forceinline__ void bw_sess_walk_begin(SessWalk& w, u32 n, u32 nm) {
+  w.n = n;
+  w.nm = nm;
+  w.nq = 0;
+  w.dead = 0;
+}
+
+// _session_find_merges, windowing.py:688-715: live records stably sorted by open (ties keep id order), each merged into
+// the running survivor when it opens within gap of the survivor's close; false when the survivors would hold more than
+// M merged ids
+template <class R>
+__device__ __forceinline__ bool bw_sess_find_merges(R* Rs, i64* MG, SessWalk& w, unsigned char* qo, unsigned char* qt, int M, i64 gap) {
+  unsigned char ix[BW_SESS_MAXM];
+  u32 nl = 0;
+  for (u32 i = 0; i < w.n; ++i)
+    if (!(w.dead >> i & 1)) {
+      u32 j = nl++;
+      const i64 op = Rs[i].open;
+      while (j > 0 && Rs[ix[j - 1]].open > op) {
+        ix[j] = ix[j - 1];
+        --j;
+      }
+      ix[j] = (unsigned char)i;
+    }
+  if (nl < 2) return true;
+  u32 last = ix[0];
+  for (u32 j = 1; j < nl; ++j) {
+    const u32 th = ix[j];
+    if (Rs[th].open - Rs[last].close <= gap) {
+      if (Rs[th].close > Rs[last].close) Rs[last].close = Rs[th].close;
+      w.dead |= 1ULL << th;
+      qo[w.nq] = (unsigned char)th;
+      qt[w.nq] = (unsigned char)last;
+      ++w.nq;
+      const i64 gone = Rs[th].id;  // its own merged ids go with it; the survivor gains its id
+      u32 k = 0;
+      for (u32 m = 0; m < w.nm; ++m)
+        if (MG[2 * m] != gone) {
+          MG[2 * k] = MG[2 * m];
+          MG[2 * k + 1] = MG[2 * m + 1];
+          ++k;
+        }
+      w.nm = k;
+      if (w.nm >= (u32)M) return false;
+      MG[2 * w.nm] = Rs[last].id;
+      MG[2 * w.nm + 1] = gone;
+      ++w.nm;
+    } else {
+      last = th;
+    }
+  }
+  return true;
+}
+
+// open_for, windowing.py:731-762: the first live session by id that takes the timestamp (merging after an extension).
+// The index the value goes to -- even if a merge just took that session away (windowing.py:1069-1076) -- or, with
+// `fresh` set, the index of a new record the caller opens there (id max_key + 1, open = close = ts); -1 when the key
+// needs more than M records or merged ids.
+template <class R>
+__device__ __forceinline__ int bw_sess_open_for(R* Rs, i64* MG, SessWalk& w, unsigned char* qo, unsigned char* qt, int M, i64 gap, i64 ts,
+                                                 bool& fresh) {
+  fresh = false;
+  int hit = -1;
+  bool moved = false;
+  for (u32 i = 0; i < w.n; ++i) {
+    if (w.dead >> i & 1) continue;
+    const i64 op = Rs[i].open, cl = Rs[i].close;
+    if (op <= ts && ts <= cl) {
+      hit = (int)i;
+      break;
+    }
+    if (op - ts > 0 && op - ts <= gap) {
+      Rs[i].open = ts;
+      hit = (int)i;
+      moved = true;
+      break;
+    }
+    if (ts - cl > 0 && ts - cl <= gap) {
+      Rs[i].close = ts;
+      hit = (int)i;
+      moved = true;
+      break;
+    }
+  }
+  if (moved) return bw_sess_find_merges(Rs, MG, w, qo, qt, M, gap) ? hit : -1;
+  if (hit >= 0) return hit;
+  if (w.n >= (u32)M) return -1;
+  fresh = true;
+  return (int)w.n++;
+}
+
+// _handle_merged, windowing.py:1079-1085: `on_merge(into, orig)` in discovery order, then the merged-away records leave
+template <class R, class F>
+__device__ __forceinline__ void bw_sess_merge_each(R* Rs, SessWalk& w, const unsigned char* qo, const unsigned char* qt, F&& on_merge) {
+  for (u32 j = 0; j < w.nq; ++j) on_merge(Rs[qt[j]], Rs[qo[j]]);
+  u32 k = 0;
+  for (u32 i = 0; i < w.n; ++i)
+    if (!(w.dead >> i & 1)) Rs[k++] = Rs[i];
+  w.n = k;
+  w.nq = 0;
+  w.dead = 0;
+}
+
+// close_for (windowing.py:774-788): live sessions with close < close_after leave in id order; `on_close(r, cnt)` sees
+// each while its cnt merged ids are still in MG (bw_sess_mids writes them), then they go with it
+template <class R, class F>
+__device__ __forceinline__ void bw_sess_close_each(R* Rs, i64* MG, u32& n, u32& nm, i64 close_after, F&& on_close) {
   u32 w = 0;
   for (u32 i = 0; i < n; ++i) {
-    const SessRec r = R[i];
+    const R r = Rs[i];
     if (!(r.close < close_after)) {
-      R[w++] = r;
+      Rs[w++] = r;
       continue;
     }
     u32 cnt = 0;
     for (u32 j = 0; j < nm; ++j) cnt += MG[2 * j] == r.id;
-    const u64 row = atomicAdd(e.n_rows, 1ULL);
-    const u64 m0 = cnt ? atomicAdd(e.n_mids, (unsigned long long)cnt) : 0;
-    if (row >= e.max_rows || m0 + cnt > e.max_rows) {
-      bw_sess_fail(t, BW_SESS_FULL_EMIT);
-    } else {
-      e.key[row] = key;
-      e.wid[row] = r.id;
-      e.acc[row] = r.acc;
-      e.open[row] = r.open;
-      e.close[row] = r.close;
-      e.epoch[row] = epoch;
-      e.ord[row] = ord;
-      e.moff[row] = m0;
-      e.mcnt[row] = cnt;
-      // ascending: each pass writes the smallest id above the previous one (ids are distinct)
-      i64 prev = -1;
-      for (u32 c = 0; c < cnt; ++c) {
-        i64 best = INT64_MAX;
-        for (u32 j = 0; j < nm; ++j)
-          if (MG[2 * j] == r.id && MG[2 * j + 1] > prev && MG[2 * j + 1] < best) best = MG[2 * j + 1];
-        e.mids[m0 + c] = best;
-        prev = best;
-      }
-    }
-    u32 k = 0;  // the closed session's merged ids go with it
+    on_close(r, cnt);
+    u32 k = 0;
     for (u32 j = 0; j < nm; ++j)
       if (MG[2 * j] != r.id) {
         MG[2 * k] = MG[2 * j];
@@ -144,12 +235,61 @@ __device__ void bw_sess_close(const SessTable& t, const SessEmit& e, u64 key, Se
   n = w;
 }
 
+// the cnt merged ids of session `id`, ascending: each pass writes the smallest id above the previous one (ids are distinct)
+__device__ __forceinline__ void bw_sess_mids(const i64* MG, u32 nm, i64 id, u32 cnt, i64* out) {
+  i64 prev = -1;
+  for (u32 c = 0; c < cnt; ++c) {
+    i64 best = INT64_MAX;
+    for (u32 j = 0; j < nm; ++j)
+      if (MG[2 * j] == id && MG[2 * j + 1] > prev && MG[2 * j + 1] < best) best = MG[2 * j + 1];
+    out[c] = best;
+    prev = best;
+  }
+}
+
 __device__ __forceinline__ i64 bw_sess_close_after(i64 watermark, i64 gap) {
   const i64 c = watermark - gap;  // watermark >= UTC_MIN and gap <= UTC_MAX - UTC_MIN: no overflow
   return c < BW_UTC_MIN_US ? BW_UTC_MIN_US : c;
 }
 
-// one thread per key segment: the key's items of this activation in arrival order
+// notify_at of the session windower (windowing.py:790-796) is min(close) + gap: true when it has come by `now`
+template <class R>
+__device__ __forceinline__ bool bw_sess_due(const R* Rs, u32 n, i64 gap, i64 now) {
+  if (n == 0) return false;
+  i64 mc = Rs[0].close;
+  for (u32 i = 1; i < n; ++i) mc = Rs[i].close < mc ? Rs[i].close : mc;
+  return mc <= now - gap;
+}
+
+// ---- K7 --------------------------------------------------------------------------------------------------------------
+// close_for with K7's rows: E + M rows, merged ids ascending
+__device__ void bw_sess_close(const SessTable& t, const SessEmit& e, u64 key, SessRec* R, i64* MG, u32& n, u32& nm, i64 close_after,
+                              u64 epoch, u64 ord) {
+  bw_sess_close_each(R, MG, n, nm, close_after, [&](const SessRec& r, u32 cnt) {
+    const u64 row = atomicAdd(e.n_rows, 1ULL);
+    const u64 m0 = cnt ? atomicAdd(e.n_mids, (unsigned long long)cnt) : 0;
+    if (row >= e.max_rows || m0 + cnt > e.max_rows) {
+      bw_sess_fail(t, BW_SESS_FULL_EMIT);
+      return;
+    }
+    e.key[row] = key;
+    e.wid[row] = r.id;
+    e.acc[row] = r.acc;
+    e.open[row] = r.open;
+    e.close[row] = r.close;
+    e.epoch[row] = epoch;
+    e.ord[row] = ord;
+    e.moff[row] = m0;
+    e.mcnt[row] = cnt;
+    bw_sess_mids(MG, nm, r.id, cnt, e.mids + m0);
+  });
+}
+
+// one thread per key segment: the key's items of this activation in arrival order.  The walk restates open_for and
+// _session_find_merges inline rather than through bw_sess_open_for / bw_sess_merge_each: routed through them, this kernel
+// compiled to a different layout and ran ~5% slower in tools/bench_sessions.py on an H100 80GB HBM3 at a 700 W power
+// limit (5.34 vs 5.08 ms per activation, three alternating runs each).  The two must agree; K10's goldens and K7's both
+// pin them to the reference.
 __global__ void k_session_apply(SessTable t, SessEmit e, SessParams p, const u64* ksorted, const u32* isorted, const u32* headpos,
                                 const u64* vals, const i64* ts_us, u64 n) {
   const int M = t.M;
@@ -318,9 +458,7 @@ __global__ void k_session_close_all(SessTable t, SessEmit e, SessParams p, int e
     SessRec* R = t.rec + s * (u64)t.M;
     i64 wm = BW_UTC_MAX_US;
     if (!eof) {
-      i64 mc = R[0].close;
-      for (u32 i = 1; i < st.n; ++i) mc = R[i].close < mc ? R[i].close : mc;
-      if (mc > p.now - p.gap) continue;
+      if (!bw_sess_due(R, st.n, p.gap, p.now)) continue;
       wm = st.wm_base + (p.now - st.sys_max);
     }
     u32 n_rec = st.n, nm = st.nm;

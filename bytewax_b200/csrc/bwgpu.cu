@@ -37,6 +37,7 @@
 #include "bw_session.cuh"
 #include "bw_jwin.cuh"
 #include "bw_collect.cuh"
+#include "bw_sjwin.cuh"
 #include "bw_prepass.cuh"
 #include "bw_slow.cuh"
 #include "bw_late.cuh"
@@ -3111,23 +3112,31 @@ static JwParams jwin_params(bw_jwin* j, u64 epoch) {
 #define JWIN_REFUSE_FAILED(j) \
   if ((j)->failed) CTX_FAIL((j)->ctx, BW_ERR_STATE, "windowed join: an earlier call failed on the device; the join is unusable")
 
+// What differs between the handle joins that share the host steps below (J: bw_jwin, K8; bw_sjwin, K10, whose overloads
+// follow its struct): the name in messages, what BW_JW_FULL_WINDOWS / BW_JW_FULL_EMIT mean, the device counters.
+static const char* jwin_what(const bw_jwin*) { return "windowed join"; }
+static const char* jwin_full_windows(const bw_jwin*) { return " a key needs more than max_windows_per_key open windows;"; }
+static const char* jwin_full_emit(const bw_jwin*) { return " more than max_emit_rows down or meta rows since the last advance;"; }
+static u64 jwin_counters(const bw_jwin*) { return 5; }  // down, meta, late, released, carried-over queue entries
+
 // wait for the last call; fail on a device-side overflow; then take its released handles and its queue count, so the
 // device buffer only ever holds one call's releases
-static bw_status jwin_drain(bw_jwin* j) {
+template <class J>
+static bw_status jwin_drain(J* j) {
   bw_ctx* ctx = j->ctx;
-  JWIN_REFUSE_FAILED(j);
+  if (j->failed) CTX_FAIL(ctx, BW_ERR_STATE, "%s: an earlier call failed on the device; the join is unusable", jwin_what(j));
   if (!j->undrained) return BW_OK;
   CU(ctx, cudaMemcpyAsync(j->h_err, j->t.err, 8, cudaMemcpyDeviceToHost, j->s));
-  CU(ctx, cudaMemcpyAsync(j->h_cnt, j->d_cnt, 40, cudaMemcpyDeviceToHost, j->s));
+  CU(ctx, cudaMemcpyAsync(j->h_cnt, j->d_cnt, 8 * jwin_counters(j), cudaMemcpyDeviceToHost, j->s));
   CU(ctx, cudaStreamSynchronize(j->s));
   if (j->h_err[0]) {
     j->failed = true;
     const u32 w = j->h_err[1];
-    CTX_FAIL(ctx, (bw_status)j->h_err[0], "windowed join kernel %s:%s%s%s%s%s%s%s",
+    CTX_FAIL(ctx, (bw_status)j->h_err[0], "%s kernel %s:%s%s%s%s%s%s%s", jwin_what(j),
              j->h_err[0] == BW_ERR_SPEC ? "rejected its input" : "ran out of capacity",
              w & BW_JW_BAD_SIDE ? " a side column value is not below sides;" : "", w & BW_JW_FULL_TABLE ? " key table full (raise capacity_hint);" : "",
-             w & BW_JW_FULL_WINDOWS ? " a key needs more than max_windows_per_key open windows;" : "",
-             w & BW_JW_FULL_EMIT ? " more than max_emit_rows down or meta rows since the last advance;" : "",
+             w & BW_JW_FULL_WINDOWS ? jwin_full_windows(j) : "",
+             w & BW_JW_FULL_EMIT ? jwin_full_emit(j) : "",
              w & BW_JW_FULL_LATE ? " more than max_late_rows late rows since the last advance;" : "",
              w & BW_JW_FULL_QUEUE ? " more than max_queued_rows queued entries;" : "", w ? "" : " (no reason recorded)");
   }
@@ -3178,18 +3187,24 @@ static bw_status jwin_sort_pool(J* j, const JwTable& t, const JwParams& p, u64 n
   return BW_OK;
 }
 
-// ordered mode: sort the pool's due entries into play order, then flush every woken key (k_jwin_flush)
-static bw_status jwin_flush_pool(bw_jwin* j, const JwParams& p, u64 n) {
+// ordered mode: sort the pool's due entries into play order, then flush every woken key: `flush(e, perm)` launches the
+// join's flush kernel (k_jwin_flush, k_sjwin_flush) with emit buffers whose carry-over pool is the next one
+template <class J, class F>
+static bw_status jwin_flush_pool(J* j, const JwParams& p, u64 n, F&& flush) {
   bw_ctx* ctx = j->ctx;
-  SortScratch& x = j->srt;
   bw_status st = jwin_sort_pool(j, j->t, p, n);
   if (st != BW_OK) return st;
-  JwEmit e = j->e;
+  auto e = j->e;
   e.next = j->pool2;
-  k_jwin_flush<<<ctx->sm_count * 8, 256, 0, j->s>>>(j->t, e, p, j->pool, x.perm);
+  flush(e, j->srt.perm);
   CU(ctx, cudaGetLastError());
   std::swap(j->pool, j->pool2);  // the next call reads what this flush carried over (count: jwin_drain)
   return BW_OK;
+}
+static bw_status jwin_flush_pool(bw_jwin* j, const JwParams& p, u64 n) {
+  return jwin_flush_pool(j, p, n, [&](const JwEmit& e, const u32* perm) {
+    k_jwin_flush<<<j->ctx->sm_count * 8, 256, 0, j->s>>>(j->t, e, p, j->pool, perm);
+  });
 }
 
 bw_status bw_jwin_apply_device(bw_jwin* j, const uint64_t* d_keys, const uint8_t* d_side, const uint64_t* d_handles, const int64_t* d_ts_us,
@@ -3220,14 +3235,18 @@ bw_status bw_jwin_apply_device(bw_jwin* j, const uint64_t* d_keys, const uint8_t
   return BW_OK;
 }
 
-bw_status bw_jwin_apply(bw_jwin* j, const uint64_t* keys, const uint8_t* side, const uint64_t* handles, const int64_t* ts_us, uint64_t rows,
-                        uint64_t epoch, int64_t system_now_us) {
+// one activation from HOST columns: check the sides, copy the columns to the join's device columns, run `apply_device`,
+// and wait, so the caller may reuse its columns (J: bw_jwin, bw_sjwin)
+template <class J, class D>
+static bw_status jwin_apply_host(J* j, const uint64_t* keys, const uint8_t* side, const uint64_t* handles, const int64_t* ts_us, uint64_t rows,
+                                 uint64_t epoch, int64_t system_now_us, D apply_device) {
   if (!j) return BW_ERR_SPEC;
   bw_ctx* ctx = j->ctx;
-  if (rows > j->spec.max_batch_rows) CTX_FAIL(ctx, BW_ERR_SPEC, "windowed join: rows > max_batch_rows");
-  if (rows && (!keys || !side || !handles || !ts_us)) CTX_FAIL(ctx, BW_ERR_SPEC, "windowed join: NULL column");
+  if (rows > j->spec.max_batch_rows) CTX_FAIL(ctx, BW_ERR_SPEC, "%s: rows > max_batch_rows", jwin_what(j));
+  if (rows && (!keys || !side || !handles || !ts_us)) CTX_FAIL(ctx, BW_ERR_SPEC, "%s: NULL column", jwin_what(j));
   for (u64 i = 0; i < rows; ++i)
-    if (side[i] >= (u32)j->spec.sides) CTX_FAIL(ctx, BW_ERR_SPEC, "windowed join: side %u of row %llu is not below sides", side[i], (unsigned long long)i);
+    if (side[i] >= (u32)j->spec.sides)
+      CTX_FAIL(ctx, BW_ERR_SPEC, "%s: side %u of row %llu is not below sides", jwin_what(j), side[i], (unsigned long long)i);
   CU(ctx, cudaSetDevice(ctx->device));
   bw_status st = jwin_drain(j);
   if (st != BW_OK) return st;
@@ -3237,10 +3256,15 @@ bw_status bw_jwin_apply(bw_jwin* j, const uint64_t* keys, const uint8_t* side, c
     CU(ctx, cudaMemcpyAsync(j->d_handles, handles, rows * 8, cudaMemcpyHostToDevice, j->s));
     CU(ctx, cudaMemcpyAsync(j->d_ts, ts_us, rows * 8, cudaMemcpyHostToDevice, j->s));
   }
-  st = bw_jwin_apply_device(j, j->k.d_keys, j->d_side, j->d_handles, j->d_ts, rows, epoch, system_now_us);
+  st = apply_device(j, j->k.d_keys, j->d_side, j->d_handles, j->d_ts, rows, epoch, system_now_us);
   if (st != BW_OK) return st;
   // the host columns may be reused by the caller once this returns
   return jwin_drain(j);
+}
+
+bw_status bw_jwin_apply(bw_jwin* j, const uint64_t* keys, const uint8_t* side, const uint64_t* handles, const int64_t* ts_us, uint64_t rows,
+                        uint64_t epoch, int64_t system_now_us) {
+  return jwin_apply_host(j, keys, side, handles, ts_us, rows, epoch, system_now_us, bw_jwin_apply_device);
 }
 
 // order rows [0, n) of one stream by (call, key string, seq) and copy `nc` columns to the host (J: bw_jwin, bw_collect)
@@ -3768,4 +3792,296 @@ bw_status bw_collect_eof(bw_collect* j, bw_collect_rows* out) {
   bw_status st = collect_wake(j, 1);
   if (st != BW_OK) return st;
   return collect_collect(j, out);
+}
+
+// ===========================================================================
+// K10 host side: windowed join over session windows (bw_sjwin.cuh)
+// ===========================================================================
+struct bw_sjwin {
+  Owner own;  // every buffer and the stream below
+  bw_ctx* ctx = nullptr;
+  bw_sjwin_spec spec{};
+  SjTable t{};
+  KeyedScratch k;
+  cudaStream_t s = nullptr;
+  u32* h_err = nullptr;                 // err, why
+  unsigned long long* d_cnt = nullptr;  // down, meta, late, released, carried-over queue entries, merged ids
+  unsigned long long* h_cnt = nullptr;
+  unsigned char *d_side = nullptr, *d_late = nullptr;
+  u64* d_handles = nullptr;
+  i64* d_ts = nullptr;
+  SjEmit e{};
+  JwPool pool{}, pool2{};  // ordered mode: the queue, and the one the next flush writes
+  u64 nq = 0;              // entries in `pool`
+  int slot_bits = 1;
+  SortScratch srt;       // pool sort and ordering scratch
+  HostCols hd[2];        // down: key, window id, h0, h1, h2 | h3, mask, epoch
+  HostCols hm[2];        // meta: key, window id, open, close, epoch | merged count, merged offset
+  HostCols hl;           // late: key, window id, epoch, activation, row
+  i64* h_mids = nullptr;
+  std::vector<u64> merged_off;
+  std::vector<i64> merged_ids;
+  std::vector<u64> released;      // since the last advance / eof
+  std::vector<u64> released_out;  // what the last advance / eof handed out
+  bool undrained = false;     // a call whose released handles and queue count are not read back yet
+  u64 outstanding = 0;        // handles passed in and not released yet: what the next call can release, besides its own
+  u32 batch_no = 0;
+  u64 calls = 0, first_call = 0;  // calls (activations, notify phases, EOF) so far; the first not yet collected
+  u64 last_epoch = 0;
+  i64 now = INT64_MIN;
+  bool failed = false;
+};
+
+bw_status bw_sjwin_create(bw_ctx* ctx, const bw_sjwin_spec* spec, bw_sjwin** out) {
+  if (!ctx || !spec || !out) CTX_FAIL(ctx, BW_ERR_SPEC, "bw_sjwin_create: NULL argument");
+  if (spec->struct_size != sizeof(bw_sjwin_spec)) CTX_FAIL(ctx, BW_ERR_SPEC, "bw_sjwin_spec.struct_size mismatch");
+  if (ctx->world != 1) CTX_FAIL(ctx, BW_ERR_SPEC, "session joins run on one GPU (world == 1)");
+  if (spec->insert_mode != BW_JOIN_INSERT_FIRST && spec->insert_mode != BW_JOIN_INSERT_LAST)
+    CTX_FAIL(ctx, BW_ERR_SPEC, "insert_mode must be first or last (product: host engine)");
+  if (spec->emit_mode < BW_JOIN_EMIT_COMPLETE || spec->emit_mode > BW_JOIN_EMIT_RUNNING) CTX_FAIL(ctx, BW_ERR_SPEC, "bad emit_mode");
+  if (spec->ordered != 0 && spec->ordered != 1) CTX_FAIL(ctx, BW_ERR_SPEC, "ordered must be 0 or 1");
+  if (spec->sides < 1 || spec->sides > BW_JW_MAXSIDES) CTX_FAIL(ctx, BW_ERR_SPEC, "sides must be in 1..%d", BW_JW_MAXSIDES);
+  if (spec->max_sessions_per_key < 1 || spec->max_sessions_per_key > BW_SESS_MAXM)
+    CTX_FAIL(ctx, BW_ERR_SPEC, "max_sessions_per_key must be in 1..%d", BW_SESS_MAXM);
+  if (spec->gap_us < 0 || spec->gap_us > BW_UTC_MAX_US - BW_UTC_MIN_US) CTX_FAIL(ctx, BW_ERR_SPEC, "gap_us must be in 0..UTC_MAX - UTC_MIN");
+  if (spec->wait_us < 0) CTX_FAIL(ctx, BW_ERR_SPEC, "wait_us must not be negative");
+  if (spec->max_batch_rows == 0 || spec->max_batch_rows >= (1ULL << 31)) CTX_FAIL(ctx, BW_ERR_SPEC, "bad max_batch_rows");
+  if (spec->max_queued_rows >= (1ULL << 31) - spec->max_batch_rows) CTX_FAIL(ctx, BW_ERR_SPEC, "max_queued_rows + max_batch_rows must stay below 2^31");
+  if (spec->capacity_hint >= (1ULL << 30)) CTX_FAIL(ctx, BW_ERR_SPEC, "capacity_hint must be below 2^30");
+  CU(ctx, cudaSetDevice(ctx->device));
+  std::unique_ptr<bw_sjwin, void (*)(bw_sjwin*)> jp(new bw_sjwin(), bw_sjwin_destroy);  // torn down on every failure
+  bw_sjwin* j = jp.get();
+  Owner& own = j->own;
+  j->ctx = ctx;
+  j->spec = *spec;
+  const u64 cap = std::max<u64>(1024, 2 * std::max<u64>(spec->capacity_hint, 1));
+  const int M = spec->max_sessions_per_key;
+  SjTable& t = j->t;
+  t.cap = cap;
+  t.M = M;
+  t.sides = spec->sides;
+  t.gap = spec->gap_us;
+  while ((1ULL << j->slot_bits) < cap + 1) ++j->slot_bits;
+  CU(ctx, own.stream(&j->s));
+  CU(ctx, own.dev(&t.keys, cap + 1));
+  CU(ctx, own.dev(&t.st, cap + 1));
+  CU(ctx, own.dev(&t.kx, cap + 1));
+  CU(ctx, own.dev(&t.rec, (cap + 1) * (u64)M));
+  CU(ctx, own.dev(&t.mrg, (cap + 1) * (u64)(2 * M)));
+  t.win = nullptr;  // (K8's window records: sessions live in rec)
+  CU(ctx, own.dev(&t.err, 2));
+  t.why = t.err + 1;
+  CU(ctx, own.dev(&j->d_cnt, 6));
+  CU(ctx, cudaMemsetAsync(t.err, 0, 8, j->s));
+  CU(ctx, cudaMemsetAsync(j->d_cnt, 0, 48, j->s));
+  CU(ctx, own.host(&j->h_err, 64 / sizeof(u32)));
+  CU(ctx, own.host(&j->h_cnt, 64 / sizeof(unsigned long long)));
+  const u64 n = spec->max_batch_rows, m = std::max<u64>(spec->max_emit_rows, 1), l = std::max<u64>(spec->max_late_rows, 1);
+  const u64 q = spec->ordered ? spec->max_queued_rows : 0;
+  bw_status st = keyed_alloc(ctx, own, j->k, n, j->s);
+  if (st != BW_OK) return st;
+  CU(ctx, own.dev(&j->d_side, n));
+  CU(ctx, own.dev(&j->d_late, n));
+  CU(ctx, own.dev(&j->d_handles, n));
+  CU(ctx, own.dev(&j->d_ts, n));
+  if (spec->ordered) {
+    if ((st = jwin_pool_alloc(ctx, own, j->pool, q + n)) != BW_OK) return st;
+    if ((st = jwin_pool_alloc(ctx, own, j->pool2, q + n)) != BW_OK) return st;
+  }
+  SjEmit& e = j->e;
+  for (u64** c : {&e.key, &e.wid, &e.h0, &e.h1, &e.h2, &e.h3, &e.mask, &e.epoch, &e.ord, &e.seq}) CU(ctx, own.dev(c, m));
+  for (u64** c : {&e.m_key, &e.m_wid, &e.m_epoch, &e.m_ord, &e.m_seq, &e.m_moff, &e.m_mcnt}) CU(ctx, own.dev(c, m));
+  for (i64** c : {&e.m_open, &e.m_close, &e.mids}) CU(ctx, own.dev(c, m));
+  for (u64** c : {&e.l_key, &e.l_wid, &e.l_epoch, &e.l_act, &e.l_row, &e.l_ord, &e.l_seq}) CU(ctx, own.dev(c, l));
+  // the release buffer grows with the handles held (jwin_room); it starts at one batch
+  e.max_rel = n;
+  CU(ctx, own.dev(&e.rel, e.max_rel));
+  e.max_rows = spec->max_emit_rows;
+  e.max_late = spec->max_late_rows;
+  e.max_queue = q;
+  e.n_rows = j->d_cnt;
+  e.n_meta = j->d_cnt + 1;
+  e.n_late = j->d_cnt + 2;
+  e.n_rel = j->d_cnt + 3;
+  e.n_next = j->d_cnt + 4;
+  e.n_mids = j->d_cnt + 5;
+  const u64 ns = std::max(std::max(m, l), q + n);
+  CU(ctx, j->srt.reserve(own, ns, ns, j->s));
+  CU(ctx, j->hd[0].reserve(own, m, m));
+  CU(ctx, j->hd[1].reserve(own, m, m));
+  CU(ctx, j->hm[0].reserve(own, m, m));
+  CU(ctx, j->hm[1].reserve(own, m, m));
+  CU(ctx, j->hl.reserve(own, l, l));
+  CU(ctx, own.host(&j->h_mids, m));
+  k_sjwin_init<<<ctx->sm_count * 4, 256, 0, j->s>>>(t);
+  CU(ctx, cudaGetLastError());
+  CU(ctx, cudaStreamSynchronize(j->s));
+  *out = jp.release();
+  return BW_OK;
+}
+
+void bw_sjwin_destroy(bw_sjwin* j) {
+  if (!j) return;
+  cudaSetDevice(j->ctx->device);
+  if (j->s) cudaStreamSynchronize(j->s);
+  delete j;  // j->own releases every buffer and the stream
+}
+
+static JwParams sjwin_params(bw_sjwin* j, u64 epoch) {
+  JwParams p{};
+  p.insert_last = j->spec.insert_mode == BW_JOIN_INSERT_LAST;
+  p.emit_mode = j->spec.emit_mode;
+  p.ordered = j->spec.ordered;
+  p.wait = j->spec.wait_us;
+  p.now = j->now;
+  p.epoch = epoch;
+  p.ord = j->calls++;
+  p.batch_no = j->batch_no;
+  return p;
+}
+
+static const char* jwin_what(const bw_sjwin*) { return "session join"; }
+static const char* jwin_full_windows(const bw_sjwin*) { return " a key needs more than max_sessions_per_key sessions or merged ids;"; }
+static const char* jwin_full_emit(const bw_sjwin*) { return " more than max_emit_rows down or meta rows or merged ids since the last advance;"; }
+static u64 jwin_counters(const bw_sjwin*) { return 6; }  // K8's five, then merged ids
+
+#define SJWIN_REFUSE_FAILED(j) \
+  if ((j)->failed) CTX_FAIL((j)->ctx, BW_ERR_STATE, "session join: an earlier call failed on the device; the join is unusable")
+
+// ordered mode: K8's pool sort and flush with the session flush kernel
+static bw_status sjwin_flush_pool(bw_sjwin* j, const JwParams& p, u64 n) {
+  return jwin_flush_pool(j, p, n, [&](const SjEmit& e, const u32* perm) {
+    k_sjwin_flush<<<j->ctx->sm_count * 8, 256, 0, j->s>>>(j->t, e, p, j->pool, perm);
+  });
+}
+
+bw_status bw_sjwin_apply_device(bw_sjwin* j, const uint64_t* d_keys, const uint8_t* d_side, const uint64_t* d_handles, const int64_t* d_ts_us,
+                                uint64_t rows, uint64_t epoch, int64_t system_now_us) {
+  if (!j) return BW_ERR_SPEC;
+  bw_ctx* ctx = j->ctx;
+  SJWIN_REFUSE_FAILED(j);
+  if (rows > j->spec.max_batch_rows) CTX_FAIL(ctx, BW_ERR_SPEC, "session join: rows > max_batch_rows");
+  if (rows && (!d_keys || !d_side || !d_handles || !d_ts_us)) CTX_FAIL(ctx, BW_ERR_SPEC, "session join: NULL column");
+  if (j->batch_no && epoch < j->last_epoch) CTX_FAIL(ctx, BW_ERR_STATE, "session join: epochs must not decrease");
+  CU(ctx, cudaSetDevice(ctx->device));
+  bw_status st = jwin_drain(j);
+  if (st != BW_OK) return st;
+  j->last_epoch = epoch;
+  if (system_now_us > j->now) j->now = system_now_us;  // `now_getter()` never goes backwards (windowing.py:250-261)
+  const JwParams p = sjwin_params(j, epoch);
+  j->batch_no++;
+  if (rows == 0) return BW_OK;
+  if ((st = jwin_room(j, rows)) != BW_OK) return st;
+  j->outstanding += rows;
+  st = keyed_group(ctx, j->k, d_keys, rows, j->s);
+  if (st != BW_OK) return st;
+  k_sjwin_apply<<<ctx->sm_count * 8, 256, 0, j->s>>>(j->t, j->e, p, j->pool, j->nq, j->k.d_ksorted, j->k.d_isorted, j->k.d_head, d_handles,
+                                                     d_side, d_ts_us, j->d_late, rows);
+  CU(ctx, cudaGetLastError());
+  j->undrained = true;
+  if (j->spec.ordered) return sjwin_flush_pool(j, p, j->nq + rows);
+  return BW_OK;
+}
+
+bw_status bw_sjwin_apply(bw_sjwin* j, const uint64_t* keys, const uint8_t* side, const uint64_t* handles, const int64_t* ts_us, uint64_t rows,
+                         uint64_t epoch, int64_t system_now_us) {
+  return jwin_apply_host(j, keys, side, handles, ts_us, rows, epoch, system_now_us, bw_sjwin_apply_device);
+}
+
+static bw_status sjwin_collect(bw_sjwin* j, bw_sjwin_rows* out) {
+  bw_ctx* ctx = j->ctx;
+  bw_status st = jwin_drain(j);
+  if (st != BW_OK) return st;
+  CU(ctx, cudaMemcpyAsync(j->h_cnt, j->d_cnt, 48, cudaMemcpyDeviceToHost, j->s));
+  CU(ctx, cudaStreamSynchronize(j->s));
+  const u64 nd = j->h_cnt[0], nm = j->h_cnt[1], nl = j->h_cnt[2], nmid = j->h_cnt[5];  // all within bounds: jwin_drain passed
+  const SjEmit& e = j->e;
+  const u64* down[] = {e.key, e.wid, e.h0, e.h1, e.h2, e.h3, e.mask, e.epoch};
+  const u64* meta[] = {e.m_key, e.m_wid, (const u64*)e.m_open, (const u64*)e.m_close, e.m_epoch, e.m_mcnt, e.m_moff};
+  const u64* late[] = {e.l_key, e.l_wid, e.l_epoch, e.l_act, e.l_row};
+  if ((st = jwin_ship(j, nd, e.key, e.seq, e.ord, down, 8, j->hd)) != BW_OK) return st;
+  if ((st = jwin_ship(j, nm, e.m_key, e.m_seq, e.m_ord, meta, 7, j->hm)) != BW_OK) return st;
+  if ((st = jwin_ship(j, nl, e.l_key, e.l_seq, e.l_ord, late, 5, &j->hl)) != BW_OK) return st;
+  if (nmid) CU(ctx, cudaMemcpyAsync(j->h_mids, e.mids, nmid * 8, cudaMemcpyDeviceToHost, j->s));
+  CU(ctx, cudaGetLastError());
+  CU(ctx, cudaMemsetAsync(j->d_cnt, 0, 24, j->s));
+  CU(ctx, cudaMemsetAsync(j->d_cnt + 5, 0, 8, j->s));
+  CU(ctx, cudaStreamSynchronize(j->s));
+  // merged ids in meta row order
+  j->merged_off.assign(nm + 1, 0);
+  j->merged_ids.resize(nmid);
+  const u64 *cnt = j->hm[1].col[0], *off = j->hm[1].col[1];
+  for (u64 r = 0; r < nm; ++r) {
+    j->merged_off[r + 1] = j->merged_off[r] + cnt[r];
+    std::copy(j->h_mids + off[r], j->h_mids + off[r] + cnt[r], j->merged_ids.begin() + j->merged_off[r]);
+  }
+  j->first_call = j->calls;
+  out->n_down = nd;
+  out->down_key = j->hd[0].col[0];
+  out->down_window_id = (const int64_t*)j->hd[0].col[1];
+  out->down_handle[0] = j->hd[0].col[2];
+  out->down_handle[1] = j->hd[0].col[3];
+  out->down_handle[2] = j->hd[0].col[4];
+  out->down_handle[3] = j->hd[1].col[0];
+  out->down_mask = j->hd[1].col[1];
+  out->down_epoch = j->hd[1].col[2];
+  out->n_meta = nm;
+  out->meta_key = j->hm[0].col[0];
+  out->meta_window_id = (const int64_t*)j->hm[0].col[1];
+  out->meta_open_us = (const int64_t*)j->hm[0].col[2];
+  out->meta_close_us = (const int64_t*)j->hm[0].col[3];
+  out->meta_epoch = j->hm[0].col[4];
+  out->merged_off = j->merged_off.data();
+  out->merged_ids = j->merged_ids.data();
+  out->n_late = nl;
+  out->late_key = j->hl.col[0];
+  out->late_epoch = j->hl.col[2];
+  out->late_activation = j->hl.col[3];
+  out->late_row = j->hl.col[4];
+  // handed out until the next advance / eof, then cleared
+  j->released.swap(j->released_out);
+  j->released.clear();
+  out->n_released = j->released_out.size();
+  out->released = j->released_out.data();
+  return BW_OK;
+}
+
+// notify phase or EOF: wake the keys (K8's k_jwin_mark with the session notify_at), then flush them (ordered: through
+// the pool)
+static bw_status sjwin_wake(bw_sjwin* j, int eof) {
+  bw_ctx* ctx = j->ctx;
+  bw_status st = jwin_drain(j);
+  if (st != BW_OK) return st;
+  if ((st = jwin_room(j, 0)) != BW_OK) return st;
+  const JwParams p = sjwin_params(j, j->last_epoch);
+  k_jwin_mark<<<ctx->sm_count * 8, 256, 0, j->s>>>((const JwTable&)j->t, (const SjRec*)j->t.rec, p, eof, SjNotifyAt{j->t.gap});
+  CU(ctx, cudaGetLastError());
+  j->undrained = true;
+  if (j->spec.ordered) return sjwin_flush_pool(j, p, j->nq);
+  k_sjwin_flush<<<ctx->sm_count * 8, 256, 0, j->s>>>(j->t, j->e, p, j->pool, nullptr);
+  CU(ctx, cudaGetLastError());
+  return BW_OK;
+}
+
+bw_status bw_sjwin_advance(bw_sjwin* j, int64_t system_now_us, bw_sjwin_rows* out) {
+  if (!j || !out) return BW_ERR_SPEC;
+  bw_ctx* ctx = j->ctx;
+  SJWIN_REFUSE_FAILED(j);
+  CU(ctx, cudaSetDevice(ctx->device));
+  if (system_now_us > 0) {
+    if (system_now_us > j->now) j->now = system_now_us;
+    bw_status st = sjwin_wake(j, 0);
+    if (st != BW_OK) return st;
+  }
+  return sjwin_collect(j, out);
+}
+
+bw_status bw_sjwin_eof(bw_sjwin* j, bw_sjwin_rows* out) {
+  if (!j || !out) return BW_ERR_SPEC;
+  bw_ctx* ctx = j->ctx;
+  SJWIN_REFUSE_FAILED(j);
+  CU(ctx, cudaSetDevice(ctx->device));
+  bw_status st = sjwin_wake(j, 1);
+  if (st != BW_OK) return st;
+  return sjwin_collect(j, out);
 }

@@ -369,13 +369,8 @@ class _GpuJoinWindowStep(_GpuWindowStep):
     def __init__(self, step_id: str, plan):
         import numpy as np
 
-        from bytewax_b200.operators.windowing import SlidingWindower
-
         self.np, self.plan, self.step_id = np, plan, step_id
-        w = plan.windower
-        self.length_us = _td_us(w.length)
-        self.offset_us = _td_us(w.offset) if isinstance(w, SlidingWindower) else self.length_us
-        self.align_us = _us(w.align_to)
+        self._windower_spec(plan.windower)
         wait = getattr(plan.clock, "wait_for_system_duration", timedelta(0))  # (SystemClock: stamped with the system time, wait 0)
         self.wait_us = None if wait >= timedelta(days=365 * 200) else _td_us(wait)
         self.key_ids: Dict[str, int] = {}
@@ -386,9 +381,14 @@ class _GpuJoinWindowStep(_GpuWindowStep):
         self.next_handle = 0
         self.jwin = None
 
-    def on_epoch(self, epoch: int, items: list) -> list:
-        from bytewax_b200 import gpu
+    def _windower_spec(self, w):
+        from bytewax_b200.operators.windowing import SlidingWindower
 
+        self.length_us = _td_us(w.length)
+        self.offset_us = _td_us(w.offset) if isinstance(w, SlidingWindower) else self.length_us
+        self.align_us = _us(w.align_to)
+
+    def on_epoch(self, epoch: int, items: list) -> list:
         np, plan = self.np, self.plan
         getter = getattr(plan.clock, "ts_getter", None)
         now = self._now_us()
@@ -408,15 +408,21 @@ class _GpuJoinWindowStep(_GpuWindowStep):
             self.values[h] = value
             labelled.append(sv)
         if self.jwin is None:
-            self.jwin = gpu.JoinWindow(
-                _get_gpu_ctx(), plan.insert_mode, plan.emit_mode, plan.ordered, plan.sides, self.length_us, self.offset_us, self.align_us,
-                self.wait_us, capacity_hint=int(os.environ.get("BYTEWAX_B200_KEYS", 1 << 20)), max_windows_per_key=64,
-                max_queued_rows=1 << 22 if plan.ordered else 0, max_batch_rows=int(os.environ.get("BYTEWAX_B200_BATCH", 1 << 22)),
-                max_emit_rows=1 << 22, max_late_rows=1 << 22)
+            self.jwin = self._make()
         self.last_epoch = max(epoch, self.last_epoch)
         self.jwin.apply(np.array(keys, dtype=np.uint64), np.array(sides, dtype=np.uint8), np.array(handles, dtype=np.uint64),
                         np.array(ts, dtype=np.int64), self.last_epoch, now or 0)
         return self._jwin_rows(self.jwin.advance(), labelled)
+
+    def _make(self):
+        from bytewax_b200 import gpu
+
+        plan = self.plan
+        return gpu.JoinWindow(
+            _get_gpu_ctx(), plan.insert_mode, plan.emit_mode, plan.ordered, plan.sides, self.length_us, self.offset_us, self.align_us,
+            self.wait_us, capacity_hint=int(os.environ.get("BYTEWAX_B200_KEYS", 1 << 20)), max_windows_per_key=64,
+            max_queued_rows=1 << 22 if plan.ordered else 0, max_batch_rows=int(os.environ.get("BYTEWAX_B200_BATCH", 1 << 22)),
+            max_emit_rows=1 << 22, max_late_rows=1 << 22)
 
     def on_notify(self) -> list:
         if self.jwin is None:
@@ -454,6 +460,46 @@ class _GpuJoinWindowStep(_GpuWindowStep):
         for ks, w in metas:
             o, c = self.jwin.window_bounds(w)
             rows.append((ks, (w, "M", WindowMetadata(_dt(o), _dt(c)))))
+        for h in out.released.tolist():  # after this call's rows are built: no later row can name these
+            del V[h]
+        return rows
+
+
+class _GpuSessionJoinWindowStep(_GpuJoinWindowStep):
+    """One worker's ``join_window`` over a ``SessionWindower`` (``GpuJoinWindowPlan``) on ``bw_sjwin_*`` (K10):
+    `_WindowLogic` over `_SessionWindowerLogic` with `_JoinWindowLogic` per session (windowing.py:671-810, 1046-1190,
+    1849-1902), one call per activation.  Handles, clock sampling, notify, EOF and the key re-sort are the join step's;
+    ``M`` rows carry each session's bounds and merged ids from the device, and late rows have window id -1."""
+
+    def _windower_spec(self, w):
+        self.gap_us = _td_us(w.gap)
+
+    def _make(self):
+        from bytewax_b200 import gpu
+
+        plan = self.plan
+        return gpu.SessionJoinWindow(
+            _get_gpu_ctx(), plan.insert_mode, plan.emit_mode, plan.ordered, plan.sides, self.gap_us, self.wait_us,
+            capacity_hint=int(os.environ.get("BYTEWAX_B200_KEYS", 1 << 20)), max_sessions_per_key=int(os.environ.get("BYTEWAX_B200_SESSIONS", 64)),
+            max_queued_rows=1 << 22 if plan.ordered else 0, max_batch_rows=int(os.environ.get("BYTEWAX_B200_BATCH", 1 << 22)),
+            max_emit_rows=1 << 22, max_late_rows=1 << 22)
+
+    def _jwin_rows(self, out, labelled) -> list:
+        from bytewax_b200.operators.windowing import WindowMetadata
+
+        V = self.values
+        lates = [(self._key_str(k), labelled[r]) for k, r in zip(out.late_key.tolist(), out.late_row.tolist())]
+        downs = [(self._key_str(k), w, tuple(None if h is None else V[h] for h in t))
+                 for k, w, t in zip(out.down_key.tolist(), out.down_window_id.tolist(), out.tuples())]
+        o, c = out.meta_open_us.tolist(), out.meta_close_us.tolist()
+        metas = [(self._key_str(k), w, WindowMetadata(_dt(o[i]), _dt(c[i]), set(out.merged(i))))
+                 for i, (k, w) in enumerate(zip(out.meta_key.tolist(), out.meta_window_id.tolist()))]
+        if self.resort:  # interned (non-numeric) keys: restore ascending key-string order; stable
+            for rows in (lates, downs, metas):
+                rows.sort(key=lambda r: r[0])
+        rows = [(ks, (-1, "L", sv)) for ks, sv in lates]
+        rows.extend((ks, (w, "E", t)) for ks, w, t in downs)
+        rows.extend((ks, (w, "M", m)) for ks, w, m in metas)
         for h in out.released.tolist():  # after this call's rows are built: no later row can name these
             del V[h]
         return rows
@@ -561,6 +607,8 @@ def _gpu_step_for(step_id: str, plan):
     from bytewax_b200.operators.windowing import GpuCollectWindowPlan, GpuJoinWindowPlan, SessionWindower
 
     if isinstance(plan, GpuJoinWindowPlan):
+        if isinstance(plan.windower, SessionWindower):
+            return _GpuSessionJoinWindowStep(step_id, plan)
         return _GpuJoinWindowStep(step_id, plan)
     if isinstance(plan, GpuCollectWindowPlan):
         return _GpuCollectWindowStep(step_id, plan)

@@ -545,21 +545,76 @@ class JoinWindowRows:
         return [tuple(int(h[s]) if mk >> s & 1 else None for s in range(len(h))) for h, mk in zip(self.down_handles.tolist(), m)]
 
 
-class JoinWindow:
+class _HandleJoin:
+    """What the handle joins `JoinWindow` (``bw_jwin_*``) and `SessionJoinWindow` (``bw_sjwin_*``) share: their modes,
+    epochs, and the apply / advance / eof / close calls, which differ only in the C prefix and the rows they wrap."""
+
+    INSERT = {"first": 0, "last": 1}
+    EMIT = {"complete": 0, "final": 1, "running": 2}
+    _PREFIX = ""  # the C ABI prefix
+    _ROWS = None  # its rows struct
+
+    def _create(self, ctx: Context, spec, sides: int):
+        self.ctx, self.lib, self.sides, self.spec = ctx, ctx.lib, sides, spec
+        h = C.c_void_p()
+        N.check(self._fn("create")(ctx.h, C.byref(spec), C.byref(h)), ctx.h)
+        self.h = h
+        self._epoch = 0
+
+    def _fn(self, name: str):
+        return getattr(self.lib, f"{self._PREFIX}_{name}")
+
+    def _next_epoch(self, epoch: Optional[int]) -> int:
+        if epoch is None:
+            self._epoch += 1
+            epoch = self._epoch
+        return epoch
+
+    def apply(self, keys, sides, handles, ts_us, epoch: Optional[int] = None, system_now_us: int = 0):
+        """One activation from host arrays.  ``system_now_us``: ``now_getter()`` of the activation."""
+        keys = np.ascontiguousarray(keys, dtype=np.uint64)
+        sides = np.ascontiguousarray(sides, dtype=np.uint8)
+        handles = np.ascontiguousarray(handles, dtype=np.uint64)
+        ts = np.ascontiguousarray(ts_us, dtype=np.int64)
+        epoch = self._next_epoch(epoch)
+        vp = lambda a: a.ctypes.data_as(C.c_void_p)  # noqa: E731
+        N.check(self._fn("apply")(self.h, vp(keys), vp(sides), vp(handles), vp(ts), keys.shape[0], epoch, int(system_now_us)), self.ctx.h)
+
+    def apply_device(self, d_keys: int, d_sides: int, d_handles: int, d_ts: int, rows: int, epoch: Optional[int] = None,
+                     system_now_us: int = 0):
+        epoch = self._next_epoch(epoch)
+        N.check(self._fn("apply_device")(self.h, C.c_void_p(d_keys), C.c_void_p(d_sides), C.c_void_p(d_handles), C.c_void_p(d_ts),
+                                         rows, epoch, int(system_now_us)), self.ctx.h)
+
+    def advance(self, system_now_us: int = 0):
+        """Rows since the last call; ``system_now_us`` > 0 first runs the notify phase at that system time."""
+        r = self._ROWS()
+        N.check(self._fn("advance")(self.h, int(system_now_us), C.byref(r)), self.ctx.h)
+        return self._wrap(r)
+
+    def eof(self):
+        r = self._ROWS()
+        N.check(self._fn("eof")(self.h, C.byref(r)), self.ctx.h)
+        return self._wrap(r)
+
+    def close(self):
+        if self.h:
+            self._fn("destroy")(self.h)
+            self.h = None
+
+
+class JoinWindow(_HandleJoin):
     """``join_window`` with insert mode first / last over tumbling or sliding windows (``bw_jwin``, K8;
     windowing.py:1046-1190, 1849-1902).  Values travel as uint64 handles; the caller keeps the objects and may drop
     each one once it comes back in ``released``."""
 
-    INSERT = {"first": 0, "last": 1}
-    EMIT = {"complete": 0, "final": 1, "running": 2}
+    _PREFIX, _ROWS = "bw_jwin", N.BwJwinRows
 
     def __init__(self, ctx: Context, insert_mode: str = "last", emit_mode: str = "final", ordered: bool = True, sides: int = 2,
                  length_us: int = 10_000_000, offset_us: Optional[int] = None, align_us: int = 0, wait_us: Optional[int] = 0,
                  capacity_hint: int = 1 << 16, max_windows_per_key: int = 16, max_queued_rows: int = 1 << 20,
                  max_batch_rows: int = 1 << 20, max_emit_rows: int = 1 << 20, max_late_rows: int = 1 << 20):
         """``offset_us=None``: tumbling.  ``wait_us=None``: the watermark never advances on data (``BW_WAIT_FOREVER``)."""
-        self.ctx, self.lib = ctx, ctx.lib
-        self.sides = sides
         s = N.BwJwinSpec()
         s.struct_size = C.sizeof(N.BwJwinSpec)
         s.insert_mode, s.emit_mode = self.INSERT.get(insert_mode, -1), self.EMIT.get(emit_mode, -1)
@@ -568,37 +623,12 @@ class JoinWindow:
         s.wait_us = N.BW_WAIT_FOREVER if wait_us is None else wait_us
         s.capacity_hint, s.max_queued_rows, s.max_batch_rows = capacity_hint, max_queued_rows, max_batch_rows
         s.max_emit_rows, s.max_late_rows = max_emit_rows, max_late_rows
-        self.spec = s
-        h = C.c_void_p()
-        N.check(self.lib.bw_jwin_create(ctx.h, C.byref(s), C.byref(h)), ctx.h)
-        self.h = h
-        self._epoch = 0
+        self._create(ctx, s, sides)
 
     def window_bounds(self, window_id: int):
         """``(open_us, close_us)`` of a window (windowing.py:620-623)."""
         o = self.spec.align_us + self.spec.offset_us * window_id
         return o, o + self.spec.length_us
-
-    def apply(self, keys, sides, handles, ts_us, epoch: Optional[int] = None, system_now_us: int = 0):
-        """One activation from host arrays.  ``system_now_us``: ``now_getter()`` of the activation."""
-        keys = np.ascontiguousarray(keys, dtype=np.uint64)
-        sides = np.ascontiguousarray(sides, dtype=np.uint8)
-        handles = np.ascontiguousarray(handles, dtype=np.uint64)
-        ts = np.ascontiguousarray(ts_us, dtype=np.int64)
-        if epoch is None:
-            self._epoch += 1
-            epoch = self._epoch
-        vp = lambda a: a.ctypes.data_as(C.c_void_p)  # noqa: E731
-        N.check(self.lib.bw_jwin_apply(self.h, vp(keys), vp(sides), vp(handles), vp(ts), keys.shape[0], epoch, int(system_now_us)),
-                self.ctx.h)
-
-    def apply_device(self, d_keys: int, d_sides: int, d_handles: int, d_ts: int, rows: int, epoch: Optional[int] = None,
-                     system_now_us: int = 0):
-        if epoch is None:
-            self._epoch += 1
-            epoch = self._epoch
-        N.check(self.lib.bw_jwin_apply_device(self.h, C.c_void_p(d_keys), C.c_void_p(d_sides), C.c_void_p(d_handles), C.c_void_p(d_ts),
-                                              rows, epoch, int(system_now_us)), self.ctx.h)
 
     def _wrap(self, r: N.BwJwinRows) -> JoinWindowRows:
         nd, nm, nl, nr = int(r.n_down), int(r.n_meta), int(r.n_late), int(r.n_released)
@@ -612,21 +642,56 @@ class JoinWindow:
                               arr(r.late_key, nl), arr(r.late_window_id, nl, np.int64), arr(r.late_epoch, nl),
                               arr(r.late_activation, nl), arr(r.late_row, nl), arr(r.released, nr))
 
-    def advance(self, system_now_us: int = 0) -> JoinWindowRows:
-        """Rows since the last call; ``system_now_us`` > 0 first runs the notify phase at that system time."""
-        r = N.BwJwinRows()
-        N.check(self.lib.bw_jwin_advance(self.h, int(system_now_us), C.byref(r)), self.ctx.h)
-        return self._wrap(r)
 
-    def eof(self) -> JoinWindowRows:
-        r = N.BwJwinRows()
-        N.check(self.lib.bw_jwin_eof(self.h, C.byref(r)), self.ctx.h)
-        return self._wrap(r)
+@dataclass
+class SessionJoinWindowRows(JoinWindowRows):
+    """Rows of one ``SessionJoinWindow.advance`` / ``eof``: the join's streams, with each meta row's session bounds and
+    merged ids.  Late rows all have window id -1 (``LATE_SESSION_ID``)."""
 
-    def close(self):
-        if self.h:
-            self.lib.bw_jwin_destroy(self.h)
-            self.h = None
+    meta_open_us: np.ndarray = None
+    meta_close_us: np.ndarray = None
+    merged_off: np.ndarray = None  # [n_meta + 1] into merged_ids
+    merged_ids: np.ndarray = None
+
+    def merged(self, i: int) -> List[int]:
+        """The ids merged directly into meta row ``i``'s session, ascending."""
+        return self.merged_ids[self.merged_off[i] : self.merged_off[i + 1]].tolist()
+
+
+class SessionJoinWindow(_HandleJoin):
+    """``join_window`` with insert mode first / last over session windows (``bw_sjwin``, K10; windowing.py:671-810,
+    1046-1190, 1849-1902).  Values travel as uint64 handles; the caller keeps the objects and may drop each one once it
+    comes back in ``released``.  Session bounds come with each meta row."""
+
+    _PREFIX, _ROWS = "bw_sjwin", N.BwSjwinRows
+
+    def __init__(self, ctx: Context, insert_mode: str = "last", emit_mode: str = "final", ordered: bool = True, sides: int = 2,
+                 gap_us: int = 10_000_000, wait_us: Optional[int] = 0, capacity_hint: int = 1 << 16, max_sessions_per_key: int = 16,
+                 max_queued_rows: int = 1 << 20, max_batch_rows: int = 1 << 20, max_emit_rows: int = 1 << 20, max_late_rows: int = 1 << 20):
+        """``wait_us=None``: the watermark never advances on data (``BW_WAIT_FOREVER``)."""
+        s = N.BwSjwinSpec()
+        s.struct_size = C.sizeof(N.BwSjwinSpec)
+        s.insert_mode, s.emit_mode = self.INSERT.get(insert_mode, -1), self.EMIT.get(emit_mode, -1)
+        s.ordered, s.sides, s.max_sessions_per_key = int(ordered), sides, max_sessions_per_key
+        s.gap_us, s.wait_us = gap_us, N.BW_WAIT_FOREVER if wait_us is None else wait_us
+        s.capacity_hint, s.max_queued_rows, s.max_batch_rows = capacity_hint, max_queued_rows, max_batch_rows
+        s.max_emit_rows, s.max_late_rows = max_emit_rows, max_late_rows
+        self._create(ctx, s, sides)
+
+    def _wrap(self, r: N.BwSjwinRows) -> SessionJoinWindowRows:
+        nd, nm, nl, nr = int(r.n_down), int(r.n_meta), int(r.n_late), int(r.n_released)
+
+        def arr(ptr, n, dt=np.uint64):
+            return np.ctypeslib.as_array(ptr, shape=(n,)).view(dt).copy() if n else np.zeros(0, dt)
+
+        hs = np.stack([arr(r.down_handle[s], nd) for s in range(self.sides)], axis=1) if nd else np.zeros((0, self.sides), np.uint64)
+        off = arr(r.merged_off, nm + 1).astype(np.int64)
+        return SessionJoinWindowRows(arr(r.down_key, nd), arr(r.down_window_id, nd, np.int64), hs, arr(r.down_mask, nd), arr(r.down_epoch, nd),
+                                     arr(r.meta_key, nm), arr(r.meta_window_id, nm, np.int64), arr(r.meta_epoch, nm),
+                                     arr(r.late_key, nl), np.full(nl, -1, np.int64), arr(r.late_epoch, nl),
+                                     arr(r.late_activation, nl), arr(r.late_row, nl), arr(r.released, nr),
+                                     arr(r.meta_open_us, nm, np.int64), arr(r.meta_close_us, nm, np.int64), off,
+                                     arr(r.merged_ids, int(off[-1]), np.int64))
 
 
 @dataclass

@@ -788,10 +788,15 @@ class _JoinWindowLogic(WindowLogic):
         return _EMPTY
 
     def on_merge(self, original):
-        if self.insert_mode == "product":
-            self.state += original.state
-        else:
+        # windowing.py:1879-1891: "first" takes the merged-away session's value on every side it set; "last" keeps the
+        # survivor's value on every side the survivor set
+        if self.insert_mode == "first":
             self.state |= original.state
+        elif self.insert_mode == "last":
+            original.state |= self.state
+            self.state = original.state
+        else:
+            self.state += original.state
         if self.emit_mode == "complete" and self.state.all_set():
             rows = self.state.astuples()
             self.state.clear()
@@ -832,9 +837,9 @@ def join_window(step_id: str, clock: Clock, windower: Windower, *sides: KeyedStr
 
 @dataclass(frozen=True)
 class GpuJoinWindowPlan:
-    """A ``join_window`` the engine may run with ``bw_jwin_*`` (K8): insert mode first / last, 1 to 4 sides, a tumbling or
-    sliding windower, and an `EventClock` with an identity ``to_system_utc`` or a `SystemClock`.  Values travel as
-    handles into a host-side dict, so they can be any Python object."""
+    """A ``join_window`` the engine may run with ``bw_jwin_*`` (K8, tumbling or sliding windower) or ``bw_sjwin_*`` (K10,
+    `SessionWindower`): insert mode first / last, 1 to 4 sides, and an `EventClock` with an identity ``to_system_utc`` or a
+    `SystemClock`.  Values travel as handles into a host-side dict, so they can be any Python object."""
 
     insert_mode: str
     emit_mode: str
@@ -845,11 +850,11 @@ class GpuJoinWindowPlan:
 
 
 def _join_window_plan(clock, windower, side_count, insert_mode, emit_mode, ordered) -> Optional[GpuJoinWindowPlan]:
-    # product keeps lists per side and session windows merge: host engine.  A custom `to_system_utc` moves the notify
-    # time away from the event time the device compares with the system clock (windowing.py:1177-1178): host engine.
+    # product keeps lists per side: host engine.  A custom `to_system_utc` moves the notify time away from the event
+    # time the device compares with the system clock (windowing.py:1177-1178): host engine.
     if insert_mode not in ("first", "last") or not 1 <= side_count <= 4:
         return None
-    if not isinstance(windower, (SlidingWindower, TumblingWindower)):
+    if not isinstance(windower, (SlidingWindower, TumblingWindower, SessionWindower)):
         return None
     if not (isinstance(clock, SystemClock) or (isinstance(clock, EventClock) and clock.to_system_utc is _identity)):
         return None

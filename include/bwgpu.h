@@ -586,6 +586,89 @@ bw_status bw_collect_advance(bw_collect* c, int64_t system_now_us, bw_collect_ro
 /* End of input: every key flushes at watermark UTC_MAX (:1144-1151). */
 bw_status bw_collect_eof(bw_collect* c, bw_collect_rows* out);
 
+/* Windowed join over session windows (K10): `join_window` (pysrc/bytewax/operators/windowing.py:2056-2140) with insert
+ * modes first / last over `SessionWindower` (:928-950), i.e. `_WindowLogic` (:1046-1190) over `_SessionWindowerLogic`
+ * (:671-810) with `_JoinWindowLogic` (:1849-1902) per session.  Values travel as u64 handles; the objects stay with the
+ * caller.  Per key, per call, in order: the EventClock's late test per item (:263-287; a late item gives one row, window
+ * LATE_SESSION_ID = -1, :671, :764-766, and is not queued); `_flush_queue` (:1095-1108) at the watermark after the key's
+ * last item (unordered: every queued entry in arrival order; ordered: the entries with ts <= watermark, stably sorted by
+ * ts, the rest kept queued across calls); per due value `open_for` (:731-762: the FIRST live session by id that contains
+ * ts or lies within gap of it, extended, then `_session_find_merges` :688-715; else a new session, id max_key + 1) and
+ * `on_value` on the session it returned, even one a merge just took away (:1064-1077, :1866-1876); then the merge queue
+ * in discovery order (:1079-1085) with `on_merge` (:1879-1891): "first" takes the merged-away session's value on every
+ * side it set, "last" keeps the survivor's on every side the survivor set; then "complete" emits under the survivor's id
+ * and clears once every side is set, "running" emits; then `close_for` (:774-788): sessions with close < watermark - gap
+ * (UTC_MIN if that is below it) in id order, each giving the `final` tuple (emit mode final) and its metadata row.
+ * Session state is never discarded (:798-806): a key's clock and session ids outlive its sessions.  One GPU only. */
+typedef struct bw_sjwin bw_sjwin;
+typedef struct bw_sjwin_spec {
+  uint32_t struct_size;
+  int32_t insert_mode;          /* BW_JOIN_INSERT_FIRST / LAST (product keeps lists per side: host engine) */
+  int32_t emit_mode;            /* BW_JOIN_EMIT_COMPLETE / FINAL / RUNNING */
+  int32_t ordered;              /* 1: play values in timestamp order once the watermark passes them (the default) */
+  int32_t sides;                /* 1..4 joined streams */
+  int32_t max_sessions_per_key; /* 1..64: sessions a key holds during a call (live ones, plus those merged away in it),
+                                   and also the merged ids its live sessions hold */
+  int64_t gap_us;               /* SessionWindower.gap, >= 0 (windowing.py:938-943) */
+  int64_t wait_us;              /* EventClock.wait_for_system_duration, or BW_WAIT_FOREVER */
+  uint64_t capacity_hint;       /* keys ever seen: session state is never freed (windowing.py:798-806) */
+  uint64_t max_queued_rows;     /* ordered mode: queued entries over ALL keys */
+  uint64_t max_batch_rows;
+  uint64_t max_emit_rows;       /* down rows, meta rows, and meta rows' merged ids, retained between bw_sjwin_advance calls */
+  uint64_t max_late_rows;       /* late rows retained between bw_sjwin_advance calls */
+} bw_sjwin_spec;
+/* Rows handed downstream since the last advance / eof, in the reference's order: per call (activation, notify phase
+ * or EOF), ascending key string (src/operators.rs:758-767, :862-894); within a key `down` rows of the inserts in play
+ * order, then of the merges in merge-queue order (under the survivor's id), then the `final` rows of the closing
+ * sessions in id order; `meta` rows in id order; `late` rows in arrival order.  Host pointers into memory owned by the
+ * library, valid until the next advance / eof / destroy. */
+typedef struct bw_sjwin_rows {
+  uint64_t n_down;
+  const uint64_t* down_key;
+  const int64_t* down_window_id;
+  const uint64_t* down_handle[4]; /* [side][row]: valid where bit `side` of down_mask is set (else the reference emits None) */
+  const uint64_t* down_mask;
+  const uint64_t* down_epoch;
+  uint64_t n_meta;                /* closed sessions: WindowMetadata(open, close, merged_ids) */
+  const uint64_t* meta_key;
+  const int64_t* meta_window_id;
+  const int64_t* meta_open_us;
+  const int64_t* meta_close_us;
+  const uint64_t* meta_epoch;
+  const uint64_t* merged_off;     /* [n_meta + 1]: row i merged ids are merged_ids[merged_off[i] .. merged_off[i+1]) */
+  const int64_t* merged_ids;      /* ascending per row: the sessions merged directly into it */
+  uint64_t n_late;                /* window id LATE_SESSION_ID = -1 */
+  const uint64_t* late_key;
+  const uint64_t* late_epoch;
+  const uint64_t* late_activation; /* (activation, row) name the input row (activations counted from 0) */
+  const uint64_t* late_row;
+  /* handles no session and no queue entry holds any more; each handle passed to apply is listed exactly once, in the
+   * rows of the call that let go of it: a late item's and a "first" value's that found its side set in the call that
+   * received it; a value replaced by "last", cleared by "complete" or losing a merge; a session's when it closes */
+  uint64_t n_released;           /* (the device buffer behind it grows with the handles held, never with the table size) */
+  const uint64_t* released;
+} bw_sjwin_rows;
+/* windowing.py:2056-2140 (join_window) + :1046-1190 (_WindowLogic) + :671-810 (_SessionWindowerLogic) */
+bw_status bw_sjwin_create(bw_ctx* ctx, const bw_sjwin_spec* spec, bw_sjwin** out);
+void bw_sjwin_destroy(bw_sjwin* j);
+/* One activation from HOST columns (keys, side 0..sides-1, handle, ts); blocks: `_WindowLogic.on_batch`
+ * (windowing.py:1115-1133).  `system_now_us` is `now_getter()` for this activation (:250-261; it must not go backwards;
+ * 0 throughout = a frozen clock).  A full key table, more than max_sessions_per_key sessions or merged ids, or a full
+ * queue, emit or late buffer returns BW_ERR_CAPACITY (reason in bw_last_error) and the join refuses further calls. */
+bw_status bw_sjwin_apply(bw_sjwin* j, const uint64_t* keys, const uint8_t* side, const uint64_t* handles, const int64_t* ts_us,
+                         uint64_t rows, uint64_t epoch, int64_t system_now_us);
+/* Same with DEVICE columns; returns once the work is enqueued (the columns must stay valid until the next call).  A side
+ * value >= sides is not played: the next call returns BW_ERR_SPEC and the join refuses further calls. */
+bw_status bw_sjwin_apply_device(bw_sjwin* j, const uint64_t* d_keys, const uint8_t* d_side, const uint64_t* d_handles,
+                                const int64_t* d_ts_us, uint64_t rows, uint64_t epoch, int64_t system_now_us);
+/* Rows since the last call.  `system_now_us` > 0 first runs the notify phase at that system time
+ * (src/operators.rs:808-858, windowing.py:1135-1142, 1153-1180 with an identity `to_system_utc`): every key whose
+ * earliest session close + gap -- or, ordered, the ts of its FIRST queued entry -- has been reached flushes at its
+ * watermark. */
+bw_status bw_sjwin_advance(bw_sjwin* j, int64_t system_now_us, bw_sjwin_rows* out);
+/* End of input: every key flushes at watermark UTC_MAX (:1144-1151), so sessions with close >= UTC_MAX - gap stay open. */
+bw_status bw_sjwin_eof(bw_sjwin* j, bw_sjwin_rows* out);
+
 /* ---- plain device-memory helpers (tests / bench / host bindings without torch) ---- */
 bw_status bw_dev_alloc(bw_ctx* ctx, uint64_t bytes, void** out);
 bw_status bw_dev_free(bw_ctx* ctx, void* ptr);
