@@ -155,6 +155,23 @@ class BwSjwinRows(C.Structure):
                 ("n_released", C.c_uint64), ("released", C.POINTER(C.c_uint64))]
 
 
+class BwArgwinSpec(C.Structure):
+    _fields_ = [("struct_size", C.c_uint32), ("extreme", C.c_int32), ("by_dtype", C.c_int32), ("session", C.c_int32),
+                ("max_windows_per_key", C.c_int32), ("pad", C.c_int32), ("length_us", C.c_int64), ("offset_us", C.c_int64),
+                ("align_us", C.c_int64), ("gap_us", C.c_int64), ("wait_us", C.c_int64), ("capacity_hint", C.c_uint64),
+                ("max_batch_rows", C.c_uint64), ("max_emit_rows", C.c_uint64), ("max_late_rows", C.c_uint64)]
+
+
+class BwArgwinRows(C.Structure):
+    _fields_ = [("n_closed", C.c_uint64), ("closed_key", C.POINTER(C.c_uint64)), ("closed_window_id", C.POINTER(C.c_int64)),
+                ("closed_handle", C.POINTER(C.c_uint64)), ("closed_open_us", C.POINTER(C.c_int64)),
+                ("closed_close_us", C.POINTER(C.c_int64)), ("closed_epoch", C.POINTER(C.c_uint64)),
+                ("merged_off", C.POINTER(C.c_uint64)), ("merged_ids", C.POINTER(C.c_int64)),
+                ("n_late", C.c_uint64), ("late_key", C.POINTER(C.c_uint64)), ("late_window_id", C.POINTER(C.c_int64)),
+                ("late_epoch", C.POINTER(C.c_uint64)), ("late_activation", C.POINTER(C.c_uint64)), ("late_row", C.POINTER(C.c_uint64)),
+                ("n_released", C.c_uint64), ("released", C.POINTER(C.c_uint64))]
+
+
 # every symbol include/bwgpu.h declares: (restype, argtypes)
 _P = C.c_void_p
 SYMBOLS = {
@@ -220,6 +237,12 @@ SYMBOLS = {
     "bw_sjwin_apply_device": (C.c_int32, [_P, _P, _P, _P, _P, C.c_uint64, C.c_uint64, C.c_int64]),
     "bw_sjwin_advance": (C.c_int32, [_P, C.c_int64, C.POINTER(BwSjwinRows)]),
     "bw_sjwin_eof": (C.c_int32, [_P, C.POINTER(BwSjwinRows)]),
+    "bw_argwin_create": (C.c_int32, [_P, C.POINTER(BwArgwinSpec), C.POINTER(_P)]),
+    "bw_argwin_destroy": (None, [_P]),
+    "bw_argwin_apply": (C.c_int32, [_P, _P, _P, _P, _P, C.c_uint64, C.c_uint64, C.c_int64]),
+    "bw_argwin_apply_device": (C.c_int32, [_P, _P, _P, _P, _P, C.c_uint64, C.c_uint64, C.c_int64]),
+    "bw_argwin_advance": (C.c_int32, [_P, C.c_int64, C.POINTER(BwArgwinRows)]),
+    "bw_argwin_eof": (C.c_int32, [_P, C.POINTER(BwArgwinRows)]),
     "bw_dev_alloc": (C.c_int32, [_P, C.c_uint64, C.POINTER(_P)]),
     "bw_dev_free": (C.c_int32, [_P, _P]),
     "bw_host_alloc": (C.c_int32, [_P, C.c_uint64, C.POINTER(_P)]),

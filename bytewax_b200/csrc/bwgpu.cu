@@ -38,6 +38,7 @@
 #include "bw_jwin.cuh"
 #include "bw_collect.cuh"
 #include "bw_sjwin.cuh"
+#include "bw_argwin.cuh"
 #include "bw_prepass.cuh"
 #include "bw_slow.cuh"
 #include "bw_late.cuh"
@@ -3120,6 +3121,11 @@ static const char* jwin_what(const bw_jwin*) { return "windowed join"; }
 static const char* jwin_full_windows(const bw_jwin*) { return " a key needs more than max_windows_per_key open windows;"; }
 static const char* jwin_full_emit(const bw_jwin*) { return " more than max_emit_rows down or meta rows since the last advance;"; }
 static u64 jwin_counters(const bw_jwin*) { return 5; }  // down, meta, late, released, carried-over queue entries
+// ordered joins keep a queue whose entry count comes back with the drain (bw_argwin, K11, has none)
+template <class J>
+static bool jwin_queues(const J* j) {
+  return j->spec.ordered;
+}
 
 // wait for the last call; fail on a device-side overflow; then take its released handles and its queue count, so the
 // device buffer only ever holds one call's releases
@@ -3149,7 +3155,7 @@ static bw_status jwin_drain(J* j) {
     j->released.resize(at + nr);
     CU(ctx, cudaMemcpyAsync(j->released.data() + at, j->e.rel, nr * 8, cudaMemcpyDeviceToHost, j->s));
   }
-  if (j->spec.ordered) j->nq = j->h_cnt[4];
+  if (jwin_queues(j)) j->nq = j->h_cnt[4];
   CU(ctx, cudaMemsetAsync(j->d_cnt + 3, 0, 16, j->s));
   CU(ctx, cudaStreamSynchronize(j->s));
   j->undrained = false;
@@ -4086,4 +4092,290 @@ bw_status bw_sjwin_eof(bw_sjwin* j, bw_sjwin_rows* out) {
   bw_status st = sjwin_wake(j, 1);
   if (st != BW_OK) return st;
   return sjwin_collect(j, out);
+}
+
+// ===========================================================================
+// K11 host side: windowed arg-max / arg-min (bw_argwin.cuh)
+// ===========================================================================
+struct bw_argwin {
+  Owner own;  // every buffer and the stream below
+  bw_ctx* ctx = nullptr;
+  bw_argwin_spec spec{};
+  AwTable t{};
+  KeyedScratch k;
+  cudaStream_t s = nullptr;
+  u32* h_err = nullptr;                 // err, why
+  unsigned long long* d_cnt = nullptr;  // closed rows, merged ids, late, released, (unused: K8's queue count)
+  unsigned long long* h_cnt = nullptr;
+  u64 *d_handles = nullptr, *d_by = nullptr;
+  i64* d_ts = nullptr;
+  AwEmit e{};
+  u64 nq = 0;            // (no queue: jwin_drain's count, always 0)
+  SortScratch srt;       // ordering scratch
+  HostCols hd[2];        // closed: key, window id, handle, open, close | epoch, merged count, merged offset
+  HostCols hl;           // late: key, window id, epoch, activation, row
+  i64* h_mids = nullptr;
+  std::vector<u64> merged_off;
+  std::vector<i64> merged_ids;
+  std::vector<u64> released;      // since the last advance / eof
+  std::vector<u64> released_out;  // what the last advance / eof handed out
+  bool undrained = false;     // a call whose released handles are not read back yet
+  u64 outstanding = 0;        // handles passed in and not released yet: what the next call can release, besides its own
+  u32 batch_no = 0;
+  u64 calls = 0, first_call = 0;  // calls (activations, notify phases, EOF) so far; the first not yet collected
+  u64 last_epoch = 0;
+  i64 now = INT64_MIN;
+  bool failed = false;
+};
+
+// what the host steps K11 shares with the handle joins (jwin_drain, jwin_room, jwin_ship) ask of it
+static const char* jwin_what(const bw_argwin*) { return "windowed arg-max / arg-min"; }
+static const char* jwin_full_windows(const bw_argwin* a) {
+  return a->spec.session ? " a key needs more than max_windows_per_key sessions or merged ids;" : " a key needs more than max_windows_per_key open windows;";
+}
+static const char* jwin_full_emit(const bw_argwin*) { return " more than max_emit_rows closed rows or merged ids since the last advance;"; }
+static u64 jwin_counters(const bw_argwin*) { return 5; }
+static bool jwin_queues(const bw_argwin*) { return false; }
+
+bw_status bw_argwin_create(bw_ctx* ctx, const bw_argwin_spec* spec, bw_argwin** out) {
+  if (!ctx || !spec || !out) CTX_FAIL(ctx, BW_ERR_SPEC, "bw_argwin_create: NULL argument");
+  if (spec->struct_size != sizeof(bw_argwin_spec)) CTX_FAIL(ctx, BW_ERR_SPEC, "bw_argwin_spec.struct_size mismatch");
+  if (ctx->world != 1) CTX_FAIL(ctx, BW_ERR_SPEC, "windowed arg-max / arg-min run on one GPU (world == 1)");
+  if (spec->extreme != BW_RED_MAX && spec->extreme != BW_RED_MIN) CTX_FAIL(ctx, BW_ERR_SPEC, "extreme must be BW_RED_MAX or BW_RED_MIN");
+  if (spec->by_dtype != BW_VAL_I64 && spec->by_dtype != BW_VAL_F64) CTX_FAIL(ctx, BW_ERR_SPEC, "by_dtype must be BW_VAL_I64 or BW_VAL_F64");
+  if (spec->session != 0 && spec->session != 1) CTX_FAIL(ctx, BW_ERR_SPEC, "session must be 0 or 1");
+  if (spec->max_windows_per_key < 1 || spec->max_windows_per_key > BW_JW_MAXM)
+    CTX_FAIL(ctx, BW_ERR_SPEC, "max_windows_per_key must be in 1..%d", BW_JW_MAXM);
+  if (spec->session) {
+    if (spec->gap_us < 0 || spec->gap_us > BW_UTC_MAX_US - BW_UTC_MIN_US) CTX_FAIL(ctx, BW_ERR_SPEC, "gap_us must be in 0..UTC_MAX - UTC_MIN");
+  } else {
+    if (spec->length_us <= 0 || spec->length_us > BW_UTC_MAX_US - BW_UTC_MIN_US) CTX_FAIL(ctx, BW_ERR_SPEC, "length_us must be in 1..UTC_MAX - UTC_MIN");
+    if (spec->offset_us <= 0 || spec->offset_us > spec->length_us) CTX_FAIL(ctx, BW_ERR_SPEC, "offset_us must be in 1..length_us");
+    if (spec->align_us < BW_UTC_MIN_US || spec->align_us > BW_UTC_MAX_US) CTX_FAIL(ctx, BW_ERR_SPEC, "align_us out of range");
+  }
+  if (spec->wait_us < 0) CTX_FAIL(ctx, BW_ERR_SPEC, "wait_us must not be negative");
+  if (spec->max_batch_rows == 0 || spec->max_batch_rows >= (1ULL << 31)) CTX_FAIL(ctx, BW_ERR_SPEC, "bad max_batch_rows");
+  if (spec->capacity_hint >= (1ULL << 30)) CTX_FAIL(ctx, BW_ERR_SPEC, "capacity_hint must be below 2^30");
+  CU(ctx, cudaSetDevice(ctx->device));
+  std::unique_ptr<bw_argwin, void (*)(bw_argwin*)> ap(new bw_argwin(), bw_argwin_destroy);  // torn down on every failure
+  bw_argwin* a = ap.get();
+  Owner& own = a->own;
+  a->ctx = ctx;
+  a->spec = *spec;
+  const u64 cap = std::max<u64>(1024, 2 * std::max<u64>(spec->capacity_hint, 1));
+  const int M = spec->max_windows_per_key;
+  AwTable& t = a->t;
+  t.j.cap = cap;
+  t.j.M = M;
+  t.j.sides = 1;
+  t.gap = spec->gap_us;
+  t.is_max = spec->extreme == BW_RED_MAX;
+  t.is_f64 = spec->by_dtype == BW_VAL_F64;
+  CU(ctx, own.stream(&a->s));
+  CU(ctx, own.dev(&t.j.keys, cap + 1));
+  CU(ctx, own.dev(&t.j.st, cap + 1));
+  if (spec->session) {
+    CU(ctx, own.dev(&t.kx, cap + 1));
+    CU(ctx, own.dev(&t.rec, (cap + 1) * (u64)M));
+    CU(ctx, own.dev(&t.mrg, (cap + 1) * (u64)(2 * M)));
+  } else {
+    CU(ctx, own.dev(&t.win, (cap + 1) * (u64)M));
+  }
+  CU(ctx, own.dev(&t.j.err, 2));
+  t.j.why = t.j.err + 1;
+  t.err = t.j.err;
+  t.why = t.j.why;
+  CU(ctx, own.dev(&a->d_cnt, 5));
+  CU(ctx, cudaMemsetAsync(t.err, 0, 8, a->s));
+  CU(ctx, cudaMemsetAsync(a->d_cnt, 0, 40, a->s));
+  CU(ctx, own.host(&a->h_err, 64 / sizeof(u32)));
+  CU(ctx, own.host(&a->h_cnt, 64 / sizeof(unsigned long long)));
+  const u64 n = spec->max_batch_rows, m = std::max<u64>(spec->max_emit_rows, 1), l = std::max<u64>(spec->max_late_rows, 1);
+  bw_status st = keyed_alloc(ctx, own, a->k, n, a->s);
+  if (st != BW_OK) return st;
+  CU(ctx, own.dev(&a->d_handles, n));
+  CU(ctx, own.dev(&a->d_by, n));
+  CU(ctx, own.dev(&a->d_ts, n));
+  AwEmit& e = a->e;
+  for (u64** c : {&e.key, &e.wid, &e.h, &e.epoch, &e.ord, &e.seq, &e.moff, &e.mcnt}) CU(ctx, own.dev(c, m));
+  for (i64** c : {&e.open, &e.close, &e.mids}) CU(ctx, own.dev(c, m));
+  for (u64** c : {&e.l_key, &e.l_wid, &e.l_epoch, &e.l_act, &e.l_row, &e.l_ord, &e.l_seq}) CU(ctx, own.dev(c, l));
+  // the release buffer grows with the handles held (jwin_room); it starts at one batch
+  e.max_rel = n;
+  CU(ctx, own.dev(&e.rel, e.max_rel));
+  e.max_rows = spec->max_emit_rows;
+  e.max_late = spec->max_late_rows;
+  e.n_rows = a->d_cnt;
+  e.n_mids = a->d_cnt + 1;
+  e.n_late = a->d_cnt + 2;
+  e.n_rel = a->d_cnt + 3;
+  const u64 ns = std::max(m, l);
+  CU(ctx, a->srt.reserve(own, ns, ns, a->s));
+  CU(ctx, a->hd[0].reserve(own, m, m));
+  CU(ctx, a->hd[1].reserve(own, m, m));
+  CU(ctx, a->hl.reserve(own, l, l));
+  CU(ctx, own.host(&a->h_mids, m));
+  k_awin_init<<<ctx->sm_count * 4, 256, 0, a->s>>>(t);
+  CU(ctx, cudaGetLastError());
+  CU(ctx, cudaStreamSynchronize(a->s));
+  *out = ap.release();
+  return BW_OK;
+}
+
+void bw_argwin_destroy(bw_argwin* a) {
+  if (!a) return;
+  cudaSetDevice(a->ctx->device);
+  if (a->s) cudaStreamSynchronize(a->s);
+  delete a;  // a->own releases every buffer and the stream
+}
+
+static JwParams argwin_params(bw_argwin* a, u64 epoch) {
+  JwParams p{};
+  p.length = a->spec.length_us;
+  p.offset = a->spec.offset_us;
+  p.align = a->spec.align_us;
+  p.wait = a->spec.wait_us;
+  p.now = a->now;
+  p.epoch = epoch;
+  p.ord = a->calls++;
+  p.batch_no = a->batch_no;
+  return p;
+}
+
+bw_status bw_argwin_apply_device(bw_argwin* a, const uint64_t* d_keys, const uint64_t* d_handles, const uint64_t* d_by_bits,
+                                 const int64_t* d_ts_us, uint64_t rows, uint64_t epoch, int64_t system_now_us) {
+  if (!a) return BW_ERR_SPEC;
+  bw_ctx* ctx = a->ctx;
+  if (rows > a->spec.max_batch_rows) CTX_FAIL(ctx, BW_ERR_SPEC, "windowed arg-max / arg-min: rows > max_batch_rows");
+  if (rows && (!d_keys || !d_handles || !d_by_bits || !d_ts_us)) CTX_FAIL(ctx, BW_ERR_SPEC, "windowed arg-max / arg-min: NULL column");
+  CU(ctx, cudaSetDevice(ctx->device));
+  bw_status st = jwin_drain(a);
+  if (st != BW_OK) return st;
+  if (a->batch_no && epoch < a->last_epoch) CTX_FAIL(ctx, BW_ERR_STATE, "windowed arg-max / arg-min: epochs must not decrease");
+  a->last_epoch = epoch;
+  if (system_now_us > a->now) a->now = system_now_us;  // `now_getter()` never goes backwards (windowing.py:250-261)
+  const JwParams p = argwin_params(a, epoch);
+  a->batch_no++;
+  if (rows == 0) return BW_OK;
+  if ((st = jwin_room(a, rows)) != BW_OK) return st;
+  a->outstanding += rows;
+  st = keyed_group(ctx, a->k, d_keys, rows, a->s);
+  if (st != BW_OK) return st;
+  if (a->spec.session)
+    k_aswin_apply<<<ctx->sm_count * 8, 256, 0, a->s>>>(a->t, a->e, p, a->k.d_ksorted, a->k.d_isorted, a->k.d_head, d_handles, d_by_bits,
+                                                       d_ts_us, rows);
+  else
+    k_awin_apply<<<ctx->sm_count * 8, 256, 0, a->s>>>(a->t, a->e, p, a->k.d_ksorted, a->k.d_isorted, a->k.d_head, d_handles, d_by_bits,
+                                                      d_ts_us, rows);
+  CU(ctx, cudaGetLastError());
+  a->undrained = true;
+  return BW_OK;
+}
+
+bw_status bw_argwin_apply(bw_argwin* a, const uint64_t* keys, const uint64_t* handles, const uint64_t* by_bits, const int64_t* ts_us,
+                          uint64_t rows, uint64_t epoch, int64_t system_now_us) {
+  if (!a) return BW_ERR_SPEC;
+  bw_ctx* ctx = a->ctx;
+  if (rows > a->spec.max_batch_rows) CTX_FAIL(ctx, BW_ERR_SPEC, "windowed arg-max / arg-min: rows > max_batch_rows");
+  if (rows && (!keys || !handles || !by_bits || !ts_us)) CTX_FAIL(ctx, BW_ERR_SPEC, "windowed arg-max / arg-min: NULL column");
+  CU(ctx, cudaSetDevice(ctx->device));
+  bw_status st = jwin_drain(a);
+  if (st != BW_OK) return st;
+  if (rows) {
+    CU(ctx, cudaMemcpyAsync(a->k.d_keys, keys, rows * 8, cudaMemcpyHostToDevice, a->s));
+    CU(ctx, cudaMemcpyAsync(a->d_handles, handles, rows * 8, cudaMemcpyHostToDevice, a->s));
+    CU(ctx, cudaMemcpyAsync(a->d_by, by_bits, rows * 8, cudaMemcpyHostToDevice, a->s));
+    CU(ctx, cudaMemcpyAsync(a->d_ts, ts_us, rows * 8, cudaMemcpyHostToDevice, a->s));
+  }
+  st = bw_argwin_apply_device(a, a->k.d_keys, a->d_handles, a->d_by, a->d_ts, rows, epoch, system_now_us);
+  if (st != BW_OK) return st;
+  // the host columns may be reused by the caller once this returns
+  return jwin_drain(a);
+}
+
+static bw_status argwin_collect(bw_argwin* a, bw_argwin_rows* out) {
+  bw_ctx* ctx = a->ctx;
+  bw_status st = jwin_drain(a);
+  if (st != BW_OK) return st;
+  CU(ctx, cudaMemcpyAsync(a->h_cnt, a->d_cnt, 24, cudaMemcpyDeviceToHost, a->s));
+  CU(ctx, cudaStreamSynchronize(a->s));
+  const u64 nc = a->h_cnt[0], nmid = a->h_cnt[1], nl = a->h_cnt[2];  // all within bounds: jwin_drain passed
+  const AwEmit& e = a->e;
+  const u64* closed[] = {e.key, e.wid, e.h, (const u64*)e.open, (const u64*)e.close, e.epoch, e.mcnt, e.moff};
+  const u64* late[] = {e.l_key, e.l_wid, e.l_epoch, e.l_act, e.l_row};
+  if ((st = jwin_ship(a, nc, e.key, e.seq, e.ord, closed, 8, a->hd)) != BW_OK) return st;
+  if ((st = jwin_ship(a, nl, e.l_key, e.l_seq, e.l_ord, late, 5, &a->hl)) != BW_OK) return st;
+  if (nmid) CU(ctx, cudaMemcpyAsync(a->h_mids, e.mids, nmid * 8, cudaMemcpyDeviceToHost, a->s));
+  CU(ctx, cudaGetLastError());
+  CU(ctx, cudaMemsetAsync(a->d_cnt, 0, 24, a->s));
+  CU(ctx, cudaStreamSynchronize(a->s));
+  // merged ids in closed row order
+  a->merged_off.assign(nc + 1, 0);
+  a->merged_ids.resize(nmid);
+  const u64 *cnt = a->hd[1].col[1], *off = a->hd[1].col[2];
+  for (u64 r = 0; r < nc; ++r) {
+    a->merged_off[r + 1] = a->merged_off[r] + cnt[r];
+    std::copy(a->h_mids + off[r], a->h_mids + off[r] + cnt[r], a->merged_ids.begin() + a->merged_off[r]);
+  }
+  a->first_call = a->calls;
+  out->n_closed = nc;
+  out->closed_key = a->hd[0].col[0];
+  out->closed_window_id = (const int64_t*)a->hd[0].col[1];
+  out->closed_handle = a->hd[0].col[2];
+  out->closed_open_us = (const int64_t*)a->hd[0].col[3];
+  out->closed_close_us = (const int64_t*)a->hd[0].col[4];
+  out->closed_epoch = a->hd[1].col[0];
+  out->merged_off = a->merged_off.data();
+  out->merged_ids = a->merged_ids.data();
+  out->n_late = nl;
+  out->late_key = a->hl.col[0];
+  out->late_window_id = (const int64_t*)a->hl.col[1];
+  out->late_epoch = a->hl.col[2];
+  out->late_activation = a->hl.col[3];
+  out->late_row = a->hl.col[4];
+  // handed out until the next advance / eof, then cleared
+  a->released.swap(a->released_out);
+  a->released.clear();
+  out->n_released = a->released_out.size();
+  out->released = a->released_out.data();
+  return BW_OK;
+}
+
+// notify phase or EOF: wake the keys (K8's k_jwin_mark with the windower's notify_at), then close them
+static bw_status argwin_wake(bw_argwin* a, int eof) {
+  bw_ctx* ctx = a->ctx;
+  bw_status st = jwin_drain(a);
+  if (st != BW_OK) return st;
+  if ((st = jwin_room(a, 0)) != BW_OK) return st;
+  const JwParams p = argwin_params(a, a->last_epoch);
+  if (a->spec.session)
+    k_jwin_mark<<<ctx->sm_count * 8, 256, 0, a->s>>>(a->t.j, (const AwSess*)a->t.rec, p, eof, AwNotifyAt{a->t.gap});
+  else
+    k_jwin_mark<<<ctx->sm_count * 8, 256, 0, a->s>>>(a->t.j, (const AwWin*)a->t.win, p, eof);
+  CU(ctx, cudaGetLastError());
+  a->undrained = true;
+  k_awin_close<<<ctx->sm_count * 8, 256, 0, a->s>>>(a->t, a->e, p, a->spec.session);
+  CU(ctx, cudaGetLastError());
+  return BW_OK;
+}
+
+bw_status bw_argwin_advance(bw_argwin* a, int64_t system_now_us, bw_argwin_rows* out) {
+  if (!a || !out) return BW_ERR_SPEC;
+  bw_ctx* ctx = a->ctx;
+  CU(ctx, cudaSetDevice(ctx->device));
+  if (system_now_us > 0) {
+    if (system_now_us > a->now) a->now = system_now_us;
+    bw_status st = argwin_wake(a, 0);
+    if (st != BW_OK) return st;
+  }
+  return argwin_collect(a, out);
+}
+
+bw_status bw_argwin_eof(bw_argwin* a, bw_argwin_rows* out) {
+  if (!a || !out) return BW_ERR_SPEC;
+  bw_ctx* ctx = a->ctx;
+  CU(ctx, cudaSetDevice(ctx->device));
+  bw_status st = argwin_wake(a, 1);
+  if (st != BW_OK) return st;
+  return argwin_collect(a, out);
 }

@@ -598,13 +598,101 @@ class _GpuCollectWindowStep(_GpuJoinWindowStep):
         return rows
 
 
+class _GpuArgWindowStep(_GpuJoinWindowStep):
+    """One worker's ``max_window`` / ``min_window`` with a ``by=`` projection (``GpuArgWindowPlan``) on ``bw_argwin_*``
+    (K11): `_WindowLogic` over a tumbling, sliding or session windower with `_FoldWindowLogic` per window whose folder
+    and merger are ``max(acc, v, key=by)`` (windowing.py:1046-1190, 1692-1714, 2145-2285), one call per activation.
+    Handles, clock sampling, notify, EOF and the key re-sort are the join step's.  ``by`` runs once per item at ingest;
+    its results must all be ints in the int64 range (not bools) or all floats, which the device compares exactly as
+    Python does.  In the first batch anything else sends the step to the host logic; later it raises."""
+
+    def _windower_spec(self, w):
+        from bytewax_b200.operators.windowing import SessionWindower
+
+        self.by_float = None  # whether the by-values are floats: fixed by the step's first one
+        self.gap_us = _td_us(w.gap) if isinstance(w, SessionWindower) else None
+        if self.gap_us is None:
+            super()._windower_spec(w)
+
+    def _unfit(self, what: str, cause=None):
+        if self.jwin is None:  # nothing on the device yet: this step runs on the host logic instead
+            raise _GpuPlanUnfit(what) from cause
+        raise TypeError(f"step {self.step_id!r}: the CUDA arg-max / arg-min needs `by` to give int64 or float64 numbers of one "
+                        f"type for every item; {what}") from cause
+
+    def _by(self, value):
+        try:
+            b = self.plan.by(value)
+        except Exception as ex:
+            self._unfit(f"`by` raised {ex!r} on {value!r}", ex)
+        if isinstance(b, bool) or not isinstance(b, (int, float)) or (isinstance(b, int) and not -(1 << 63) <= b < (1 << 63)):
+            self._unfit(f"`by` gave {b!r} of type {type(b)!r}")
+        is_float = isinstance(b, float)
+        if self.by_float is None:
+            self.by_float = is_float
+        elif is_float != self.by_float:
+            self._unfit(f"`by` gave {b!r} after {'float' if self.by_float else 'int'} values")
+        return b
+
+    def on_epoch(self, epoch: int, items: list) -> list:
+        from bytewax_b200 import gpu
+
+        np, plan = self.np, self.plan
+        getter = getattr(plan.clock, "ts_getter", None)
+        now = self._now_us()
+        if getter is None:  # SystemClock (windowing.py:196-222): an item's timestamp is the system time of its batch
+            now_dt = _dt(now)
+            getter = lambda _v: now_dt  # noqa: E731
+        keys, ts, bys, vals = [], [], [], []
+        for item in items:
+            key, value = _split_item(self.step_id, item)
+            keys.append(self._key_id(key))
+            ts.append(_us(getter(value)))
+            bys.append(self._by(value))
+            vals.append(value)
+        if self.jwin is None:
+            self.jwin = gpu.ArgWindow(
+                _get_gpu_ctx(), plan.extreme, "f64" if self.by_float else "i64", self.length_us if self.gap_us is None else 1,
+                self.offset_us if self.gap_us is None else None, self.align_us if self.gap_us is None else 0, self.gap_us, self.wait_us,
+                capacity_hint=int(os.environ.get("BYTEWAX_B200_KEYS", 1 << 20)),
+                max_windows_per_key=64 if self.gap_us is None else int(os.environ.get("BYTEWAX_B200_SESSIONS", 64)),
+                max_batch_rows=int(os.environ.get("BYTEWAX_B200_BATCH", 1 << 22)), max_emit_rows=1 << 22, max_late_rows=1 << 22)
+        handles = list(range(self.next_handle, self.next_handle + len(vals)))
+        self.next_handle += len(vals)
+        self.values.update(zip(handles, vals))
+        self.last_epoch = max(epoch, self.last_epoch)
+        self.jwin.apply(np.array(keys, dtype=np.uint64), np.array(handles, dtype=np.uint64),
+                        np.array(bys, dtype=np.float64 if self.by_float else np.int64), np.array(ts, dtype=np.int64), self.last_epoch, now or 0)
+        return self._jwin_rows(self.jwin.advance(), vals)
+
+    def _jwin_rows(self, out, vals) -> list:
+        from bytewax_b200.operators.windowing import WindowMetadata
+
+        V = self.values
+        lates = [(self._key_str(k), w, vals[r]) for k, w, r in zip(out.late_key.tolist(), out.late_window_id.tolist(), out.late_row.tolist())]
+        closed = [(self._key_str(k), i) for i, k in enumerate(out.closed_key.tolist())]
+        if self.resort:  # interned (non-numeric) keys: restore ascending key-string order; stable
+            lates.sort(key=lambda r: r[0])
+            closed.sort(key=lambda r: r[0])
+        rows = [(ks, (w, "L", v)) for ks, w, v in lates]
+        wid, hs = out.closed_window_id.tolist(), out.closed_handle.tolist()
+        o, c = out.closed_open_us.tolist(), out.closed_close_us.tolist()
+        for ks, i in closed:
+            meta = WindowMetadata(_dt(o[i]), _dt(c[i])) if self.gap_us is None else WindowMetadata(_dt(o[i]), _dt(c[i]), set(out.merged(i)))
+            rows.append((ks, (wid[i], "E", V[hs[i]])))
+            rows.append((ks, (wid[i], "M", meta)))
+        for h in out.released.tolist():  # after this call's rows are built: no later row can name these
+            del V[h]
+        return rows
+
+
 def _td_us(td: timedelta) -> int:
     return (td.days * 86400 + td.seconds) * 1_000_000 + td.microseconds
 
 
 def _gpu_step_for(step_id: str, plan):
     from bytewax_b200.operators import GpuFinalPlan, GpuJoinPlan, GpuSmapPlan
-    from bytewax_b200.operators.windowing import GpuCollectWindowPlan, GpuJoinWindowPlan, SessionWindower
+    from bytewax_b200.operators.windowing import GpuArgWindowPlan, GpuCollectWindowPlan, GpuJoinWindowPlan, SessionWindower
 
     if isinstance(plan, GpuJoinWindowPlan):
         if isinstance(plan.windower, SessionWindower):
@@ -612,6 +700,8 @@ def _gpu_step_for(step_id: str, plan):
         return _GpuJoinWindowStep(step_id, plan)
     if isinstance(plan, GpuCollectWindowPlan):
         return _GpuCollectWindowStep(step_id, plan)
+    if isinstance(plan, GpuArgWindowPlan):  # (before the SessionWindower check below, which would catch it)
+        return _GpuArgWindowStep(step_id, plan)
     if isinstance(getattr(plan, "windower", None), SessionWindower):
         return _GpuSessionStep(step_id, plan)
     if isinstance(plan, GpuSmapPlan):

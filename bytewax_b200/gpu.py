@@ -791,3 +791,110 @@ class CollectWindow:
         if self.h:
             self.lib.bw_collect_destroy(self.h)
             self.h = None
+
+
+@dataclass
+class ArgWindowRows:
+    """Rows of one ``ArgWindow.advance`` / ``eof``, each stream in the reference's downstream order, and the handles
+    released since the previous one.  Each closed row is a window's ``E`` row (the pick's handle) followed by its ``M``
+    row ``WindowMetadata(open, close[, merged ids])``.  Session late rows have window id -1 (``LATE_SESSION_ID``)."""
+
+    closed_key: np.ndarray
+    closed_window_id: np.ndarray
+    closed_handle: np.ndarray
+    closed_open_us: np.ndarray
+    closed_close_us: np.ndarray
+    closed_epoch: np.ndarray
+    merged_off: np.ndarray  # [n_closed + 1] into merged_ids
+    merged_ids: np.ndarray
+    late_key: np.ndarray
+    late_window_id: np.ndarray
+    late_epoch: np.ndarray
+    late_activation: np.ndarray
+    late_row: np.ndarray
+    released: np.ndarray  # uint64, in no particular order
+
+    def merged(self, i: int) -> List[int]:
+        """The ids merged directly into closed row ``i``'s session, ascending (none for tumbling / sliding windows)."""
+        return self.merged_ids[self.merged_off[i] : self.merged_off[i + 1]].tolist()
+
+
+class ArgWindow:
+    """``max_window`` / ``min_window`` with a ``by=`` projection over tumbling, sliding or session windows (``bw_argwin``,
+    K11; windowing.py:1046-1190, 1692-1714, 2145-2285).  Items travel as uint64 handles with their by-values (int64 or
+    float64); the caller keeps the items and may drop each one once its handle comes back in ``released``."""
+
+    EXTREME = {"max": N.RED["max"], "min": N.RED["min"]}
+
+    def __init__(self, ctx: Context, extreme: str = "max", by_dtype: str = "i64", length_us: int = 10_000_000,
+                 offset_us: Optional[int] = None, align_us: int = 0, gap_us: Optional[int] = None, wait_us: Optional[int] = 0,
+                 capacity_hint: int = 1 << 16, max_windows_per_key: int = 16, max_batch_rows: int = 1 << 20,
+                 max_emit_rows: int = 1 << 20, max_late_rows: int = 1 << 20):
+        """``gap_us`` set: session windows (``length_us`` / ``offset_us`` / ``align_us`` unused).  ``offset_us=None``:
+        tumbling.  ``wait_us=None``: the watermark never advances on data (``BW_WAIT_FOREVER``)."""
+        self.ctx, self.lib = ctx, ctx.lib
+        self.by_dtype = by_dtype
+        s = N.BwArgwinSpec()
+        s.struct_size = C.sizeof(N.BwArgwinSpec)
+        s.extreme, s.by_dtype = self.EXTREME.get(extreme, -1), N.VAL.get(by_dtype, -1)
+        s.session, s.max_windows_per_key = int(gap_us is not None), max_windows_per_key
+        s.length_us, s.offset_us, s.align_us = length_us, length_us if offset_us is None else offset_us, align_us
+        s.gap_us = 0 if gap_us is None else gap_us
+        s.wait_us = N.BW_WAIT_FOREVER if wait_us is None else wait_us
+        s.capacity_hint, s.max_batch_rows, s.max_emit_rows, s.max_late_rows = capacity_hint, max_batch_rows, max_emit_rows, max_late_rows
+        self.spec = s
+        h = C.c_void_p()
+        N.check(self.lib.bw_argwin_create(ctx.h, C.byref(s), C.byref(h)), ctx.h)
+        self.h = h
+        self._epoch = 0
+
+    def _next_epoch(self, epoch: Optional[int]) -> int:
+        if epoch is None:
+            self._epoch += 1
+            epoch = self._epoch
+        return epoch
+
+    def apply(self, keys, handles, by, ts_us, epoch: Optional[int] = None, system_now_us: int = 0):
+        """One activation from host arrays; ``by`` holds the by-values (int64 or float64 as the step's ``by_dtype``).
+        ``system_now_us``: ``now_getter()`` of the activation."""
+        keys = np.ascontiguousarray(keys, dtype=np.uint64)
+        handles = np.ascontiguousarray(handles, dtype=np.uint64)
+        b = np.ascontiguousarray(by, dtype=np.float64 if self.by_dtype == "f64" else np.int64)
+        ts = np.ascontiguousarray(ts_us, dtype=np.int64)
+        epoch = self._next_epoch(epoch)
+        vp = lambda a: a.ctypes.data_as(C.c_void_p)  # noqa: E731
+        N.check(self.lib.bw_argwin_apply(self.h, vp(keys), vp(handles), vp(b), vp(ts), keys.shape[0], epoch, int(system_now_us)), self.ctx.h)
+
+    def apply_device(self, d_keys: int, d_handles: int, d_by: int, d_ts: int, rows: int, epoch: Optional[int] = None,
+                     system_now_us: int = 0):
+        epoch = self._next_epoch(epoch)
+        N.check(self.lib.bw_argwin_apply_device(self.h, C.c_void_p(d_keys), C.c_void_p(d_handles), C.c_void_p(d_by), C.c_void_p(d_ts),
+                                                rows, epoch, int(system_now_us)), self.ctx.h)
+
+    def _wrap(self, r: N.BwArgwinRows) -> ArgWindowRows:
+        nc, nl, nr = int(r.n_closed), int(r.n_late), int(r.n_released)
+
+        def arr(ptr, n, dt=np.uint64):
+            return np.ctypeslib.as_array(ptr, shape=(n,)).view(dt).copy() if n else np.zeros(0, dt)
+
+        off = arr(r.merged_off, nc + 1).astype(np.int64)
+        return ArgWindowRows(arr(r.closed_key, nc), arr(r.closed_window_id, nc, np.int64), arr(r.closed_handle, nc),
+                             arr(r.closed_open_us, nc, np.int64), arr(r.closed_close_us, nc, np.int64), arr(r.closed_epoch, nc), off,
+                             arr(r.merged_ids, int(off[-1]), np.int64), arr(r.late_key, nl), arr(r.late_window_id, nl, np.int64),
+                             arr(r.late_epoch, nl), arr(r.late_activation, nl), arr(r.late_row, nl), arr(r.released, nr))
+
+    def advance(self, system_now_us: int = 0) -> ArgWindowRows:
+        """Rows since the last call; ``system_now_us`` > 0 first runs the notify phase at that system time."""
+        r = N.BwArgwinRows()
+        N.check(self.lib.bw_argwin_advance(self.h, int(system_now_us), C.byref(r)), self.ctx.h)
+        return self._wrap(r)
+
+    def eof(self) -> ArgWindowRows:
+        r = N.BwArgwinRows()
+        N.check(self.lib.bw_argwin_eof(self.h, C.byref(r)), self.ctx.h)
+        return self._wrap(r)
+
+    def close(self):
+        if self.h:
+            self.lib.bw_argwin_destroy(self.h)
+            self.h = None

@@ -687,17 +687,40 @@ def reduce_window(step_id: str, up: KeyedStream, clock: Clock, windower: Windowe
     return fold_window("fold_window", up, clock, windower, _untyped_none, shim_folder, reducer, ordered=False, _gpu_plan=plan)
 
 
+@dataclass(frozen=True)
+class GpuArgWindowPlan:
+    """A ``max_window`` / ``min_window`` with a ``by=`` projection the engine may run with ``bw_argwin_*`` (K11): a
+    tumbling, sliding or session windower and an `EventClock` with an identity ``to_system_utc`` or a `SystemClock`.
+    Items travel as handles into a host-side dict with the number ``by`` gives each; ``by`` runs once per item at
+    ingest, so it must be pure and defined on every item, late ones included."""
+
+    extreme: str  # max | min
+    by: Callable[[Any], Any]
+    clock: Any
+    windower: Any
+
+
+def _arg_window_plan(extreme, by, clock, windower) -> Optional[GpuArgWindowPlan]:
+    # a custom `to_system_utc` moves the notify time away from the event time the device compares with the system clock
+    # (windowing.py:1177-1178): host engine
+    if not isinstance(windower, (SlidingWindower, TumblingWindower, SessionWindower)):
+        return None
+    if not (isinstance(clock, SystemClock) or (isinstance(clock, EventClock) and clock.to_system_utc is _identity)):
+        return None
+    return GpuArgWindowPlan(extreme, by, clock, windower)
+
+
 @operator
 def max_window(step_id: str, up: KeyedStream, clock: Clock, windower: Windower, by: Callable[[Any], Any] = _identity) -> WindowOut:
     """windowing.py:2145."""
-    plan = _plan_for("max", clock, windower, False) if by is _identity else None
+    plan = _plan_for("max", clock, windower, False) if by is _identity else _arg_window_plan("max", by, clock, windower)
     return reduce_window("reduce_window", up, clock, windower, partial(max, key=by), _gpu_plan=plan)
 
 
 @operator
 def min_window(step_id: str, up: KeyedStream, clock: Clock, windower: Windower, by: Callable[[Any], Any] = _identity) -> WindowOut:
     """windowing.py:2192."""
-    plan = _plan_for("min", clock, windower, False) if by is _identity else None
+    plan = _plan_for("min", clock, windower, False) if by is _identity else _arg_window_plan("min", by, clock, windower)
     return reduce_window("reduce_window", up, clock, windower, partial(min, key=by), _gpu_plan=plan)
 
 

@@ -669,6 +669,85 @@ bw_status bw_sjwin_advance(bw_sjwin* j, int64_t system_now_us, bw_sjwin_rows* ou
 /* End of input: every key flushes at watermark UTC_MAX (:1144-1151), so sessions with close >= UTC_MAX - gap stay open. */
 bw_status bw_sjwin_eof(bw_sjwin* j, bw_sjwin_rows* out);
 
+/* Windowed arg-max / arg-min (K11): `max_window` / `min_window` with a `by=` projection
+ * (pysrc/bytewax/operators/windowing.py:2145-2236), i.e. `reduce_window(partial(max, key=by))` = `fold_window(ordered=
+ * False)` (:2268-2285) with `_FoldWindowLogic` (:1692-1714) per window, over `_SlidingWindowerLogic` (:603-668; tumbling
+ * == offset equal to length) or `_SessionWindowerLogic` (:671-810).  Items travel as u64 handles (any u64) with their
+ * by-value (i64 or f64 bits, the caller's `by(item)`); the objects stay with the caller.  Per key, per call, in order:
+ * the EventClock's late test per item (:263-287; a late item gives one row per id of `intersects(ts)`, ascending, or
+ * for sessions one row with window LATE_SESSION_ID = -1); then every on-time item in arrival order goes to every window
+ * of `open_for(ts)` (or to the session `open_for` returns, even one a merge just took away, :1064-1077): the first value
+ * seeds the window's pick, a later one replaces it only if its by-value is strictly greater (max) / less (min) -- i64
+ * compared signed, f64 by IEEE, so ties, -0.0 == +0.0 and NaN keep the earlier pick; then, for sessions, the merge
+ * queue in discovery order (:1079-1085) with `into = max(into, orig, key=by)`; then `_handle_closed` (:1087-1093):
+ * windows with close <= watermark in first-opened order, or sessions with close < watermark - gap in id order.  A
+ * tumbling / sliding key with no open window is discarded, clock included (:1110-1113); session state never is
+ * (:798-806).  One GPU only. */
+typedef struct bw_argwin bw_argwin;
+typedef struct bw_argwin_spec {
+  uint32_t struct_size;
+  int32_t extreme;              /* BW_RED_MAX / BW_RED_MIN */
+  int32_t by_dtype;             /* BW_VAL_I64 / BW_VAL_F64: what the by-value bits hold */
+  int32_t session;              /* 0: tumbling / sliding (length_us, offset_us, align_us); 1: SessionWindower (gap_us) */
+  int32_t max_windows_per_key;  /* 1..64 open windows per key; sessions: sessions a key holds during a call (live ones,
+                                   plus those merged away in it), and also the merged ids its live sessions hold */
+  int32_t pad;
+  int64_t length_us;            /* window length, > 0 */
+  int64_t offset_us;            /* 0 < offset <= length (TumblingWindower: == length) */
+  int64_t align_us;             /* align_to */
+  int64_t gap_us;               /* SessionWindower.gap, >= 0 (windowing.py:938-943) */
+  int64_t wait_us;              /* EventClock.wait_for_system_duration, or BW_WAIT_FOREVER */
+  uint64_t capacity_hint;       /* live keys (sessions: keys ever seen); a key's slot is kept once seen */
+  uint64_t max_batch_rows;
+  uint64_t max_emit_rows;       /* closed rows, and their merged ids, retained between bw_argwin_advance calls */
+  uint64_t max_late_rows;       /* late rows retained between bw_argwin_advance calls */
+} bw_argwin_spec;
+/* Rows handed downstream since the last advance / eof, in the reference's order: per call (activation, notify phase
+ * or EOF), ascending key string (src/operators.rs:758-767, :862-894); within a key closed rows in first-opened order
+ * (sessions: id order), late rows in arrival order.  Each closed row is the `E` row (the pick's handle) and its `M` row
+ * WindowMetadata(open, close[, merged_ids]).  Host pointers into memory owned by the library, valid until the next
+ * advance / eof / destroy. */
+typedef struct bw_argwin_rows {
+  uint64_t n_closed;
+  const uint64_t* closed_key;
+  const int64_t* closed_window_id;
+  const uint64_t* closed_handle;  /* the pick */
+  const int64_t* closed_open_us;
+  const int64_t* closed_close_us;
+  const uint64_t* closed_epoch;   /* the epoch of the activation, or of the last one before a notify / EOF */
+  const uint64_t* merged_off;     /* [n_closed + 1]: row i merged ids are merged_ids[merged_off[i] .. merged_off[i+1]) */
+  const int64_t* merged_ids;      /* ascending per row; none for tumbling / sliding windows */
+  uint64_t n_late;
+  const uint64_t* late_key;
+  const int64_t* late_window_id;
+  const uint64_t* late_epoch;
+  const uint64_t* late_activation; /* (activation, row) name the input row (activations counted from 0) */
+  const uint64_t* late_row;
+  /* handles no window holds any more; each handle passed to apply is listed exactly once, in the rows of the call that
+   * let go of it: a late item's, and a value that is the pick of none of its windows, in the call that received it; a
+   * pick replaced in the last window holding it, or losing a session merge; a pick when the last window holding it
+   * closes */
+  uint64_t n_released;           /* (the device buffer behind it grows with the handles held, never with the table size) */
+  const uint64_t* released;
+} bw_argwin_rows;
+bw_status bw_argwin_create(bw_ctx* ctx, const bw_argwin_spec* spec, bw_argwin** out);
+void bw_argwin_destroy(bw_argwin* a);
+/* One activation from HOST columns (keys, handle, by-value bits, ts); blocks.  `system_now_us` is `now_getter()` for
+ * this activation (windowing.py:250-261; it must not go backwards; 0 throughout = a frozen clock).  A full key table,
+ * more than max_windows_per_key windows / sessions / merged ids, or a full emit or late buffer returns BW_ERR_CAPACITY
+ * (reason in bw_last_error) and the step refuses further calls. */
+bw_status bw_argwin_apply(bw_argwin* a, const uint64_t* keys, const uint64_t* handles, const uint64_t* by_bits, const int64_t* ts_us,
+                          uint64_t rows, uint64_t epoch, int64_t system_now_us);
+/* Same with DEVICE columns; returns once the work is enqueued (the columns must stay valid until the next call). */
+bw_status bw_argwin_apply_device(bw_argwin* a, const uint64_t* d_keys, const uint64_t* d_handles, const uint64_t* d_by_bits,
+                                 const int64_t* d_ts_us, uint64_t rows, uint64_t epoch, int64_t system_now_us);
+/* Rows since the last call.  `system_now_us` > 0 first runs the notify phase at that system time
+ * (src/operators.rs:808-858, windowing.py:1135-1142, 1153-1180 with an identity `to_system_utc`): every key whose
+ * earliest window close (sessions: earliest close + gap) has been reached closes what its watermark allows. */
+bw_status bw_argwin_advance(bw_argwin* a, int64_t system_now_us, bw_argwin_rows* out);
+/* End of input: every key closes at watermark UTC_MAX (:1144-1151), so sessions with close >= UTC_MAX - gap stay open. */
+bw_status bw_argwin_eof(bw_argwin* a, bw_argwin_rows* out);
+
 /* ---- plain device-memory helpers (tests / bench / host bindings without torch) ---- */
 bw_status bw_dev_alloc(bw_ctx* ctx, uint64_t bytes, void** out);
 bw_status bw_dev_free(bw_ctx* ctx, void* ptr);
