@@ -253,42 +253,6 @@ struct Stage {  // device staging for host-ingested batches
   bool used = false;
 };
 
-// optional per-phase timing (env BW_TIMING=1): events on the streams, summed at destroy
-struct PhaseTimer {
-  static const int NPH = 8;
-  const char* names[NPH] = {"part_hist+scan+scatter", "barrier", "prepass", "fold", "close", "scatter + verdict", "segfold", "spill + close"};
-  std::vector<cudaEvent_t> ev[NPH][2];
-  bool on = false;
-  Owner* own = nullptr;  // the fold's
-  void mark(int ph, int which, cudaStream_t s) {
-    cudaEvent_t e;
-    if (!on || own->event(&e, cudaEventDefault) != cudaSuccess) return;
-    cudaEventRecord(e, s);
-    ev[ph][which].push_back(e);
-  }
-  void report(int rank) {
-    if (!on) return;
-    for (int p = 0; p < NPH; ++p) {
-      size_t n = std::min(ev[p][0].size(), ev[p][1].size());
-      if (!n) continue;
-      double tot = 0, mn = 1e30, mx = 0;
-      std::vector<float> all;
-      for (size_t i = 0; i < n; ++i) {
-        float ms = 0;
-        if (cudaEventElapsedTime(&ms, ev[p][0][i], ev[p][1][i]) == cudaSuccess) {
-          tot += ms;
-          mn = std::min<double>(mn, ms);
-          mx = std::max<double>(mx, ms);
-          all.push_back(ms);
-        }
-      }
-      std::sort(all.begin(), all.end());
-      fprintf(stderr, "[bwgpu rank %d] %-24s n=%zu avg %.3f ms (min %.3f, median %.3f, max %.3f)\n", rank, names[p], n, tot / n, mn,
-              all.empty() ? 0.0 : all[all.size() / 2], mx);
-    }
-  }
-};
-
 struct EventPair {
   cudaEvent_t a, b;
   u64 rows;
@@ -371,11 +335,13 @@ struct bw_fold {
   Counters* d_ctr = nullptr;
   Counters* h_ctr = nullptr;  // pinned mirror
   cudaStream_t s_compute = nullptr, s_copy = nullptr, s_pre = nullptr, s_x = nullptr;  // s_x: partition + exchange
-  cudaEvent_t ev_fold_done = nullptr, ev_xchg_done = nullptr, ev_src_ready = nullptr;
+  cudaEvent_t ev_fold_done = nullptr, ev_xchg_done = nullptr;
   bool fold_recorded = false;
   cudaEvent_t ev_gen = nullptr;      // last bw_gen_c1 (the only producer of device columns this library runs itself)
-  cudaEvent_t pre_wait = nullptr;    // what the verdict pass of the activation in flight has to wait for, if anything
-  cudaEvent_t ev_in = nullptr, ev_pre = nullptr, ev_h2d = nullptr, ev_t0 = nullptr, ev_t1 = nullptr;
+  // the columns of the activation in flight are complete once this has happened (null: nothing to wait for); the
+  // lateness pass on s_pre and the exchange on s_x wait on it
+  cudaEvent_t cols_ready = nullptr;
+  cudaEvent_t ev_pre = nullptr, ev_h2d = nullptr, ev_t0 = nullptr, ev_t1 = nullptr;
   int val_bytes = 8;
   bool has_vals = true, has_ts = false;
   // ingest
@@ -456,7 +422,7 @@ struct bw_fold {
   i64* late_chunk_pre = nullptr;  // [tiles][32] running maximum before every 64-row chunk
   Deferred dq{};            // the activation whose fold has not been launched yet
   i64* d_span = nullptr;   // [min ts, max ts] of the activation (prepass)
-  // snapshot staging (bw_snapshot_take)
+  // snapshot staging (bw_snapshot_take, bw_snapshot_load)
   void* snap_dev = nullptr;
   void* snap_host = nullptr;
   unsigned long long* d_snap_ctr = nullptr;
@@ -479,7 +445,6 @@ struct bw_fold {
   bw_stats st{};
   std::vector<EventPair> timers;
   size_t timers_used = 0;
-  PhaseTimer pt;
 };
 
 #define FAIL(f, code, ...) CTX_FAIL((f)->ctx, code, __VA_ARGS__)
@@ -925,15 +890,13 @@ static bw_status fold_alloc(bw_fold* f) {
     CU(ctx, cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi));
     CU(ctx, own.stream(&f->s_pre, prio_hi));
   }
-  if (getenv("BW_NO_OVERLAP")) f->s_x = f->s_compute;  // diagnostic: serialise exchange and fold
-  else CU(ctx, own.stream(&f->s_x));
-  for (cudaEvent_t* e : {&f->ev_fold_done, &f->ev_xchg_done, &f->ev_src_ready, &f->ev_in, &f->ev_pre, &f->ev_h2d})
+  CU(ctx, own.stream(&f->s_x));
+  for (cudaEvent_t* e : {&f->ev_fold_done, &f->ev_xchg_done, &f->ev_pre, &f->ev_h2d})
     CU(ctx, own.event(e));
   // No persisting-L2 carve-out: a persisting window on the hot slots would leave too little normal
   // L2 for the second-pane array at window boundaries; plain LRU + evict_first input loads instead.
   int occ = 0;
   f->fold_kernel = pick_fold_kernel(f->p);
-  f->pt.on = getenv("BW_TIMING") != nullptr;
   if (const char* e = getenv("BW_SUB_AUTO")) f->sub_auto = atoi(e) != 0;
   if (const char* e = getenv("BW_SUB_ROWS")) {
     long long v = atoll(e);
@@ -944,7 +907,7 @@ static bw_status fold_alloc(bw_fold* f) {
   f->fold_grid = ctx->sm_count * occ;
   // multi-GPU: leave register-file room on every SM so the next activation's partition/scatter
   // (NVLink-bound, on its own stream) can really run beside the fold instead of queueing behind it
-  if (ctx->world > 1 && occ > 2 && !getenv("BW_FOLD_FULL")) f->fold_grid = ctx->sm_count * 2;
+  if (ctx->world > 1 && occ > 2) f->fold_grid = ctx->sm_count * 2;
   f->close_grid = ctx->sm_count * 8;
   {
     bw_status st = stream_alloc(f);
@@ -1032,7 +995,6 @@ bw_status bw_fold_create(bw_ctx* ctx, const bw_fold_spec* spec, bw_fold** out) {
   bw_fold* f = fp.get();
   f->ctx = ctx;
   f->spec = *spec;
-  f->pt.own = &f->own;
   FoldParams& p = f->p;
   p.length_us = spec->length_us;
   p.offset_us = spec->offset_us;
@@ -1116,7 +1078,6 @@ void bw_fold_destroy(bw_fold* f) {
   cudaSetDevice(f->ctx->device);
   stream_resolve(f);
   cudaDeviceSynchronize();
-  f->pt.report(f->ctx->rank);
   for (int r = 0; r < f->ctx->world; ++r)
     if (r != f->ctx->rank && !f->ctx->loop) {
       if (f->peer_base[r] && f->spec.exchange == BW_XCHG_P2P) cudaIpcCloseMemHandle(f->peer_base[r]);
@@ -1161,22 +1122,26 @@ bw_status bw_ingest_acquire(bw_fold* f, uint64_t max_rows, bw_batch* out) {
   return BW_OK;
 }
 
-// CUDA-event pair for one kernel launch of activation `batch_no`.  Every record with timing drains the stream for a few
-// microseconds, so only every timer_stride-th activation is timed (env BW_TIMER_STRIDE, default 4): the averages in bw_stats
-// are over that sample.
-static EventPair* next_timer(bw_fold* f, u32 batch_no) {
-  if (f->timer_stride > 1 && batch_no % f->timer_stride != 0) return nullptr;
+// Time one kernel launch of activation `batch_no` on `s`: timer_begin before it, timer_end after it (`kind` and `rows` as
+// in EventPair).  Every record with timing drains the stream for a few microseconds, so only every timer_stride-th
+// activation is timed (env BW_TIMER_STRIDE, default 4): the averages in bw_stats are over that sample.  *ep is null when
+// the launch is not timed.
+static cudaError_t timer_begin(bw_fold* f, EventPair** ep, u32 batch_no, int kind, u64 rows, cudaStream_t s) {
+  *ep = nullptr;
+  if (f->timer_stride > 1 && batch_no % f->timer_stride != 0) return cudaSuccess;
   if (f->timers_used == f->timers.size()) {
-    if (f->timers.size() >= 4096) return nullptr;
-    EventPair ep;
-    if (f->own.event(&ep.a, cudaEventDefault) != cudaSuccess || f->own.event(&ep.b, cudaEventDefault) != cudaSuccess) return nullptr;
-    ep.rows = 0;
-    ep.kind = 0;
-    f->timers.push_back(ep);
+    if (f->timers.size() >= 4096) return cudaSuccess;
+    EventPair e;
+    if (f->own.event(&e.a, cudaEventDefault) != cudaSuccess || f->own.event(&e.b, cudaEventDefault) != cudaSuccess) return cudaSuccess;
+    f->timers.push_back(e);
   }
-  return &f->timers[f->timers_used++];
+  *ep = &f->timers[f->timers_used++];
+  (*ep)->rows = rows;
+  (*ep)->kind = kind;
+  return cudaEventRecord((*ep)->a, s);
 }
 
+static cudaError_t timer_end(const EventPair* ep, cudaStream_t s) { return ep ? cudaEventRecord(ep->b, s) : cudaSuccess; }
 
 // Partition + exchange of this rank's rows; fills `bv` with the received segments.
 static bw_status exchange(bw_fold* f, const u64* d_keys, const void* d_vals, const i64* d_ts, u64 rows, BatchView* bv) {
@@ -1184,10 +1149,10 @@ static bw_status exchange(bw_fold* f, const u64* d_keys, const void* d_vals, con
   const int W = ctx->world, R = ctx->rank;
   // Partition + exchange run on their own stream so that the scatter of activation b+1 (NVLink-bound)
   // overlaps the fold of activation b.  The producer of the input columns is ordered before it through
-  // ev_src_ready; the barrier waits for this rank's fold of the previous activation, which is what makes
+  // cols_ready; the barrier waits for this rank's fold of the previous activation, which is what makes
   // the double-buffered receive regions safe to overwrite two activations later.
   cudaStream_t s = f->s_x;
-  CU(ctx, cudaStreamWaitEvent(s, f->ev_src_ready, 0));
+  if (f->cols_ready) CU(ctx, cudaStreamWaitEvent(s, f->cols_ready, 0));
   const int buf = f->xbuf;
   f->xbuf ^= 1;
   XLayout L = xlayout(f);
@@ -1219,18 +1184,15 @@ static bw_status exchange(bw_fold* f, const u64* d_keys, const void* d_vals, con
   }
   const u64 ntiles = (rows + BW_PART_TILE - 1) / BW_PART_TILE;
   int grid = (int)std::min<u64>(std::max<u64>(ntiles, 1), (u64)ctx->sm_count * 8);
-  f->pt.mark(0, 0, s);
   k_part_hist<<<grid, BW_PART_THREADS, 0, s>>>(in, f->d_tile_counts);
   k_part_scan<<<W, 1024, 0, s>>>(rows, W, f->d_tile_counts, po, f->d_ctr);
   const size_t stage_bytes = (size_t)BW_PART_TILE * (8 + (size_t)in.val_bytes + (in.ts ? 8 : 0));
   k_part_scatter<<<grid, BW_PART_THREADS, stage_bytes, s>>>(in, f->d_tile_counts, po);
   CU(ctx, cudaGetLastError());
   f->st.kernel_launches += 3;
-  f->pt.mark(0, 1, s);
   char* mine = (char*)f->xchg_base;
   u64* my_counts = (u64*)(mine + L.counts_off[buf]);
   if (f->fold_recorded) CU(ctx, cudaStreamWaitEvent(s, f->ev_fold_done, 0));
-  f->pt.mark(1, 0, s);
   if (p2p) {
     // every rank's stores are complete once it enters this collective (stream
     // order); its completion here means all peers have entered it.
@@ -1268,7 +1230,6 @@ static bw_status exchange(bw_fold* f, const u64* d_keys, const void* d_vals, con
     // recv_counts is a stack array: make the copy complete before returning
     CU(ctx, cudaStreamSynchronize(s));
   }
-  f->pt.mark(1, 1, s);
   memset(bv, 0, sizeof *bv);
   bv->nseg = W;
   bv->counts_on_device = 1;
@@ -1285,12 +1246,10 @@ static bw_status exchange(bw_fold* f, const u64* d_keys, const void* d_vals, con
 // K4 for the keys the fold marked, then the end-of-activation resets
 static bw_status close_stage(bw_fold* f, u64 ord, u32 batch_no, StreamVerdict* sv) {
   bw_ctx* ctx = f->ctx;
-  f->pt.mark(4, 0, f->s_compute);
   k_close_dirty<<<f->close_grid, 256, 0, f->s_compute>>>(f->t, f->p, f->e, ord, batch_no);
   k_stream_reset<<<1, 1, 0, f->s_compute>>>(f->t, sv);
   CU(ctx, cudaGetLastError());
   f->st.kernel_launches += 2;
-  f->pt.mark(4, 1, f->s_compute);
   return BW_OK;
 }
 
@@ -1319,22 +1278,14 @@ static bw_status direct_fold(bw_fold* f, const BatchView& bv, u64 known, u32 bat
   if (n_sub < 1) n_sub = 1;
   for (u32 i = 0; i < n_sub; ++i) {
     const u64 n_hi = (known * (i + 1ULL)) / n_sub, n_lo = (known * (u64)i) / n_sub;
-    EventPair* ep = next_timer(f, batch_no);
-    if (ep) {
-      ep->rows = (ctx->world > 1) ? 0 : (n_hi - n_lo);
-      ep->kind = 0;
-      CU(ctx, cudaEventRecord(ep->a, f->s_compute));
-    }
+    EventPair* ep;
+    CU(ctx, timer_begin(f, &ep, batch_no, 0, (ctx->world > 1) ? 0 : (n_hi - n_lo), f->s_compute));
     int grid = (int)std::min<u64>((n_hi - n_lo + tile - 1) / tile + 1, (u64)f->fold_grid);
     f->fold_kernel<<<grid, BW_FOLD_THREADS, 0, f->s_compute>>>(bv, f->t, f->p, batch_no, i, n_sub);
     CU(ctx, cudaGetLastError());
-    if (ep) CU(ctx, cudaEventRecord(ep->b, f->s_compute));
+    CU(ctx, timer_end(ep, f->s_compute));
     f->st.kernel_launches++;
     f->st.fold_launches++;
-    if (f->pt.on && ep) {
-      f->pt.ev[3][0].push_back(ep->a);
-      f->pt.ev[3][1].push_back(ep->b);
-    }
     if (i + 1 < n_sub) {
       k_close_dirty<<<f->close_grid, 256, 0, f->s_compute>>>(f->t, f->p, f->e, ord, batch_no);
       k_reset_dirty<<<1, 1, 0, f->s_compute>>>(f->t);
@@ -1397,28 +1348,17 @@ static bw_status stream_front(bw_fold* f, const u64* d_keys, const void* d_vals,
   const int grid = (int)std::min<u64>(ntiles, (u64)std::min<u32>((u32)f->scatter_grid, sb.nlanes));
   f->last_scatter_grid = (u32)grid;
   if (multi && !usable && rows) CU(ctx, cudaMemsetAsync(&sb.side[side].sv->flags, 0xFF, sizeof(u32), s));  // every flag: legacy path
-  EventPair* ep = next_timer(f, batch_no);
-  if (ep) {
-    ep->rows = rows;
-    ep->kind = 1;
-    CU(ctx, cudaEventRecord(ep->a, s));
-  }
-  f->pt.mark(5, 0, s);
+  EventPair* ep;
+  CU(ctx, timer_begin(f, &ep, batch_no, 1, rows, s));
   if (grid) f->scatter_kernel<<<grid, BW_SC_THREADS, f->scatter_smem, s>>>(A, f->p);
-  if (ep) CU(ctx, cudaEventRecord(ep->b, s));  // (the scatter kernel alone: the one-block verdict is timed apart)
-  EventPair* ev = next_timer(f, batch_no);
-  if (ev) {
-    ev->rows = 0;
-    ev->kind = 2;
-    CU(ctx, cudaEventRecord(ev->a, s));
-  }
+  CU(ctx, timer_end(ep, s));  // (the scatter kernel alone: the one-block verdict is timed apart)
+  CU(ctx, timer_begin(f, &ep, batch_no, 2, 0, s));
   if (f->p.ts_from_value == 2) k_verdict_none<<<1, 1, 0, s>>>(f->p, f->d_ctr, sb.side[side].sv, vg, rows);
   else
     k_verdict<<<1, 1024, 0, s>>>(A.tile_min, A.tile_max, A.tile_bad, (u32)ntiles, f->p, f->d_ctr, sb.side[side].sv,
                                  f->has_ts ? d_ts : nullptr, (const u64*)d_vals, vg);
   CU(ctx, cudaGetLastError());
-  f->pt.mark(5, 1, s);
-  if (ev) CU(ctx, cudaEventRecord(ev->b, s));
+  CU(ctx, timer_end(ep, s));
   f->st.kernel_launches += 2;
   CU(ctx, cudaMemcpyAsync(&f->h_sv[side], sb.side[side].sv, sizeof(StreamVerdict), cudaMemcpyDeviceToHost, s));
   if (multi) f->vg_pending[side] = true;  // gathered by the next collective on the stream (gather_verdict)
@@ -1428,88 +1368,78 @@ static bw_status stream_front(bw_fold* f, const u64* d_keys, const void* d_vals,
 
 static bw_status slow_path(bw_fold* f, const BatchView& bv, u64 total, u64 epoch_ord, u32 batch_no);
 
-// The direct path of one activation, start to finish: (world > 1: partition + exchange of the rows) -> lateness pass ->
-// k_fold or the exact path -> K4.
-static bw_status legacy_batch(bw_fold* f, const u64* d_keys, const void* d_vals, const i64* d_ts, u64 rows, u32 batch_no, u64 ord, Stage* stage) {
-  bw_ctx* ctx = f->ctx;
+// The caller's columns of activation d as one segment.
+static BatchView one_segment(const bw_fold* f, const Deferred& d) {
   BatchView bv;
   memset(&bv, 0, sizeof bv);
-  u64 max_total = rows;
+  bv.nseg = 1;
+  bv.keys[0] = d.d_keys;
+  bv.vals[0] = d.d_vals;
+  bv.ts[0] = f->has_ts ? d.d_ts : nullptr;
+  bv.h_counts[0] = d.rows;
+  bv.max_rows = d.rows;
+  return bv;
+}
+
+// The segment-fold arguments of streamed activation d that every mode shares.  The span (ts0, q_lo, npass) and the
+// multi-GPU fields are the caller's.
+static SegArgs seg_args(const bw_fold* f, const Deferred& d) {
+  const StreamBufs& sb = f->sb;
+  SegArgs A;
+  memset(&A, 0, sizeof A);
+  A.in = sb.side[d.side];
+  A.nb = sb.nb;
+  A.nlanes = sb.nlanes;
+  A.lane_cap = sb.lane_cap;
+  A.nlanes_used = d.lanes;
+  A.spill_cap = sb.spill_cap;
+  A.val_bytes = sb.val_bytes;
+  A.seg_shift = f->t.seg_shift;
+  A.batch_no = d.batch_no;
+  A.epoch = d.ord;
+  return A;
+}
+
+// The lateness pass over activation d's rows on this rank (bw_prepass.cuh); on world > 1 behind the partition + exchange
+// of the raw rows, which point *bv at the received segments.  *clean: no row can be late, and [*tmin, *tmax] is the
+// span of its event times (0 when the fold keeps no watermark).
+static bw_status prepass(bw_fold* f, const Deferred& d, BatchView* bv, bool* clean, i64* tmin, i64* tmax) {
+  bw_ctx* ctx = f->ctx;
+  u64 max_total = d.rows;
   cudaStream_t pre_stream = f->s_pre;
   if (ctx->world > 1) {
-    bw_status st = exchange(f, d_keys, d_vals, d_ts, rows, &bv);
+    bw_status st = exchange(f, d.d_keys, d.d_vals, d.d_ts, d.rows, bv);
     if (st != BW_OK) return st;
     max_total = f->max_recv_rows;
     pre_stream = f->s_x;  // the verdict is computed right behind the exchange, beside the previous fold
-  } else {
-    bv.nseg = 1;
-    bv.keys[0] = d_keys;
-    bv.vals[0] = d_vals;
-    bv.ts[0] = f->has_ts ? d_ts : nullptr;
-    bv.h_counts[0] = rows;
-    bv.max_rows = rows;
-    f->st.rows_received += rows;
   }
-  bool clean = true;
+  *clean = true;
+  *tmin = *tmax = 0;
   if (f->p.track_wm && max_total > 0) {
-    if (pre_stream != f->s_compute && ctx->world == 1 && f->pre_wait) CU(ctx, cudaStreamWaitEvent(pre_stream, f->pre_wait, 0));
+    if (ctx->world == 1 && f->cols_ready) CU(ctx, cudaStreamWaitEvent(pre_stream, f->cols_ready, 0));
     const u64 nranges = (max_total + BW_RANGE_ROWS - 1) / BW_RANGE_ROWS;
     // one warp per 2048-row range; cap at 64 warps per SM in total (the block size is small so that a block fits beside the fold)
     int grid = (int)std::min<u64>((nranges * 32 + BW_PRE_THREADS - 1) / BW_PRE_THREADS, (u64)ctx->sm_count * (2048 / BW_PRE_THREADS));
     if (grid < 1) grid = 1;
-    f->pt.mark(2, 0, pre_stream);
-    k_prepass_ranges<<<grid, BW_PRE_THREADS, 0, pre_stream>>>(bv, f->p, f->d_rmin, f->d_rmax, f->d_rbad);
-    k_prepass_scan<<<1, 1024, 0, pre_stream>>>(bv, f->p, f->d_rmin, f->d_rmax, f->d_rbad, f->d_ctr, f->d_verdict, f->d_span);
+    k_prepass_ranges<<<grid, BW_PRE_THREADS, 0, pre_stream>>>(*bv, f->p, f->d_rmin, f->d_rmax, f->d_rbad);
+    k_prepass_scan<<<1, 1024, 0, pre_stream>>>(*bv, f->p, f->d_rmin, f->d_rmax, f->d_rbad, f->d_ctr, f->d_verdict, f->d_span);
     CU(ctx, cudaGetLastError());
     f->st.kernel_launches += 2;
-    f->pt.mark(2, 1, pre_stream);
     CU(ctx, cudaMemcpyAsync(f->h_verdict, f->d_verdict, sizeof(u32), cudaMemcpyDeviceToHost, pre_stream));
     CU(ctx, cudaMemcpyAsync(f->h_verdict + 4, f->d_span, 2 * sizeof(i64), cudaMemcpyDeviceToHost, pre_stream));
     CU(ctx, cudaEventRecord(f->ev_pre, pre_stream));
     CU(ctx, cudaEventSynchronize(f->ev_pre));
-    clean = (*f->h_verdict != 0);
+    *clean = (*f->h_verdict != 0);
+    *tmin = ((const i64*)(f->h_verdict + 4))[0];
+    *tmax = ((const i64*)(f->h_verdict + 4))[1];
     if (pre_stream != f->s_compute) CU(ctx, cudaStreamWaitEvent(f->s_compute, f->ev_pre, 0));
   }
   if (ctx->world > 1) {  // the fold may start once the exchange (and the verdict pass behind it) is done
     CU(ctx, cudaEventRecord(f->ev_xchg_done, f->s_x));
     CU(ctx, cudaStreamWaitEvent(f->s_compute, f->ev_xchg_done, 0));
   }
-  if (max_total > 0) {
-    if (clean) {
-      const u64 known = (ctx->world == 1) ? rows : max_total;
-      const i64 tmin = ((const i64*)(f->h_verdict + 4))[0], tmax = ((const i64*)(f->h_verdict + 4))[1];
-      bw_status st = direct_fold(f, bv, known, batch_no, ord, f->p.track_wm ? tmin : 0, f->p.track_wm ? tmax : 0);
-      if (st != BW_OK) return st;
-    } else {
-      u64 total = rows;
-      if (ctx->world > 1) {
-        u64 hc[BW_MAX_WORLD];
-        CU(ctx, cudaMemcpyAsync(hc, bv.d_counts, sizeof(u64) * ctx->world, cudaMemcpyDeviceToHost, f->s_compute));
-        CU(ctx, cudaStreamSynchronize(f->s_compute));
-        total = 0;
-        for (int r = 0; r < ctx->world; ++r) total += hc[r];
-      }
-      bw_status st = slow_path(f, bv, total, ord, batch_no);
-      if (st != BW_OK) return st;
-      f->st.slow_batches++;
-    }
-    bw_status st = close_stage(f, ord, batch_no, nullptr);
-    if (st != BW_OK) return st;
-  }
-  if (ctx->world > 1) {
-    CU(ctx, cudaEventRecord(f->ev_fold_done, f->s_compute));
-    f->fold_recorded = true;
-  } else {
-    bw_status mst = mark_rows(f, ord);
-    if (mst != BW_OK) return mst;
-  }
-  if (stage) {
-    CU(ctx, cudaEventRecord(stage->consumed, f->s_compute));
-    stage->used = true;
-  }
   return BW_OK;
 }
-
 
 // One collective per activation: the all-gather that brings every rank's verdict of the activation just scattered is
 // also the barrier behind the previous activation's combine (a rank enters it after its peer stores, in stream order).
@@ -1529,16 +1459,17 @@ static bw_status gather_verdict(bw_fold* f, int side) {
   return BW_OK;
 }
 
-// Multi-GPU fold stage of the deferred activation.  Every rank has the same gathered verdicts, so every rank takes
-// the same branch (the collectives below line up): either combine -> partials over NVLink -> barrier -> merge, or
-// the legacy path (partition + exchange of the raw rows, direct / exact fold).
-static bw_status stream_resolve_multi(bw_fold* f, const Deferred& d) {
+// World > 1: combine -> partials over NVLink -> barrier -> merge for streamed activation d, when the gathered verdicts
+// of every rank allow it (*folded).  Every rank has the same gathered verdicts, so every rank takes the same branch and
+// the collectives line up.  *running: the maximum event time over all ranks after d.
+static bw_status combine_merge(bw_fold* f, const Deferred& d, bool* folded, i64* running) {
   bw_ctx* ctx = f->ctx;
   const StreamBufs& sb = f->sb;
   const FoldParams& p = f->p;
   cudaStream_t s = f->s_compute;
   const int W = ctx->world, R = ctx->rank;
   const StreamVerdict sv = f->h_sv[d.side];
+  *folded = false;
   f->st.scatter_spill_rows += sv.n_spill;
   // this activation's verdicts: gathered by the previous activation's exchange barrier, else (first activation, or
   // after a flush) by a collective of their own
@@ -1550,13 +1481,14 @@ static bw_status stream_resolve_multi(bw_fold* f, const Deferred& d) {
   const int next_side = d.side ^ 1;  // the activation scattered after this one (if any) waits for its gather
   const VerdictGather* vg = f->h_vg + (size_t)d.side * W;
   // chain the ranks' slices in source order: the arrival order at every destination (bw_prepass.cuh's rule)
-  i64 running = f->h_gmax, gmin = INT64_MAX, gmax = INT64_MIN;
+  i64 gmin = INT64_MAX, gmax = INT64_MIN;
+  *running = f->h_gmax;
   bool bad = false, unfit = false;
   for (int r = 0; r < W; ++r) {
     if (vg[r].flags || vg[r].n_spill) unfit = true;  // a row some scatter set aside belongs to another rank's table
     if (vg[r].tmax < vg[r].tmin) continue;            // no rows on that rank
-    if (vg[r].bad || vg[r].tmin < bw_sub_sat(running, p.wait_us)) bad = true;
-    running = std::max(running, vg[r].tmax);
+    if (vg[r].bad || vg[r].tmin < bw_sub_sat(*running, p.wait_us)) bad = true;
+    *running = std::max(*running, vg[r].tmax);
     gmin = std::min(gmin, vg[r].tmin);
     gmax = std::max(gmax, vg[r].tmax);
     // the combine folds a rank's slice in one pass: two panes
@@ -1570,37 +1502,19 @@ static bw_status stream_resolve_multi(bw_fold* f, const Deferred& d) {
     q_hi = bw_floordiv(gmax - p.align_us, p.pane_us);
     if ((u64)(gmax - gmin) >= 0x7FFFFFF0ULL || q_hi - q_lo >= 2 * 64) unfit = true;
   }
-  f->h_gmax = running;
-  k_set_gmax<<<1, 1, 0, s>>>(f->d_ctr, running);  // (the legacy path's lateness pass chains from the same maximum)
+  f->h_gmax = *running;
+  k_set_gmax<<<1, 1, 0, s>>>(f->d_ctr, *running);  // (the legacy path's lateness pass chains from the same maximum)
   f->st.kernel_launches++;
   if (!clean || unfit) {
-    if (f->vg_pending[next_side]) {
-      bw_status gst = gather_verdict(f, next_side);
-      if (gst != BW_OK) return gst;
-    }
-    bw_status st = legacy_batch(f, d.d_keys, d.d_vals, d.d_ts, d.rows, d.batch_no, d.ord, d.stage);
-    if (st != BW_OK) return st;
-    k_stream_reset<<<1, 1, 0, s>>>(f->t, sb.side[d.side].sv);
-    k_set_gmax<<<1, 1, 0, s>>>(f->d_ctr, running);
+    if (f->vg_pending[next_side]) return gather_verdict(f, next_side);
     return BW_OK;
   }
   f->st.rows_received += d.rows;  // (this rank's share of the rows arrives as partials)
-  SegArgs A;
-  memset(&A, 0, sizeof A);
-  A.in = sb.side[d.side];
-  A.nb = sb.nb;
-  A.nlanes = sb.nlanes;
-  A.lane_cap = sb.lane_cap;
-  A.nlanes_used = d.lanes;
-  A.spill_cap = sb.spill_cap;
-  A.val_bytes = sb.val_bytes;
-  A.seg_shift = f->t.seg_shift;
+  SegArgs A = seg_args(f, d);
   A.world = (u32)W;
   A.rank = (u32)R;
   A.nb_local = f->nb_local;
   A.part_cap = f->part_cap;
-  A.batch_no = d.batch_no;
-  A.epoch = d.ord;
   for (int r = 0; r < W; ++r) {
     char* base = (char*)f->precv_peer[r];
     A.pcnt_out[r] = (u32*)(base + f->precv_cnt_off[d.side]) + (size_t)R * f->nb_local;
@@ -1608,22 +1522,16 @@ static bw_status stream_resolve_multi(bw_fold* f, const Deferred& d) {
   }
   A.pcnt_in = (const u32*)((char*)f->precv_base + f->precv_cnt_off[d.side]);
   A.pin = (const Partial*)((char*)f->precv_base + f->precv_rec_off[d.side]);
-  EventPair* ep = next_timer(f, d.batch_no);
-  if (ep) {
-    ep->rows = d.rows;
-    ep->kind = 0;
-    CU(ctx, cudaEventRecord(ep->a, s));
-  }
+  EventPair* ep;
+  CU(ctx, timer_begin(f, &ep, d.batch_no, 0, d.rows, s));
   // combine this rank's slice (one pass over its own two panes) and store the partials in their owners' regions
   A.ts0 = sv.ts0;
   A.q_lo = (sv.tmax >= sv.tmin) ? bw_floordiv(sv.tmin - p.align_us, p.pane_us) : 0;
   A.npass = 1;
-  f->pt.mark(6, 0, s);
   f->combine_kernel<<<(int)std::min<u32>(sb.nb, (u32)f->combine_grid), BW_SF_THREADS, f->segfold_smem, s>>>(A, f->t, f->p, f->e);
   CU(ctx, cudaGetLastError());
   // every rank's partials are in place once every rank has entered this collective -- which also carries the verdicts
   // of the activation scattered after this one
-  f->pt.mark(1, 0, s);
   if (f->vg_pending[next_side]) {
     bw_status gst = gather_verdict(f, next_side);
     if (gst != BW_OK) return gst;
@@ -1631,7 +1539,6 @@ static bw_status stream_resolve_multi(bw_fold* f, const Deferred& d) {
     bw_status cst = coll_barrier(ctx, f->d_barrier_word, s);
     if (cst != BW_OK) return cst;
   }
-  f->pt.mark(1, 1, s);
   // merge what every source left for this rank's segments, in source order, over the activation's whole span
   A.nb = f->nb_local;
   A.ts0 = any_rows ? gmin : p.align_us;
@@ -1639,24 +1546,15 @@ static bw_status stream_resolve_multi(bw_fold* f, const Deferred& d) {
   A.npass = (u32)((q_hi - q_lo) / 2 + 1);
   f->merge_kernel<<<(int)std::min<u32>(f->nb_local, (u32)f->merge_grid), BW_SF_THREADS, f->segfold_smem, s>>>(A, f->t, f->p, f->e);
   CU(ctx, cudaGetLastError());
-  f->pt.mark(6, 1, s);
-  if (ep) CU(ctx, cudaEventRecord(ep->b, s));
-  f->pt.mark(7, 0, s);
+  CU(ctx, timer_end(ep, s));
   k_spill<<<ctx->sm_count, 256, 0, s>>>(f->t, f->p, sb.side[d.side].spill, sb.side[d.side].sv, sb.spill_cap, d.batch_no, 0u, 0xFFFFFFFFu);
   f->st.kernel_launches += 3;
   f->st.fold_launches++;
   f->st.combined_folds++;
-  bw_status st = close_stage(f, d.ord, d.batch_no, sb.side[d.side].sv);
-  f->pt.mark(7, 1, s);
-  if (d.stage) {
-    CU(ctx, cudaEventRecord(d.stage->consumed, s));
-    d.stage->used = true;
-  }
-  return st;
+  *folded = true;
+  return BW_OK;
 }
 
-// The fold stage of the deferred activation: the segment fold when its verdict allows, else what the
-// direct path would have done (its scatter output is dropped; the input columns are still there).
 // An activation the verdict could not prove clean (one GPU): find its late rows without sorting it (bw_late.cuh), then
 // scatter it again without them.  *ok: *sv is now the verdict of the rows that are left -- none of them late, so the
 // streaming fold is exact for them -- and the late rows wait in f->late for k_late_emit.  Not ok (more suspects than
@@ -1726,116 +1624,126 @@ static bw_status late_split(bw_fold* f, const Deferred& d, const BatchView& bv, 
   return BW_OK;
 }
 
-static bw_status stream_resolve(bw_fold* f) {
+// One GPU: the segment fold of streamed activation d (bv: its columns), when its verdict allows (*folded) -- after the
+// late-row split of an activation the verdict could not prove clean.  *sv: the verdict the fold stage goes by.
+static bw_status segment_fold(bw_fold* f, const Deferred& d, const BatchView& bv, StreamVerdict* sv, bool* folded) {
   bw_ctx* ctx = f->ctx;
-  Deferred d = f->dq;
-  if (!d.valid) return BW_OK;
-  f->dq.valid = false;
   const StreamBufs& sb = f->sb;
-  cudaStream_t s = f->s_compute;
-  CU(ctx, cudaEventSynchronize(f->ev_sv[d.side]));
-  if (ctx->world > 1) return stream_resolve_multi(f, d);
-  StreamVerdict sv = f->h_sv[d.side];
   const FoldParams& p = f->p;
-  BatchView bv;
-  memset(&bv, 0, sizeof bv);
-  bv.nseg = 1;
-  bv.keys[0] = d.d_keys;
-  bv.vals[0] = d.d_vals;
-  bv.ts[0] = f->has_ts ? d.d_ts : nullptr;
-  bv.h_counts[0] = d.rows;
-  bv.max_rows = d.rows;
+  cudaStream_t s = f->s_compute;
+  *sv = f->h_sv[d.side];
   bool split = false;
-  if (!sv.clean && p.track_wm && f->late_split) {
-    bw_status lst = late_split(f, d, bv, &sv, &split);
+  if (!sv->clean && p.track_wm && f->late_split) {
+    bw_status lst = late_split(f, d, bv, sv, &split);
     if (lst != BW_OK) return lst;
   }
-  f->st.scatter_spill_rows += sv.n_spill;
+  f->st.scatter_spill_rows += sv->n_spill;
   i64 q_lo = 0, q_hi = 0;
-  if (sv.tmax >= sv.tmin) {
-    q_lo = bw_floordiv(sv.tmin - p.align_us, p.pane_us);
-    q_hi = bw_floordiv(sv.tmax - p.align_us, p.pane_us);
+  if (sv->tmax >= sv->tmin) {
+    q_lo = bw_floordiv(sv->tmin - p.align_us, p.pane_us);
+    q_hi = bw_floordiv(sv->tmax - p.align_us, p.pane_us);
   }
-  const bool fits = sv.clean && !sv.flags && (q_hi - q_lo) < 2 * 64;
-  bw_status st = BW_OK;
-  if (fits) {
-    SegArgs A;
-    memset(&A, 0, sizeof A);
-    A.in = sb.side[d.side];
-    A.nb = sb.nb;
-    A.nlanes = sb.nlanes;
-    A.lane_cap = sb.lane_cap;
-    A.nlanes_used = d.lanes;
-    A.spill_cap = sb.spill_cap;
-    A.val_bytes = sb.val_bytes;
-    A.seg_shift = f->t.seg_shift;
-    A.ts0 = sv.ts0;
-    A.q_lo = q_lo;
-    A.npass = (u32)((q_hi - q_lo) / 2 + 1);
-    A.batch_no = d.batch_no;
-    A.epoch = d.ord;
-    EventPair* ep = next_timer(f, d.batch_no);
-    if (ep) {
-      ep->rows = d.rows;
-      ep->kind = 0;
-      CU(ctx, cudaEventRecord(ep->a, s));
-    }
-    if (getenv("BW_DEBUG_CURSOR")) {
-      std::vector<u32> hc((size_t)sb.nb * sb.nlanes);
-      cudaMemcpy(hc.data(), sb.side[d.side].cnt, sizeof(u32) * hc.size(), cudaMemcpyDeviceToHost);
-      u64 sum = 0;
-      u32 mx = 0;
-      for (u32 bb = 0; bb < sb.nb; ++bb)
-        for (u32 l = 0; l < d.lanes; ++l) {
-          sum += hc[(size_t)bb * sb.nlanes + l];
-          mx = std::max(mx, hc[(size_t)bb * sb.nlanes + l]);
-        }
-      fprintf(stderr, "[bwgpu] batch %u: nb %u lanes %u lane_cap %u rows %llu in lanes %llu max %u spill %u flags %u span [%lld, %lld]\n", d.batch_no,
-              sb.nb, d.lanes, sb.lane_cap, (unsigned long long)d.rows, (unsigned long long)sum, mx, sv.n_spill, sv.flags, (long long)sv.tmin,
-              (long long)sv.tmax);
-    }
-    if (split) {
-      k_late_emit<<<ctx->sm_count * 4, 256, 0, s>>>(bv, f->t, f->p, f->e, f->late, d.batch_no,
-                                                                                                            d.ord);
-      f->st.kernel_launches++;
-      f->st.split_batches++;
-    }
-    const u32 n_pre = std::min<u32>(sv.n_spill, sb.spill_cap);  // rows the scatter set aside: fold them first
-    if (n_pre) {
-      k_spill<<<(int)std::min<u32>((n_pre + 255) / 256, (u32)ctx->sm_count * 4), 256, 0, s>>>(f->t, f->p, sb.side[d.side].spill, sb.side[d.side].sv,
-                                                                                           sb.spill_cap, d.batch_no, 0u, n_pre);
-      f->st.kernel_launches++;
-    }
-    f->pt.mark(6, 0, s);
-    const int grid = (int)std::min<u32>(sb.nb, (u32)f->segfold_grid);
-    f->segfold_kernel<<<grid, BW_SF_THREADS, f->segfold_smem, s>>>(A, f->t, f->p, f->e);
-    CU(ctx, cudaGetLastError());
-    f->pt.mark(6, 1, s);
-    if (ep) CU(ctx, cudaEventRecord(ep->b, s));
-    f->pt.mark(7, 0, s);
-    k_spill<<<ctx->sm_count, 256, 0, s>>>(f->t, f->p, sb.side[d.side].spill, sb.side[d.side].sv, sb.spill_cap, d.batch_no, n_pre, 0xFFFFFFFFu);
-    f->st.kernel_launches += 2;
-    f->st.fold_launches++;
-    f->st.combined_folds++;
-    st = close_stage(f, d.ord, d.batch_no, sb.side[d.side].sv);
-    f->pt.mark(7, 1, s);
-  } else {
+  *folded = sv->clean && !sv->flags && (q_hi - q_lo) < 2 * 64;
+  if (!*folded) {
     // (the scatter output of this activation is simply not read)
-    if (split) sv = f->h_sv[d.side], sv.clean = 0u;  // (split, but too many panes for the segment fold: the sort path; nothing was emitted)
-    if (sv.clean) {
-      st = direct_fold(f, bv, d.rows, d.batch_no, d.ord, sv.tmin, sv.tmax);
+    if (split) *sv = f->h_sv[d.side], sv->clean = 0u;  // (split, but too many panes for the segment fold: the sort path; nothing was emitted)
+    return BW_OK;
+  }
+  SegArgs A = seg_args(f, d);
+  A.ts0 = sv->ts0;
+  A.q_lo = q_lo;
+  A.npass = (u32)((q_hi - q_lo) / 2 + 1);
+  EventPair* ep;
+  CU(ctx, timer_begin(f, &ep, d.batch_no, 0, d.rows, s));
+  if (split) {
+    k_late_emit<<<ctx->sm_count * 4, 256, 0, s>>>(bv, f->t, f->p, f->e, f->late, d.batch_no, d.ord);
+    f->st.kernel_launches++;
+    f->st.split_batches++;
+  }
+  const u32 n_pre = std::min<u32>(sv->n_spill, sb.spill_cap);  // rows the scatter set aside: fold them first
+  if (n_pre) {
+    k_spill<<<(int)std::min<u32>((n_pre + 255) / 256, (u32)ctx->sm_count * 4), 256, 0, s>>>(f->t, f->p, sb.side[d.side].spill, sb.side[d.side].sv,
+                                                                                           sb.spill_cap, d.batch_no, 0u, n_pre);
+    f->st.kernel_launches++;
+  }
+  const int grid = (int)std::min<u32>(sb.nb, (u32)f->segfold_grid);
+  f->segfold_kernel<<<grid, BW_SF_THREADS, f->segfold_smem, s>>>(A, f->t, f->p, f->e);
+  CU(ctx, cudaGetLastError());
+  CU(ctx, timer_end(ep, s));
+  k_spill<<<ctx->sm_count, 256, 0, s>>>(f->t, f->p, sb.side[d.side].spill, sb.side[d.side].sv, sb.spill_cap, d.batch_no, n_pre, 0xFFFFFFFFu);
+  f->st.kernel_launches += 2;
+  f->st.fold_launches++;
+  f->st.combined_folds++;
+  return BW_OK;
+}
+
+// The fold stage of activation d, whose columns are on the device: `streamed` when its scatter + verdict are queued
+// (the deferred activation).  A streamed activation takes the segment fold (one GPU) or combine + merge (world > 1) when
+// its verdict allows.  Otherwise the direct kernel folds it when it is clean, else the sort path; whether it is clean is
+// the streamed verdict on one GPU, else the lateness pass over the caller's columns or, on world > 1, over the rows
+// the exchange brought.  Every path ends in the same tail: close, mark the rows (one GPU) or record the fold's end (world
+// > 1), release the staging buffer.
+static bw_status fold_stage(bw_fold* f, const Deferred& d, bool streamed) {
+  bw_ctx* ctx = f->ctx;
+  const bool multi = ctx->world > 1;
+  cudaStream_t s = f->s_compute;
+  StreamVerdict* dsv = f->sb.side[d.side].sv;  // (streamed) the scatter's verdict on the device
+  BatchView bv = one_segment(f, d);
+  StreamVerdict sv{};
+  bool folded = false;
+  i64 running = 0;
+  bw_status st = BW_OK;
+  if (streamed) {
+    st = multi ? combine_merge(f, d, &folded, &running) : segment_fold(f, d, bv, &sv, &folded);
+    if (st != BW_OK) return st;
+  }
+  const bool prepassed = !folded && (multi || !streamed);
+  bool clean = sv.clean;
+  i64 tmin = sv.tmin, tmax = sv.tmax;
+  if (prepassed && (st = prepass(f, d, &bv, &clean, &tmin, &tmax)) != BW_OK) return st;
+  const bool any = multi || d.rows > 0;  // (on world > 1 the exchange may bring rows to a rank that has none)
+  if (!folded && any) {
+    if (clean) {
+      st = direct_fold(f, bv, multi ? f->max_recv_rows : d.rows, d.batch_no, d.ord, tmin, tmax);
     } else {
-      st = slow_path(f, bv, d.rows, d.ord, d.batch_no);
+      u64 total = d.rows;
+      if (multi) {
+        u64 hc[BW_MAX_WORLD];
+        CU(ctx, cudaMemcpyAsync(hc, bv.d_counts, sizeof(u64) * ctx->world, cudaMemcpyDeviceToHost, s));
+        CU(ctx, cudaStreamSynchronize(s));
+        total = 0;
+        for (int r = 0; r < ctx->world; ++r) total += hc[r];
+      }
+      st = slow_path(f, bv, total, d.ord, d.batch_no);
       f->st.slow_batches++;
     }
-    if (st == BW_OK) st = close_stage(f, d.ord, d.batch_no, sb.side[d.side].sv);
+    if (st != BW_OK) return st;
   }
-  if (st == BW_OK) st = mark_rows(f, d.ord);
+  // the scatter's verdict is reset with the close, unless the rows went through the lateness pass instead
+  if (any && (st = close_stage(f, d.ord, d.batch_no, streamed && !prepassed ? dsv : nullptr)) != BW_OK) return st;
+  if (streamed && prepassed) {  // (world > 1) the scatter's verdict, and the chain's maximum the lateness pass moved
+    k_stream_reset<<<1, 1, 0, s>>>(f->t, dsv);
+    k_set_gmax<<<1, 1, 0, s>>>(f->d_ctr, running);
+  }
+  if (multi) {
+    CU(ctx, cudaEventRecord(f->ev_fold_done, s));
+    f->fold_recorded = true;
+  } else if ((st = mark_rows(f, d.ord)) != BW_OK) {
+    return st;
+  }
   if (d.stage) {
     CU(ctx, cudaEventRecord(d.stage->consumed, s));
     d.stage->used = true;
   }
-  return st;
+  return BW_OK;
+}
+
+static bw_status stream_resolve(bw_fold* f) {
+  Deferred d = f->dq;
+  if (!d.valid) return BW_OK;
+  f->dq.valid = false;
+  CU(f->ctx, cudaEventSynchronize(f->ev_sv[d.side]));
+  return fold_stage(f, d, true);
 }
 
 // Everything after the columns are on the device (on s_compute's dependency chain).
@@ -1846,37 +1754,33 @@ static bw_status run_batch(bw_fold* f, const u64* d_keys, const void* d_vals, co
   if (!f->have_pending) { f->min_epoch = epoch; f->have_pending = true; }
   f->last_epoch = epoch;
   f->have_epoch = true;
-  const u64 ord = epoch;
   f->st.rows_ingested += rows;
-  if (ctx->world > 1 ? f->stream_ok : stream_usable(f, d_keys, d_vals, d_ts, rows)) {
+  if (ctx->world == 1) f->st.rows_received += rows;
+  Deferred d;
+  d.side = (int)(batch_no & 1u);
+  d.d_keys = d_keys;
+  d.d_vals = d_vals;
+  d.d_ts = d_ts;
+  d.rows = rows;
+  d.ord = epoch;
+  d.batch_no = batch_no;
+  d.stage = stage;
+  const bool streamed = ctx->world > 1 ? f->stream_ok : stream_usable(f, d_keys, d_vals, d_ts, rows);
+  bw_status st = BW_OK;
+  if (streamed) {
     // queue this activation's scatter + verdict BEFORE looking at the previous verdict: the device
     // always has the next stage waiting while the host decides
-    const int side = (int)(batch_no & 1u);
-    if (ctx->world == 1) f->st.rows_received += rows;
-    bw_status st = stream_front(f, d_keys, d_vals, d_ts, rows, batch_no, side);
-    if (st != BW_OK) return st;
-    const u32 lanes = f->last_scatter_grid;  // (resolving the previous activation may scatter it a second time)
-    st = stream_resolve(f);
-    if (st != BW_OK) return st;
-    Deferred& d = f->dq;
+    if ((st = stream_front(f, d_keys, d_vals, d_ts, rows, batch_no, d.side)) != BW_OK) return st;
+    d.lanes = f->last_scatter_grid;  // (resolving the previous activation may scatter it a second time)
+  }
+  if ((st = stream_resolve(f)) != BW_OK) return st;  // activations fold in order
+  if (streamed) {
     d.valid = true;
-    d.side = side;
-    d.d_keys = d_keys;
-    d.d_vals = d_vals;
-    d.d_ts = d_ts;
-    d.rows = rows;
-    d.ord = ord;
-    d.batch_no = batch_no;
-    d.lanes = lanes;
-    d.stage = stage;
-    return flush_rows(f);
+    f->dq = d;
+  } else if ((st = fold_stage(f, d, false)) != BW_OK) {
+    return st;
   }
-  {  // activations fold in order
-    bw_status st = stream_resolve(f);
-    if (st != BW_OK) return st;
-  }
-  bw_status st = legacy_batch(f, d_keys, d_vals, d_ts, rows, batch_no, ord, stage);
-  return st == BW_OK ? flush_rows(f) : st;
+  return flush_rows(f);
 }
 
 bw_status bw_ingest_commit(bw_fold* f, const bw_batch* batch, uint64_t rows, uint64_t epoch) {
@@ -1907,9 +1811,7 @@ bw_status bw_ingest_commit(bw_fold* f, const bw_batch* batch, uint64_t rows, uin
   }
   CU(ctx, cudaEventRecord(f->ev_h2d, f->s_copy));
   CU(ctx, cudaStreamWaitEvent(f->s_compute, f->ev_h2d, 0));
-  CU(ctx, cudaEventRecord(f->ev_in, f->s_copy));
-  f->pre_wait = f->ev_in;
-  CU(ctx, cudaEventRecord(f->ev_src_ready, f->s_copy));
+  f->cols_ready = f->ev_h2d;
   bw_status st = run_batch(f, sg.d_keys, sg.d_vals, sg.d_ts, rows, epoch, &sg);
   if (st != BW_OK) {  // (the slot goes back to the ring on the error paths too: repeated failures must not use it up)
     cudaEventSynchronize(f->ev_h2d);
@@ -1931,13 +1833,10 @@ bw_status bw_ingest_device(bw_fold* f, const uint64_t* d_keys, const void* d_val
   if (rows && (!d_keys || (!d_vals && (f->spec.reduction != BW_RED_COUNT || f->spec.ts_source == BW_TS_FROM_VALUE)) || (f->has_ts && !d_ts_us)))
     FAIL(f, BW_ERR_SPEC, "ingest: missing column");
   CU(ctx, cudaSetDevice(ctx->device));
-  // The caller's columns are complete (bwgpu.h): the verdict pass takes no ordering from the fold's stream, so
-  // it runs beside the previous activation's fold instead of behind it.  Columns written by this library's own
-  // generator are ordered through its event.
-  f->pre_wait = f->ev_gen;
-  // multi-GPU: the caller's columns must already be complete (see bwgpu.h); no ordering with the fold's
-  // stream is taken, so that this activation's exchange can overlap the previous activation's fold
-  CU(ctx, cudaEventRecord(f->ev_src_ready, f->s_x));
+  // The caller's columns are complete (bwgpu.h): the lateness pass and the exchange take no ordering from the fold's
+  // stream, so they run beside the previous activation's fold instead of behind it.  Columns written by this
+  // library's own generator are ordered through its event.
+  f->cols_ready = f->ev_gen;
   return run_batch(f, d_keys, d_vals, d_ts_us, rows, epoch, nullptr);
 }
 
@@ -2279,9 +2178,8 @@ bw_status bw_snapshot_load(bw_fold* f, const bw_snapshot* in) {
   cudaStream_t s = f->s_compute;
   const u64 n = in->n;
   if (n) {
-    void* dev = nullptr;
-    CU(ctx, cudaMalloc(&dev, n * 7 * 8));
-    SnapCols dc = snap_cols(dev, n);
+    CU(ctx, f->own.regrow(Owner::DEV, &f->snap_dev, n * 7 * 8));
+    SnapCols dc = snap_cols(f->snap_dev, n);
     const void* src[7] = {in->key, in->pane_id, in->acc, in->count, in->open_seq, in->max_ts_us, in->closed_upto};
     void* dst[7] = {dc.key, dc.pane, dc.acc, dc.cnt, dc.seq, dc.max_ts, dc.closed_upto};
     for (int c = 0; c < 7; ++c) CU(ctx, cudaMemcpyAsync(dst[c], src[c], n * 8, cudaMemcpyHostToDevice, s));
@@ -2292,7 +2190,6 @@ bw_status bw_snapshot_load(bw_fold* f, const bw_snapshot* in) {
     k_reset_dirty<<<1, 1, 0, s>>>(f->t);
     f->st.kernel_launches += 3;
     CU(ctx, cudaStreamSynchronize(s));
-    cudaFree(dev);
   }
   k_snap_set_gmax<<<1, 1, 0, s>>>(f->d_ctr, (i64)in->gmax_ts_us);
   CU(ctx, cudaMemcpyAsync(f->h_ctr, f->d_ctr, sizeof(Counters), cudaMemcpyDeviceToHost, s));
@@ -2363,18 +2260,19 @@ bw_status bw_fold_reset_timers(bw_fold* f) {
   f->st.split_batches = 0;
   return BW_OK;
 }
+// Fold the deferred activation, then wait for the copy, lateness and exchange streams, and for the fold's own stream
+// too when `compute`.
+static bw_status resolve_and_sync(bw_fold* f, bool compute) {
+  bw_status st = stream_resolve(f);
+  if (st != BW_OK) return st;
+  for (cudaStream_t s : {f->s_copy, f->s_pre, f->s_x}) CU(f->ctx, cudaStreamSynchronize(s));
+  if (compute) CU(f->ctx, cudaStreamSynchronize(f->s_compute));
+  return BW_OK;
+}
 bw_status bw_fold_sync(bw_fold* f) {
   if (!f) return BW_ERR_SPEC;
   CU(f->ctx, cudaSetDevice(f->ctx->device));
-  {
-    bw_status st = stream_resolve(f);
-    if (st != BW_OK) return st;
-  }
-  CU(f->ctx, cudaStreamSynchronize(f->s_copy));
-  CU(f->ctx, cudaStreamSynchronize(f->s_pre));
-  CU(f->ctx, cudaStreamSynchronize(f->s_x));
-  CU(f->ctx, cudaStreamSynchronize(f->s_compute));
-  return BW_OK;
+  return resolve_and_sync(f, true);
 }
 bw_status bw_fold_time_begin(bw_fold* f) {
   if (!f) return BW_ERR_SPEC;
@@ -2385,27 +2283,16 @@ bw_status bw_fold_time_begin(bw_fold* f) {
     CU(ctx, f->own.event(&f->ev_t1, cudaEventDefault));
   }
   // everything submitted so far (copies, prepass) must be done before the clock starts
-  {
-    bw_status st = stream_resolve(f);
-    if (st != BW_OK) return st;
-  }
-  CU(ctx, cudaStreamSynchronize(f->s_copy));
-  CU(ctx, cudaStreamSynchronize(f->s_pre));
-  CU(ctx, cudaStreamSynchronize(f->s_x));
-  CU(ctx, cudaStreamSynchronize(f->s_compute));
+  bw_status st = resolve_and_sync(f, true);
+  if (st != BW_OK) return st;
   CU(ctx, cudaEventRecord(f->ev_t0, f->s_compute));
   return BW_OK;
 }
 bw_status bw_fold_time_end(bw_fold* f, float* ms) {
   if (!f || !ms || !f->ev_t0) return BW_ERR_SPEC;
   bw_ctx* ctx = f->ctx;
-  {
-    bw_status st = stream_resolve(f);
-    if (st != BW_OK) return st;
-  }
-  CU(ctx, cudaStreamSynchronize(f->s_copy));
-  CU(ctx, cudaStreamSynchronize(f->s_pre));
-  CU(ctx, cudaStreamSynchronize(f->s_x));
+  bw_status st = resolve_and_sync(f, false);  // (the fold's stream ends in the record below)
+  if (st != BW_OK) return st;
   CU(ctx, cudaEventRecord(f->ev_t1, f->s_compute));
   CU(ctx, cudaEventSynchronize(f->ev_t1));
   CU(ctx, cudaEventElapsedTime(ms, f->ev_t0, f->ev_t1));

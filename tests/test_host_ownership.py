@@ -12,9 +12,8 @@ SRC = os.path.join(ROOT, "bytewax_b200", "csrc", "bwgpu.cu")
 
 RAW = re.compile(r"\b(cudaMalloc\w*|cudaHostAlloc|cudaFree\w*|cudaEventCreate\w*|cudaEventDestroy|cudaStreamCreate\w*"
                  r"|cudaStreamDestroy)\s*\(")
-# memory the caller owns (bw_dev_*, bw_host_*), the context's L2-flush buffer, and the snapshot load's staging copy
-ALLOWED = ["bw_dev_alloc", "bw_dev_free", "bw_host_alloc", "bw_host_free", "bw_ctx_destroy", "bw_flush_l2",
-           "bw_snapshot_load"]
+# memory the caller owns (bw_dev_*, bw_host_*) and the context's L2-flush buffer
+ALLOWED = ["bw_dev_alloc", "bw_dev_free", "bw_host_alloc", "bw_host_free", "bw_ctx_destroy", "bw_flush_l2"]
 
 
 def _source():
