@@ -155,6 +155,23 @@ class BwSjwinRows(C.Structure):
                 ("n_released", C.c_uint64), ("released", C.POINTER(C.c_uint64))]
 
 
+class BwScwinSpec(C.Structure):
+    _fields_ = [("struct_size", C.c_uint32), ("ordered", C.c_int32), ("max_sessions_per_key", C.c_int32), ("pad", C.c_int32),
+                ("gap_us", C.c_int64), ("wait_us", C.c_int64), ("capacity_hint", C.c_uint64), ("max_queued_rows", C.c_uint64),
+                ("max_batch_rows", C.c_uint64), ("max_emit_rows", C.c_uint64), ("max_late_rows", C.c_uint64)]
+
+
+class BwScwinRows(C.Structure):
+    _fields_ = [("n_down", C.c_uint64), ("down_key", C.POINTER(C.c_uint64)), ("down_window_id", C.POINTER(C.c_int64)),
+                ("down_epoch", C.POINTER(C.c_uint64)), ("down_offset", C.POINTER(C.c_uint64)), ("handle", C.POINTER(C.c_uint64)),
+                ("open_us", C.POINTER(C.c_int64)), ("close_us", C.POINTER(C.c_int64)),
+                ("merged_off", C.POINTER(C.c_uint64)), ("merged_ids", C.POINTER(C.c_int64)),
+                ("merge_off", C.POINTER(C.c_uint64)), ("merge_start", C.POINTER(C.c_uint64)), ("merge_end", C.POINTER(C.c_uint64)),
+                ("n_late", C.c_uint64), ("late_key", C.POINTER(C.c_uint64)), ("late_epoch", C.POINTER(C.c_uint64)),
+                ("late_activation", C.POINTER(C.c_uint64)), ("late_row", C.POINTER(C.c_uint64)),
+                ("n_released", C.c_uint64), ("released", C.POINTER(C.c_uint64))]
+
+
 class BwArgwinSpec(C.Structure):
     _fields_ = [("struct_size", C.c_uint32), ("extreme", C.c_int32), ("by_dtype", C.c_int32), ("session", C.c_int32),
                 ("max_windows_per_key", C.c_int32), ("pad", C.c_int32), ("length_us", C.c_int64), ("offset_us", C.c_int64),
@@ -237,6 +254,12 @@ SYMBOLS = {
     "bw_sjwin_apply_device": (C.c_int32, [_P, _P, _P, _P, _P, C.c_uint64, C.c_uint64, C.c_int64]),
     "bw_sjwin_advance": (C.c_int32, [_P, C.c_int64, C.POINTER(BwSjwinRows)]),
     "bw_sjwin_eof": (C.c_int32, [_P, C.POINTER(BwSjwinRows)]),
+    "bw_scwin_create": (C.c_int32, [_P, C.POINTER(BwScwinSpec), C.POINTER(_P)]),
+    "bw_scwin_destroy": (None, [_P]),
+    "bw_scwin_apply": (C.c_int32, [_P, _P, _P, _P, C.c_uint64, C.c_uint64, C.c_int64]),
+    "bw_scwin_apply_device": (C.c_int32, [_P, _P, _P, _P, C.c_uint64, C.c_uint64, C.c_int64]),
+    "bw_scwin_advance": (C.c_int32, [_P, C.c_int64, C.POINTER(BwScwinRows)]),
+    "bw_scwin_eof": (C.c_int32, [_P, C.POINTER(BwScwinRows)]),
     "bw_argwin_create": (C.c_int32, [_P, C.POINTER(BwArgwinSpec), C.POINTER(_P)]),
     "bw_argwin_destroy": (None, [_P]),
     "bw_argwin_apply": (C.c_int32, [_P, _P, _P, _P, _P, C.c_uint64, C.c_uint64, C.c_int64]),

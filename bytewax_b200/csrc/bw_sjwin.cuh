@@ -59,13 +59,14 @@ struct SjEmit : JwEmit {  // K8's down, late, release and carry-over buffers (la
 };
 
 // notify_at (windowing.py:1153-1180 with an identity `to_system_utc`; the windower's :790-796): the earliest close +
-// gap, or, ordered, the ts of queue[0] if that is sooner
+// gap, or, ordered, the ts of queue[0] if that is sooner (R: SjRec here, ScRec in bw_scwin.cuh)
 struct SjNotifyAt {
   i64 gap;
-  __device__ __forceinline__ i64 operator()(const JwParams& p, const JwState& st, const SjRec* R) const {
+  template <class R>
+  __device__ __forceinline__ i64 operator()(const JwParams& p, const JwState& st, const R* Rs) const {
     i64 at = INT64_MAX;
     for (u32 i = 0; i < st.n; ++i) {
-      const i64 c = R[i].close + gap;  // close <= UTC_MAX and gap <= UTC_MAX - UTC_MIN: no overflow
+      const i64 c = Rs[i].close + gap;  // close <= UTC_MAX and gap <= UTC_MAX - UTC_MIN: no overflow
       at = c < at ? c : at;
     }
     if (p.ordered && st.nq && st.q0ts < at) at = st.q0ts;

@@ -38,6 +38,7 @@
 #include "bw_jwin.cuh"
 #include "bw_collect.cuh"
 #include "bw_sjwin.cuh"
+#include "bw_scwin.cuh"
 #include "bw_argwin.cuh"
 #include "bw_prepass.cuh"
 #include "bw_slow.cuh"
@@ -3027,13 +3028,14 @@ static bw_status jwin_drain(J* j) {
   if (j->h_err[0]) {
     j->failed = true;
     const u32 w = j->h_err[1];
-    CTX_FAIL(ctx, (bw_status)j->h_err[0], "%s kernel %s:%s%s%s%s%s%s%s", jwin_what(j),
+    CTX_FAIL(ctx, (bw_status)j->h_err[0], "%s kernel %s:%s%s%s%s%s%s%s%s", jwin_what(j),
              j->h_err[0] == BW_ERR_SPEC ? "rejected its input" : "ran out of capacity",
              w & BW_JW_BAD_SIDE ? " a side column value is not below sides;" : "", w & BW_JW_FULL_TABLE ? " key table full (raise capacity_hint);" : "",
              w & BW_JW_FULL_WINDOWS ? jwin_full_windows(j) : "",
              w & BW_JW_FULL_EMIT ? jwin_full_emit(j) : "",
              w & BW_JW_FULL_LATE ? " more than max_late_rows late rows since the last advance;" : "",
-             w & BW_JW_FULL_QUEUE ? " more than max_queued_rows queued entries;" : "", w ? "" : " (no reason recorded)");
+             w & BW_JW_FULL_QUEUE ? " more than max_queued_rows queued entries;" : "",
+             w & BW_CW_FULL_STORE ? " entry store or staging buffer full;" : "", w ? "" : " (no reason recorded)");
   }
   const u64 nr = j->h_cnt[3];
   j->outstanding -= std::min(nr, j->outstanding);
@@ -3467,8 +3469,9 @@ static bw_status collect_drain(bw_collect* j) {
 }
 
 // a device buffer of `cap` elements, the first `used` of them kept, regrown to `grow` (nothing on the stream reads it)
-template <class T>
-static cudaError_t collect_grow_keep(bw_collect* j, T** p, u64 used, u64 grow) {
+// (J: bw_collect, bw_scwin)
+template <class J, class T>
+static cudaError_t collect_grow_keep(J* j, T** p, u64 used, u64 grow) {
   T* q = nullptr;
   cudaError_t e = j->own.dev(&q, grow);
   if (!e && used) e = cudaMemcpyAsync(q, *p, used * sizeof(T), cudaMemcpyDeviceToDevice, j->s);
@@ -3484,8 +3487,9 @@ static cudaError_t collect_grow_keep(bw_collect* j, T** p, u64 used, u64 grow) {
 
 // Before a call that can play `values` values (its rows, and ordered the queued entries): compact the store once dead
 // entries outnumber live ones, then grow the store, the staging buffer and the release buffer so that nothing the call
-// can add or close overflows them.  Called after collect_drain: nothing on the stream reads them.
-static bw_status collect_room(bw_collect* j, u64 rows) {
+// can add or close overflows them.  Called after the drain: nothing on the stream reads them.  (J: bw_collect, bw_scwin)
+template <class J>
+static bw_status collect_room(J* j, u64 rows) {
   bw_ctx* ctx = j->ctx;
   CwStore& es = j->es;
   CwEmit& e = j->e;
@@ -3596,6 +3600,35 @@ bw_status bw_collect_apply(bw_collect* j, const uint64_t* keys, const uint64_t* 
   return collect_drain(j);
 }
 
+// advance / eof, after jwin_ship put the nd closed records in the reference's order (x.perm): their lists as CSR --
+// offsets (nd + 1 of them, to h_off) by a scan of their counts, then every one of the ns staged handles to its place in
+// parallel, to h_out (J: bw_collect, bw_scwin)
+template <class J>
+static bw_status collect_place(J* j, u64 nd, u64 ns, u64* h_off) {
+  bw_ctx* ctx = j->ctx;
+  if (ns > j->out_cap) {
+    j->out_cap = 0;
+    CU(ctx, j->own.regrow(Owner::DEV, &j->d_out, ns));
+    CU(ctx, j->own.regrow(Owner::HOST, &j->h_out, ns));
+    j->out_cap = ns;
+  }
+  if (!nd) {
+    h_off[0] = 0;
+    return BW_OK;
+  }
+  const int grid = ctx->sm_count * 4;
+  SortScratch& x = j->srt;
+  const auto& e = j->e;
+  k_cwin_order<<<grid, 256, 0, j->s>>>(x.perm, e.cnt, j->d_inv, j->d_cs, nd);
+  CU(ctx, cudaMemsetAsync(j->d_cs + nd, 0, 8, j->s));
+  size_t tb = x.cub_bytes;
+  CU(ctx, cub::DeviceScan::ExclusiveSum(x.cub, tb, j->d_cs, j->d_off, (int)(nd + 1), j->s));
+  k_cwin_place<<<ctx->sm_count * 8, 256, 0, j->s>>>(e.stage, e.stage_rec, e.soff, j->d_inv, j->d_off, j->d_out, ns);
+  CU(ctx, cudaMemcpyAsync(h_off, j->d_off, (nd + 1) * 8, cudaMemcpyDeviceToHost, j->s));
+  if (ns) CU(ctx, cudaMemcpyAsync(j->h_out, j->d_out, ns * 8, cudaMemcpyDeviceToHost, j->s));
+  return BW_OK;
+}
+
 static bw_status collect_collect(bw_collect* j, bw_collect_rows* out) {
   bw_ctx* ctx = j->ctx;
   bw_status st = collect_drain(j);
@@ -3604,28 +3637,10 @@ static bw_status collect_collect(bw_collect* j, bw_collect_rows* out) {
   CU(ctx, cudaStreamSynchronize(j->s));
   const u64 nd = j->h_cnt[0], nl = j->h_cnt[1], ns = j->h_cnt[4];  // all within bounds: collect_drain passed
   const CwEmit& e = j->e;
-  if (ns > j->out_cap) {
-    j->out_cap = 0;
-    CU(ctx, j->own.regrow(Owner::DEV, &j->d_out, ns));
-    CU(ctx, j->own.regrow(Owner::HOST, &j->h_out, ns));
-    j->out_cap = ns;
-  }
   const u64* down[] = {e.key, e.wid, e.epoch};
   const u64* late[] = {e.l_key, e.l_wid, e.l_epoch, e.l_act, e.l_row};
   if ((st = jwin_ship(j, nd, e.key, e.seq, e.ord, down, 3, &j->hd)) != BW_OK) return st;
-  if (nd) {  // the lists in the closed windows' order: offsets by a scan of their counts, then every handle in parallel
-    const int grid = ctx->sm_count * 4;
-    SortScratch& x = j->srt;
-    k_cwin_order<<<grid, 256, 0, j->s>>>(x.perm, e.cnt, j->d_inv, j->d_cs, nd);
-    CU(ctx, cudaMemsetAsync(j->d_cs + nd, 0, 8, j->s));
-    size_t tb = x.cub_bytes;
-    CU(ctx, cub::DeviceScan::ExclusiveSum(x.cub, tb, j->d_cs, j->d_off, (int)(nd + 1), j->s));
-    k_cwin_place<<<ctx->sm_count * 8, 256, 0, j->s>>>(e.stage, e.stage_rec, e.soff, j->d_inv, j->d_off, j->d_out, ns);
-    CU(ctx, cudaMemcpyAsync(j->hd.col[3], j->d_off, (nd + 1) * 8, cudaMemcpyDeviceToHost, j->s));
-    if (ns) CU(ctx, cudaMemcpyAsync(j->h_out, j->d_out, ns * 8, cudaMemcpyDeviceToHost, j->s));
-  } else {
-    j->hd.col[3][0] = 0;
-  }
+  if ((st = collect_place(j, nd, ns, j->hd.col[3])) != BW_OK) return st;
   if ((st = jwin_ship(j, nl, e.l_key, e.l_seq, e.l_ord, late, 5, &j->hl)) != BW_OK) return st;
   CU(ctx, cudaGetLastError());
   CU(ctx, cudaMemsetAsync(j->d_cnt, 0, 16, j->s));
@@ -3979,6 +3994,385 @@ bw_status bw_sjwin_eof(bw_sjwin* j, bw_sjwin_rows* out) {
   bw_status st = sjwin_wake(j, 1);
   if (st != BW_OK) return st;
   return sjwin_collect(j, out);
+}
+
+// ===========================================================================
+// K12 host side: collect_window over session windows (bw_scwin.cuh)
+// ===========================================================================
+// K9's store, staging, output and growth (collect_room, collect_place) and K8's drain and release-buffer growth
+// (jwin_drain, jwin_room) read these members by the names bw_collect / bw_jwin give them.
+struct bw_scwin {
+  Owner own;  // every buffer and the stream below
+  bw_ctx* ctx = nullptr;
+  bw_scwin_spec spec{};
+  ScTable t{};
+  CwStore es{};
+  KeyedScratch k;
+  cudaStream_t s = nullptr;
+  u32* h_err = nullptr;  // err, why
+  // closed sessions, merged ids, late rows, released, carried-over queue entries, staged, store, intervals, merges
+  unsigned long long* d_cnt = nullptr;
+  unsigned long long* h_cnt = nullptr;
+  unsigned char *d_late = nullptr, *d_flag = nullptr;
+  u64* d_handles = nullptr;
+  i64* d_ts = nullptr;
+  ScEmit e{};
+  JwPool pool{}, pool2{};  // ordered mode: the queue, and the one the next flush writes
+  u64 nq = 0;              // entries in `pool`
+  int slot_bits = 1;
+  u64 kmax = 1;            // entries one value adds: it joins one session
+  u64 n_store = 0, dead = 0;    // entries in the store, and how many of them are dead
+  u64 n_rows = 0, n_stage = 0;  // closed sessions and staged handles since the last advance / eof
+  u64 n_mrg = 0;                // merges applied so far
+  SortScratch srt;              // pool sort, ordering and compaction scratch
+  u32* d_inv = nullptr;         // advance / eof: a closed session's place in the reference's order
+  u64 *d_cs = nullptr, *d_off = nullptr;  // its count in that order, and the exclusive scan of them
+  u64* d_out = nullptr;         // the handles in the reference's order
+  u64* h_out = nullptr;
+  u64 out_cap = 0;
+  HostCols hd[2];  // down: key, id, epoch, open, close | merged count, merged offset, interval count, interval offset, CSR
+  HostCols hl;     // late: key, window id, epoch, activation, row
+  i64* h_mids = nullptr;
+  u64* h_ivs = nullptr;
+  std::vector<u64> merged_off, merge_off, merge_start, merge_end;
+  std::vector<i64> merged_ids;
+  std::vector<u64> released;      // since the last advance / eof
+  std::vector<u64> released_out;  // what the last advance / eof handed out
+  bool undrained = false;     // a call whose counts are not read back yet
+  u64 outstanding = 0;        // handles passed in and not released yet: what the next call can release, besides its own
+  u32 batch_no = 0;
+  u64 calls = 0, first_call = 0;  // calls (activations, notify phases, EOF) so far; the first not yet collected
+  u64 last_epoch = 0;
+  i64 now = INT64_MIN;
+  bool failed = false;
+};
+
+bw_status bw_scwin_create(bw_ctx* ctx, const bw_scwin_spec* spec, bw_scwin** out) {
+  if (!ctx || !spec || !out) CTX_FAIL(ctx, BW_ERR_SPEC, "bw_scwin_create: NULL argument");
+  if (spec->struct_size != sizeof(bw_scwin_spec)) CTX_FAIL(ctx, BW_ERR_SPEC, "bw_scwin_spec.struct_size mismatch");
+  if (ctx->world != 1) CTX_FAIL(ctx, BW_ERR_SPEC, "session collects run on one GPU (world == 1)");
+  if (spec->ordered != 0 && spec->ordered != 1) CTX_FAIL(ctx, BW_ERR_SPEC, "ordered must be 0 or 1");
+  if (spec->max_sessions_per_key < 1 || spec->max_sessions_per_key > BW_SESS_MAXM)
+    CTX_FAIL(ctx, BW_ERR_SPEC, "max_sessions_per_key must be in 1..%d", BW_SESS_MAXM);
+  if (spec->gap_us < 0 || spec->gap_us > BW_UTC_MAX_US - BW_UTC_MIN_US) CTX_FAIL(ctx, BW_ERR_SPEC, "gap_us must be in 0..UTC_MAX - UTC_MIN");
+  if (spec->wait_us < 0) CTX_FAIL(ctx, BW_ERR_SPEC, "wait_us must not be negative");
+  if (spec->max_batch_rows == 0 || spec->max_batch_rows >= (1ULL << 31)) CTX_FAIL(ctx, BW_ERR_SPEC, "bad max_batch_rows");
+  if (spec->max_queued_rows >= (1ULL << 31) - spec->max_batch_rows) CTX_FAIL(ctx, BW_ERR_SPEC, "max_queued_rows + max_batch_rows must stay below 2^31");
+  if (spec->max_emit_rows >= (1ULL << 31)) CTX_FAIL(ctx, BW_ERR_SPEC, "max_emit_rows must be below 2^31");
+  if (spec->capacity_hint >= (1ULL << 30)) CTX_FAIL(ctx, BW_ERR_SPEC, "capacity_hint must be below 2^30");
+  CU(ctx, cudaSetDevice(ctx->device));
+  std::unique_ptr<bw_scwin, void (*)(bw_scwin*)> cp(new bw_scwin(), bw_scwin_destroy);  // torn down on every failure
+  bw_scwin* j = cp.get();
+  Owner& own = j->own;
+  j->ctx = ctx;
+  j->spec = *spec;
+  const u64 cap = std::max<u64>(1024, 2 * std::max<u64>(spec->capacity_hint, 1));
+  const int M = spec->max_sessions_per_key;
+  const u64 cells = (cap + 1) * (u64)M;
+  ScTable& t = j->t;
+  t.j.cap = cap;
+  t.j.M = M;
+  t.j.sides = 1;
+  t.gap = spec->gap_us;
+  while ((1ULL << j->slot_bits) < cap + 1) ++j->slot_bits;
+  CU(ctx, own.stream(&j->s));
+  CU(ctx, own.dev(&t.j.keys, cap + 1));
+  CU(ctx, own.dev(&t.j.st, cap + 1));
+  CU(ctx, own.dev(&t.kx, cap + 1));
+  CU(ctx, own.dev(&t.rec, cells));
+  CU(ctx, own.dev(&t.mrg, 2 * cells));
+  CU(ctx, own.dev(&t.iv, cells));
+  CU(ctx, own.dev(&t.cell_ord, cells));
+  CU(ctx, own.dev(&t.cell_c, cells));
+  CU(ctx, own.dev(&t.cell_mord, cells));
+  CU(ctx, own.dev(&t.cell_root, cells));
+  CU(ctx, own.dev(&t.cell_base, cells));
+  t.j.win = nullptr;  // (K8's window records: sessions live in rec)
+  t.win = nullptr;
+  CU(ctx, own.dev(&t.j.err, 2));
+  t.j.why = t.j.err + 1;
+  t.err = t.j.err;
+  t.why = t.j.why;
+  CU(ctx, own.dev(&j->d_cnt, 9));
+  CU(ctx, cudaMemsetAsync(t.err, 0, 8, j->s));
+  CU(ctx, cudaMemsetAsync(j->d_cnt, 0, 72, j->s));
+  CU(ctx, own.host(&j->h_err, 64 / sizeof(u32)));
+  CU(ctx, own.host(&j->h_cnt, 128 / sizeof(unsigned long long)));
+  const u64 n = spec->max_batch_rows, m = std::max<u64>(spec->max_emit_rows, 1), l = std::max<u64>(spec->max_late_rows, 1);
+  const u64 q = spec->ordered ? spec->max_queued_rows : 0;
+  bw_status st = keyed_alloc(ctx, own, j->k, n, j->s);
+  if (st != BW_OK) return st;
+  CU(ctx, own.dev(&j->d_late, n));
+  CU(ctx, own.dev(&j->d_handles, n));
+  CU(ctx, own.dev(&j->d_ts, n));
+  if (spec->ordered) {
+    if ((st = jwin_pool_alloc(ctx, own, j->pool, q + n)) != BW_OK) return st;
+    if ((st = jwin_pool_alloc(ctx, own, j->pool2, q + n)) != BW_OK) return st;
+  }
+  ScEmit& e = j->e;
+  for (u64** c : {&e.key, &e.wid, &e.cnt, &e.soff, &e.epoch, &e.ord, &e.seq, &e.moff, &e.mcnt, &e.ioff, &e.icnt, &e.ivs}) CU(ctx, own.dev(c, m));
+  for (i64** c : {&e.open, &e.close, &e.mids}) CU(ctx, own.dev(c, m));
+  for (u64** c : {&e.l_key, &e.l_wid, &e.l_epoch, &e.l_act, &e.l_row, &e.l_ord, &e.l_seq}) CU(ctx, own.dev(c, l));
+  CU(ctx, own.dev(&j->d_inv, m));
+  CU(ctx, own.dev(&j->d_cs, m + 1));
+  CU(ctx, own.dev(&j->d_off, m + 1));
+  // the store, the staging buffer, the output and the release buffer grow with what the collect holds (collect_room);
+  // they start at one batch
+  CwStore& es = j->es;
+  es.cap = n;
+  CU(ctx, own.dev(&es.ref, n));
+  CU(ctx, own.dev(&es.rank, n));
+  CU(ctx, own.dev(&es.h, n));
+  CU(ctx, own.dev(&j->d_flag, n));
+  e.max_stage = n;
+  CU(ctx, own.dev(&e.stage, n));
+  CU(ctx, own.dev(&e.stage_rec, n));
+  j->out_cap = n;
+  CU(ctx, own.dev(&j->d_out, n));
+  CU(ctx, own.host(&j->h_out, n));
+  e.max_rel = n;
+  CU(ctx, own.dev(&e.rel, e.max_rel));
+  e.max_rows = spec->max_emit_rows;
+  e.max_late = spec->max_late_rows;
+  e.max_queue = q;
+  e.n_rows = j->d_cnt;
+  e.n_mids = j->d_cnt + 1;
+  e.n_late = j->d_cnt + 2;
+  e.n_rel = j->d_cnt + 3;   // (jwin_drain reads these two)
+  e.n_next = j->d_cnt + 4;
+  e.n_stage = j->d_cnt + 5;
+  es.n = j->d_cnt + 6;
+  e.n_ivs = j->d_cnt + 7;
+  e.n_mrg = j->d_cnt + 8;
+  const u64 ns = std::max(std::max(m, l), q + n);
+  CU(ctx, j->srt.reserve(own, ns, ns, j->s));
+  size_t b = 0;
+  CU(ctx, cub::DeviceScan::ExclusiveSum(nullptr, b, j->d_cs, j->d_off, (int)(m + 1), j->s));
+  CU(ctx, j->srt.grow_cub(own, b + 256));
+  CU(ctx, j->hd[0].reserve(own, m, m));
+  CU(ctx, j->hd[1].reserve(own, m + 1, m + 1));
+  CU(ctx, j->hl.reserve(own, l, l));
+  CU(ctx, own.host(&j->h_mids, m));
+  CU(ctx, own.host(&j->h_ivs, m));
+  k_scwin_init<<<ctx->sm_count * 4, 256, 0, j->s>>>(t);
+  CU(ctx, cudaGetLastError());
+  CU(ctx, cudaStreamSynchronize(j->s));
+  *out = cp.release();
+  return BW_OK;
+}
+
+void bw_scwin_destroy(bw_scwin* j) {
+  if (!j) return;
+  cudaSetDevice(j->ctx->device);
+  if (j->s) cudaStreamSynchronize(j->s);
+  delete j;  // j->own releases every buffer and the stream
+}
+
+static JwParams scwin_params(bw_scwin* j, u64 epoch) {
+  JwParams p{};
+  p.ordered = j->spec.ordered;
+  p.wait = j->spec.wait_us;
+  p.now = j->now;
+  p.epoch = epoch;
+  p.ord = j->calls++;
+  p.batch_no = j->batch_no;
+  return p;
+}
+
+static const char* jwin_what(const bw_scwin*) { return "session collect"; }
+static const char* jwin_full_windows(const bw_scwin*) {
+  return " a key needs more than max_sessions_per_key sessions, merged ids or merge intervals;";
+}
+static const char* jwin_full_emit(const bw_scwin*) {
+  return " more than max_emit_rows closed sessions, merged ids or merge intervals since the last advance;";
+}
+static u64 jwin_counters(const bw_scwin*) { return 9; }
+
+#define SCWIN_REFUSE_FAILED(j) \
+  if ((j)->failed) CTX_FAIL((j)->ctx, BW_ERR_STATE, "session collect: an earlier call failed on the device; the collect is unusable")
+
+// K8's drain (fail on a device-side overflow, take the released handles and the queue count), then the store's counts
+static bw_status scwin_drain(bw_scwin* j) {
+  const bool fresh = j->undrained;
+  bw_status st = jwin_drain(j);
+  if (st != BW_OK || !fresh) return st;
+  j->n_rows = j->h_cnt[0];
+  j->dead += j->h_cnt[5] - j->n_stage;  // every staged handle left a dead entry behind
+  j->n_stage = j->h_cnt[5];
+  j->n_store = j->h_cnt[6];
+  j->n_mrg = j->h_cnt[8];
+  return BW_OK;
+}
+
+// after the per-key kernels of a call: retag the merged-away sessions' entries, move the closed sessions' out
+static bw_status scwin_gather(bw_scwin* j, const JwParams& p) {
+  k_scwin_gather<<<j->ctx->sm_count * 8, 256, 0, j->s>>>(j->t, j->e, j->es, p, j->n_rows, j->n_mrg);
+  CU(j->ctx, cudaGetLastError());
+  return BW_OK;
+}
+
+// K8's pool sort (ordered), then every woken key's flush (k_scwin_flush), then the gather
+static bw_status scwin_flush(bw_scwin* j, const JwParams& p, u64 n) {
+  bw_ctx* ctx = j->ctx;
+  bw_status st = j->spec.ordered ? jwin_sort_pool(j, j->t.j, p, n) : BW_OK;
+  if (st != BW_OK) return st;
+  ScEmit e = j->e;
+  e.next = j->pool2;
+  k_scwin_flush<<<ctx->sm_count * 8, 256, 0, j->s>>>(j->t, e, j->es, p, j->pool, j->srt.perm);
+  CU(ctx, cudaGetLastError());
+  if (j->spec.ordered) std::swap(j->pool, j->pool2);  // the next call reads what this flush carried over (count: the drain)
+  return scwin_gather(j, p);
+}
+
+bw_status bw_scwin_apply_device(bw_scwin* j, const uint64_t* d_keys, const uint64_t* d_handles, const int64_t* d_ts_us, uint64_t rows,
+                                uint64_t epoch, int64_t system_now_us) {
+  if (!j) return BW_ERR_SPEC;
+  bw_ctx* ctx = j->ctx;
+  SCWIN_REFUSE_FAILED(j);
+  if (rows > j->spec.max_batch_rows) CTX_FAIL(ctx, BW_ERR_SPEC, "session collect: rows > max_batch_rows");
+  if (rows && (!d_keys || !d_handles || !d_ts_us)) CTX_FAIL(ctx, BW_ERR_SPEC, "session collect: NULL column");
+  if (j->batch_no && epoch < j->last_epoch) CTX_FAIL(ctx, BW_ERR_STATE, "session collect: epochs must not decrease");
+  CU(ctx, cudaSetDevice(ctx->device));
+  bw_status st = scwin_drain(j);
+  if (st != BW_OK) return st;
+  j->last_epoch = epoch;
+  if (system_now_us > j->now) j->now = system_now_us;  // `now_getter()` never goes backwards (windowing.py:250-261)
+  const JwParams p = scwin_params(j, epoch);
+  j->batch_no++;
+  if (rows == 0) return BW_OK;
+  if ((st = collect_room(j, rows)) != BW_OK) return st;
+  j->outstanding += rows;
+  st = keyed_group(ctx, j->k, d_keys, rows, j->s);
+  if (st != BW_OK) return st;
+  k_scwin_apply<<<ctx->sm_count * 8, 256, 0, j->s>>>(j->t, j->e, j->es, p, j->pool, j->nq, j->k.d_ksorted, j->k.d_isorted, j->k.d_head,
+                                                     d_handles, d_ts_us, j->d_late, rows);
+  CU(ctx, cudaGetLastError());
+  j->undrained = true;
+  if (j->spec.ordered) return scwin_flush(j, p, j->nq + rows);
+  return scwin_gather(j, p);
+}
+
+bw_status bw_scwin_apply(bw_scwin* j, const uint64_t* keys, const uint64_t* handles, const int64_t* ts_us, uint64_t rows, uint64_t epoch,
+                         int64_t system_now_us) {
+  if (!j) return BW_ERR_SPEC;
+  bw_ctx* ctx = j->ctx;
+  if (rows > j->spec.max_batch_rows) CTX_FAIL(ctx, BW_ERR_SPEC, "session collect: rows > max_batch_rows");
+  if (rows && (!keys || !handles || !ts_us)) CTX_FAIL(ctx, BW_ERR_SPEC, "session collect: NULL column");
+  CU(ctx, cudaSetDevice(ctx->device));
+  bw_status st = scwin_drain(j);
+  if (st != BW_OK) return st;
+  if (rows) {
+    CU(ctx, cudaMemcpyAsync(j->k.d_keys, keys, rows * 8, cudaMemcpyHostToDevice, j->s));
+    CU(ctx, cudaMemcpyAsync(j->d_handles, handles, rows * 8, cudaMemcpyHostToDevice, j->s));
+    CU(ctx, cudaMemcpyAsync(j->d_ts, ts_us, rows * 8, cudaMemcpyHostToDevice, j->s));
+  }
+  st = bw_scwin_apply_device(j, j->k.d_keys, j->d_handles, j->d_ts, rows, epoch, system_now_us);
+  if (st != BW_OK) return st;
+  // the host columns may be reused by the caller once this returns
+  return scwin_drain(j);
+}
+
+static bw_status scwin_collect(bw_scwin* j, bw_scwin_rows* out) {
+  bw_ctx* ctx = j->ctx;
+  bw_status st = scwin_drain(j);
+  if (st != BW_OK) return st;
+  CU(ctx, cudaMemcpyAsync(j->h_cnt, j->d_cnt, 72, cudaMemcpyDeviceToHost, j->s));
+  CU(ctx, cudaStreamSynchronize(j->s));
+  // all within bounds: the drain passed
+  const u64 nd = j->h_cnt[0], nmid = j->h_cnt[1], nl = j->h_cnt[2], ns = j->h_cnt[5], niv = j->h_cnt[7];
+  const ScEmit& e = j->e;
+  const u64* down[] = {e.key, e.wid, e.epoch, (const u64*)e.open, (const u64*)e.close, e.mcnt, e.moff, e.icnt, e.ioff};
+  const u64* late[] = {e.l_key, e.l_wid, e.l_epoch, e.l_act, e.l_row};
+  if ((st = jwin_ship(j, nd, e.key, e.seq, e.ord, down, 9, j->hd)) != BW_OK) return st;
+  if ((st = collect_place(j, nd, ns, j->hd[1].col[4])) != BW_OK) return st;
+  if ((st = jwin_ship(j, nl, e.l_key, e.l_seq, e.l_ord, late, 5, &j->hl)) != BW_OK) return st;
+  if (nmid) CU(ctx, cudaMemcpyAsync(j->h_mids, e.mids, nmid * 8, cudaMemcpyDeviceToHost, j->s));
+  if (niv) CU(ctx, cudaMemcpyAsync(j->h_ivs, e.ivs, niv * 8, cudaMemcpyDeviceToHost, j->s));
+  CU(ctx, cudaGetLastError());
+  CU(ctx, cudaMemsetAsync(j->d_cnt, 0, 24, j->s));
+  CU(ctx, cudaMemsetAsync(j->d_cnt + 5, 0, 8, j->s));
+  CU(ctx, cudaMemsetAsync(j->d_cnt + 7, 0, 8, j->s));
+  CU(ctx, cudaStreamSynchronize(j->s));
+  // merged ids and intervals in down row order
+  j->merged_off.assign(nd + 1, 0);
+  j->merged_ids.resize(nmid);
+  j->merge_off.assign(nd + 1, 0);
+  j->merge_start.resize(niv);
+  j->merge_end.resize(niv);
+  const u64 *mcnt = j->hd[1].col[0], *moff = j->hd[1].col[1], *icnt = j->hd[1].col[2], *ioff = j->hd[1].col[3];
+  for (u64 r = 0; r < nd; ++r) {
+    j->merged_off[r + 1] = j->merged_off[r] + mcnt[r];
+    std::copy(j->h_mids + moff[r], j->h_mids + moff[r] + mcnt[r], j->merged_ids.begin() + j->merged_off[r]);
+    j->merge_off[r + 1] = j->merge_off[r] + icnt[r];
+    for (u64 k = 0; k < icnt[r]; ++k) {
+      const u64 v = j->h_ivs[ioff[r] + k];
+      j->merge_start[j->merge_off[r] + k] = v >> 32;
+      j->merge_end[j->merge_off[r] + k] = v & 0xffffffffULL;
+    }
+  }
+  j->n_rows = j->n_stage = 0;
+  j->first_call = j->calls;
+  out->n_down = nd;
+  out->down_key = j->hd[0].col[0];
+  out->down_window_id = (const int64_t*)j->hd[0].col[1];
+  out->down_epoch = j->hd[0].col[2];
+  out->down_offset = j->hd[1].col[4];
+  out->handle = j->h_out;
+  out->open_us = (const int64_t*)j->hd[0].col[3];
+  out->close_us = (const int64_t*)j->hd[0].col[4];
+  out->merged_off = j->merged_off.data();
+  out->merged_ids = j->merged_ids.data();
+  out->merge_off = j->merge_off.data();
+  out->merge_start = j->merge_start.data();
+  out->merge_end = j->merge_end.data();
+  out->n_late = nl;
+  out->late_key = j->hl.col[0];
+  out->late_epoch = j->hl.col[2];
+  out->late_activation = j->hl.col[3];
+  out->late_row = j->hl.col[4];
+  // handed out until the next advance / eof, then cleared
+  j->released.swap(j->released_out);
+  j->released.clear();
+  out->n_released = j->released_out.size();
+  out->released = j->released_out.data();
+  return BW_OK;
+}
+
+// notify phase or EOF: wake the keys (K8's k_jwin_mark with the session notify_at), then flush them (ordered: through
+// the pool)
+static bw_status scwin_wake(bw_scwin* j, int eof) {
+  bw_ctx* ctx = j->ctx;
+  bw_status st = scwin_drain(j);
+  if (st != BW_OK) return st;
+  if ((st = collect_room(j, 0)) != BW_OK) return st;
+  const JwParams p = scwin_params(j, j->last_epoch);
+  k_jwin_mark<<<ctx->sm_count * 8, 256, 0, j->s>>>(j->t.j, (const ScRec*)j->t.rec, p, eof, SjNotifyAt{j->t.gap});
+  CU(ctx, cudaGetLastError());
+  j->undrained = true;
+  return scwin_flush(j, p, j->nq);
+}
+
+bw_status bw_scwin_advance(bw_scwin* j, int64_t system_now_us, bw_scwin_rows* out) {
+  if (!j || !out) return BW_ERR_SPEC;
+  bw_ctx* ctx = j->ctx;
+  SCWIN_REFUSE_FAILED(j);
+  CU(ctx, cudaSetDevice(ctx->device));
+  if (system_now_us > 0) {
+    if (system_now_us > j->now) j->now = system_now_us;
+    bw_status st = scwin_wake(j, 0);
+    if (st != BW_OK) return st;
+  }
+  return scwin_collect(j, out);
+}
+
+bw_status bw_scwin_eof(bw_scwin* j, bw_scwin_rows* out) {
+  if (!j || !out) return BW_ERR_SPEC;
+  bw_ctx* ctx = j->ctx;
+  SCWIN_REFUSE_FAILED(j);
+  CU(ctx, cudaSetDevice(ctx->device));
+  bw_status st = scwin_wake(j, 1);
+  if (st != BW_OK) return st;
+  return scwin_collect(j, out);
 }
 
 // ===========================================================================

@@ -512,8 +512,6 @@ class _GpuCollectWindowStep(_GpuJoinWindowStep):
     built here from its handles in play order, with the reference's own folder calls (`append`, `add`, ``d[k] = v``)."""
 
     def on_epoch(self, epoch: int, items: list) -> list:
-        from bytewax_b200 import gpu
-
         np, plan = self.np, self.plan
         getter = getattr(plan.clock, "ts_getter", None)
         now = self._now_us()
@@ -528,11 +526,7 @@ class _GpuCollectWindowStep(_GpuJoinWindowStep):
             ts.append(_us(getter(value)))
             vals.append(value)
         if self.jwin is None:
-            self.jwin = gpu.CollectWindow(
-                _get_gpu_ctx(), plan.ordered, self.length_us, self.offset_us, self.align_us, self.wait_us,
-                capacity_hint=int(os.environ.get("BYTEWAX_B200_KEYS", 1 << 20)), max_windows_per_key=64,
-                max_queued_rows=1 << 22 if plan.ordered else 0, max_batch_rows=int(os.environ.get("BYTEWAX_B200_BATCH", 1 << 22)),
-                max_emit_rows=1 << 22, max_late_rows=1 << 22)
+            self.jwin = self._make()
         for value in vals:
             h = self.next_handle
             self.next_handle += 1
@@ -542,6 +536,16 @@ class _GpuCollectWindowStep(_GpuJoinWindowStep):
         self.jwin.apply(np.array(keys, dtype=np.uint64), np.array(handles, dtype=np.uint64), np.array(ts, dtype=np.int64),
                         self.last_epoch, now or 0)
         return self._jwin_rows(self.jwin.advance(), vals)
+
+    def _make(self):
+        from bytewax_b200 import gpu
+
+        plan = self.plan
+        return gpu.CollectWindow(
+            _get_gpu_ctx(), plan.ordered, self.length_us, self.offset_us, self.align_us, self.wait_us,
+            capacity_hint=int(os.environ.get("BYTEWAX_B200_KEYS", 1 << 20)), max_windows_per_key=64,
+            max_queued_rows=1 << 22 if plan.ordered else 0, max_batch_rows=int(os.environ.get("BYTEWAX_B200_BATCH", 1 << 22)),
+            max_emit_rows=1 << 22, max_late_rows=1 << 22)
 
     def _check_value(self, value):
         # what the folder would reject when it plays the value (windowing.py:1365-1376; `set.add` of an unhashable
@@ -593,6 +597,79 @@ class _GpuCollectWindowStep(_GpuJoinWindowStep):
         for ks, w, _c in downs:
             o, c = self.jwin.window_bounds(w)
             rows.append((ks, (w, "M", WindowMetadata(_dt(o), _dt(c)))))
+        for h in out.released.tolist():  # after this call's rows are built: no later row can name these
+            del self.values[h]
+        return rows
+
+
+class _GpuSessionCollectWindowStep(_GpuCollectWindowStep):
+    """One worker's ``collect_window`` over a ``SessionWindower`` (``GpuSessionCollectWindowPlan``) on ``bw_scwin_*``
+    (K12): `_WindowLogic` over `_SessionWindowerLogic` with the collect folder and merger per session (windowing.py:
+    671-810, 1046-1190, 1356-1384, 1692-1714), one call per activation.  Ingest and the value check are the collect
+    step's; ``M`` rows carry each session's bounds and merged ids, and late rows have window id -1, as in the session
+    join step.  Each container repeats the reference's calls: the folder per value in flattened play order and, at each
+    merge interval, the merged-away session's container built the same way and joined with the reference's merger."""
+
+    _MERGERS = {list: list.__add__, set: set.union}
+
+    def _windower_spec(self, w):
+        self.gap_us = _td_us(w.gap)
+
+    def _make(self):
+        from bytewax_b200 import gpu
+
+        plan = self.plan
+        return gpu.SessionCollectWindow(
+            _get_gpu_ctx(), plan.ordered, self.gap_us, self.wait_us, capacity_hint=int(os.environ.get("BYTEWAX_B200_KEYS", 1 << 20)),
+            max_sessions_per_key=int(os.environ.get("BYTEWAX_B200_SESSIONS", 64)), max_queued_rows=1 << 22 if plan.ordered else 0,
+            max_batch_rows=int(os.environ.get("BYTEWAX_B200_BATCH", 1 << 22)), max_emit_rows=1 << 22, max_late_rows=1 << 22)
+
+    def _session_container(self, handles, merges):
+        V, into = self.values, self.plan.into
+        if not merges:
+            return self._container(handles)
+        merger = self._MERGERS.get(into)
+
+        def build(lo, hi, k):  # the block [lo, hi) of the list; merges[k:] are the intervals from lo on, in pre-order
+            state = into()
+            i = lo
+            while i < hi:
+                if k < len(merges) and merges[k][0] == i:  # a merged-away session's block: its container, then the merger
+                    end = merges[k][1]
+                    child, k = build(i, end, k + 1)
+                    if merger is None:  # dict: `_collect_dict_merger` (windowing.py:1351-1353)
+                        state.update(child)
+                    else:
+                        state = merger(state, child)
+                    i = end
+                    continue
+                v = V[handles[i]]
+                if into is list:
+                    state.append(v)
+                elif into is set:
+                    state.add(v)
+                else:
+                    k_, v_ = v
+                    state[k_] = v_
+                i += 1
+            return state, k
+
+        return build(0, len(handles), 0)[0]
+
+    def _jwin_rows(self, out, vals) -> list:
+        from bytewax_b200.operators.windowing import WindowMetadata
+
+        lates = [(self._key_str(k), vals[r]) for k, r in zip(out.late_key.tolist(), out.late_row.tolist())]
+        o, c = out.open_us.tolist(), out.close_us.tolist()
+        downs = [(self._key_str(k), w, self._session_container(hs, out.merges(i)), WindowMetadata(_dt(o[i]), _dt(c[i]), set(out.merged(i))))
+                 for i, (k, w, hs) in enumerate(zip(out.down_key.tolist(), out.down_window_id.tolist(), out.lists()))]
+        if self.resort:  # interned (non-numeric) keys: restore ascending key-string order; stable
+            for rows in (lates, downs):
+                rows.sort(key=lambda r: r[0])
+        rows = [(ks, (-1, "L", v)) for ks, v in lates]
+        for ks, w, cont, meta in downs:
+            rows.append((ks, (w, "E", cont)))
+            rows.append((ks, (w, "M", meta)))
         for h in out.released.tolist():  # after this call's rows are built: no later row can name these
             del self.values[h]
         return rows
@@ -692,7 +769,8 @@ def _td_us(td: timedelta) -> int:
 
 def _gpu_step_for(step_id: str, plan):
     from bytewax_b200.operators import GpuFinalPlan, GpuJoinPlan, GpuSmapPlan
-    from bytewax_b200.operators.windowing import GpuArgWindowPlan, GpuCollectWindowPlan, GpuJoinWindowPlan, SessionWindower
+    from bytewax_b200.operators.windowing import (GpuArgWindowPlan, GpuCollectWindowPlan, GpuJoinWindowPlan,
+                                                  GpuSessionCollectWindowPlan, SessionWindower)
 
     if isinstance(plan, GpuJoinWindowPlan):
         if isinstance(plan.windower, SessionWindower):
@@ -700,6 +778,8 @@ def _gpu_step_for(step_id: str, plan):
         return _GpuJoinWindowStep(step_id, plan)
     if isinstance(plan, GpuCollectWindowPlan):
         return _GpuCollectWindowStep(step_id, plan)
+    if isinstance(plan, GpuSessionCollectWindowPlan):
+        return _GpuSessionCollectWindowStep(step_id, plan)
     if isinstance(plan, GpuArgWindowPlan):  # (before the SessionWindower check below, which would catch it)
         return _GpuArgWindowStep(step_id, plan)
     if isinstance(getattr(plan, "windower", None), SessionWindower):
@@ -1077,7 +1157,9 @@ class _Run:
 
     def _run_stateful(self, st, eof: bool):
         S = self.state.get(st.step_id)
-        plan = getattr(st.builder, "_gpu_plan", None) if self.gpu else None
+        plan = None
+        if self.gpu:  # (a session collect_window carries its plan on an attribute of its own)
+            plan = getattr(st.builder, "_gpu_plan", None) or getattr(st.builder, "_gpu_session_collect_plan", None)
         if S is None:
             S = self.state[st.step_id] = {
                 "logics": [dict() for _ in range(self.W)], "sched": [dict() for _ in range(self.W)],

@@ -794,6 +794,103 @@ class CollectWindow:
 
 
 @dataclass
+class SessionCollectWindowRows(CollectWindowRows):
+    """Rows of one ``SessionCollectWindow.advance`` / ``eof``.  Each down row is a closed session: its handles in
+    flattened play order (``lists()``), its merge intervals (``merges(i)``) and its ``M`` row's bounds and merged ids
+    (``merged(i)``).  Late rows all have window id -1 (``LATE_SESSION_ID``)."""
+
+    open_us: np.ndarray = None
+    close_us: np.ndarray = None
+    merged_off: np.ndarray = None  # [n_down + 1] into merged_ids
+    merged_ids: np.ndarray = None
+    merge_off: np.ndarray = None  # [n_down + 1] into merge_start / merge_end
+    merge_start: np.ndarray = None
+    merge_end: np.ndarray = None
+
+    def merged(self, i: int) -> List[int]:
+        """The ids merged directly into down row ``i``'s session, ascending."""
+        return self.merged_ids[self.merged_off[i] : self.merged_off[i + 1]].tolist()
+
+    def merges(self, i: int) -> List[Tuple[int, int]]:
+        """Down row ``i``'s merge intervals ``(start, end)`` into its list: each block one merged-away session's values,
+        transitive merges included, by start ascending then end descending (the merge tree in pre-order)."""
+        a, b = int(self.merge_off[i]), int(self.merge_off[i + 1])
+        return list(zip(self.merge_start[a:b].tolist(), self.merge_end[a:b].tolist()))
+
+
+class SessionCollectWindow:
+    """``collect_window`` over session windows (``bw_scwin``, K12; windowing.py:671-810, 1046-1190, 1436-1576).  Values
+    travel as uint64 handles; the caller keeps the objects, builds each session's container from its handles and merge
+    intervals, and may drop each object once its handle comes back in ``released``."""
+
+    def __init__(self, ctx: Context, ordered: bool = True, gap_us: int = 10_000_000, wait_us: Optional[int] = 0,
+                 capacity_hint: int = 1 << 16, max_sessions_per_key: int = 16, max_queued_rows: int = 1 << 20,
+                 max_batch_rows: int = 1 << 20, max_emit_rows: int = 1 << 20, max_late_rows: int = 1 << 20):
+        """``wait_us=None``: the watermark never advances on data (``BW_WAIT_FOREVER``)."""
+        self.ctx, self.lib = ctx, ctx.lib
+        s = N.BwScwinSpec()
+        s.struct_size = C.sizeof(N.BwScwinSpec)
+        s.ordered, s.max_sessions_per_key = int(ordered), max_sessions_per_key
+        s.gap_us, s.wait_us = gap_us, N.BW_WAIT_FOREVER if wait_us is None else wait_us
+        s.capacity_hint, s.max_queued_rows, s.max_batch_rows = capacity_hint, max_queued_rows, max_batch_rows
+        s.max_emit_rows, s.max_late_rows = max_emit_rows, max_late_rows
+        self.spec = s
+        h = C.c_void_p()
+        N.check(self.lib.bw_scwin_create(ctx.h, C.byref(s), C.byref(h)), ctx.h)
+        self.h = h
+        self._epoch = 0
+
+    def _next_epoch(self, epoch: Optional[int]) -> int:
+        if epoch is None:
+            self._epoch += 1
+            epoch = self._epoch
+        return epoch
+
+    def apply(self, keys, handles, ts_us, epoch: Optional[int] = None, system_now_us: int = 0):
+        """One activation from host arrays.  ``system_now_us``: ``now_getter()`` of the activation."""
+        keys = np.ascontiguousarray(keys, dtype=np.uint64)
+        handles = np.ascontiguousarray(handles, dtype=np.uint64)
+        ts = np.ascontiguousarray(ts_us, dtype=np.int64)
+        vp = lambda a: a.ctypes.data_as(C.c_void_p)  # noqa: E731
+        N.check(self.lib.bw_scwin_apply(self.h, vp(keys), vp(handles), vp(ts), keys.shape[0], self._next_epoch(epoch), int(system_now_us)),
+                self.ctx.h)
+
+    def apply_device(self, d_keys: int, d_handles: int, d_ts: int, rows: int, epoch: Optional[int] = None, system_now_us: int = 0):
+        N.check(self.lib.bw_scwin_apply_device(self.h, C.c_void_p(d_keys), C.c_void_p(d_handles), C.c_void_p(d_ts), rows,
+                                               self._next_epoch(epoch), int(system_now_us)), self.ctx.h)
+
+    def _wrap(self, r: N.BwScwinRows) -> SessionCollectWindowRows:
+        nd, nl, nr = int(r.n_down), int(r.n_late), int(r.n_released)
+
+        def arr(ptr, n, dt=np.uint64):
+            return np.ctypeslib.as_array(ptr, shape=(n,)).view(dt).copy() if n else np.zeros(0, dt)
+
+        off, moff, ioff = arr(r.down_offset, nd + 1), arr(r.merged_off, nd + 1), arr(r.merge_off, nd + 1)
+        return SessionCollectWindowRows(arr(r.down_key, nd), arr(r.down_window_id, nd, np.int64), arr(r.down_epoch, nd), off,
+                                        arr(r.handle, int(off[-1])), arr(r.late_key, nl), np.full(nl, -1, np.int64),
+                                        arr(r.late_epoch, nl), arr(r.late_activation, nl), arr(r.late_row, nl), arr(r.released, nr),
+                                        arr(r.open_us, nd, np.int64), arr(r.close_us, nd, np.int64), moff,
+                                        arr(r.merged_ids, int(moff[-1]), np.int64), ioff, arr(r.merge_start, int(ioff[-1])),
+                                        arr(r.merge_end, int(ioff[-1])))
+
+    def advance(self, system_now_us: int = 0) -> SessionCollectWindowRows:
+        """Rows since the last call; ``system_now_us`` > 0 first runs the notify phase at that system time."""
+        r = N.BwScwinRows()
+        N.check(self.lib.bw_scwin_advance(self.h, int(system_now_us), C.byref(r)), self.ctx.h)
+        return self._wrap(r)
+
+    def eof(self) -> SessionCollectWindowRows:
+        r = N.BwScwinRows()
+        N.check(self.lib.bw_scwin_eof(self.h, C.byref(r)), self.ctx.h)
+        return self._wrap(r)
+
+    def close(self):
+        if self.h:
+            self.lib.bw_scwin_destroy(self.h)
+            self.h = None
+
+
+@dataclass
 class ArgWindowRows:
     """Rows of one ``ArgWindow.advance`` / ``eof``, each stream in the reference's downstream order, and the handles
     released since the previous one.  Each closed row is a window's ``E`` row (the pick's handle) followed by its ``M``

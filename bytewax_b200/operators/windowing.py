@@ -560,7 +560,7 @@ class GpuFoldPlan:
 
 @operator
 def window(step_id: str, up: KeyedStream, clock: Clock, windower: Windower, builder: Callable[[Optional[Any]], WindowLogic],
-           ordered: bool = True, _gpu_plan: Optional[GpuFoldPlan] = None) -> WindowOut:
+           ordered: bool = True, _gpu_plan: Optional[GpuFoldPlan] = None, _gpu_session_collect_plan=None) -> WindowOut:
     """Generic windowing operator (windowing.py:1254)."""
 
     def shim_builder(resume_state):
@@ -573,6 +573,7 @@ def window(step_id: str, up: KeyedStream, clock: Clock, windower: Windower, buil
         )
 
     shim_builder._gpu_plan = _gpu_plan  # read by bytewax_b200.engine
+    shim_builder._gpu_session_collect_plan = _gpu_session_collect_plan  # (engine: read after `_gpu_plan`)
     events = op.stateful_batch("stateful_batch", up, shim_builder)
     downs = op.filter_map_value("unwrap_down", events, partial(_unwrap, "E"))
     lates = op.filter_map_value("unwrap_late", events, partial(_unwrap, "L"))
@@ -606,14 +607,14 @@ class _FoldWindowLogic(WindowLogic):
 @operator
 def fold_window(step_id: str, up: KeyedStream, clock: Clock, windower: Windower, builder: Callable[[], Any],
                 folder: Callable[[Any, Any], Any], merger: Callable[[Any, Any], Any], ordered: bool = True,
-                _gpu_plan: Optional[GpuFoldPlan] = None) -> WindowOut:
+                _gpu_plan: Optional[GpuFoldPlan] = None, _gpu_session_collect_plan=None) -> WindowOut:
     """Build an accumulator per window (windowing.py:1717)."""
 
     def shim_builder(resume_state):
         state = resume_state if resume_state is not None else builder()
         return _FoldWindowLogic(folder, merger, state)
 
-    return window("window", up, clock, windower, shim_builder, ordered, _gpu_plan)
+    return window("window", up, clock, windower, shim_builder, ordered, _gpu_plan, _gpu_session_collect_plan)
 
 
 def _plan_for(reduction: str, clock, windower, ordered, value_of=_identity) -> Optional[GpuFoldPlan]:
@@ -757,7 +758,8 @@ def collect_window(step_id: str, up: KeyedStream, clock: Clock, windower: Window
     else:
         raise TypeError(f"`collect_window` doesn't support `{into:!}`; only `set`, `list`, and `dict`; use `fold_window` directly")
     return fold_window("fold_window", up, clock, windower, into, folder, merger, ordered,
-                       _gpu_plan=_collect_window_plan(step_id, clock, windower, into, ordered))
+                       _gpu_plan=_collect_window_plan(step_id, clock, windower, into, ordered),
+                       _gpu_session_collect_plan=_session_collect_window_plan(step_id, clock, windower, into, ordered))
 
 
 @dataclass(frozen=True)
@@ -784,6 +786,30 @@ def _collect_window_plan(step_id, clock, windower, into, ordered) -> Optional[Gp
     if not (isinstance(clock, SystemClock) or (isinstance(clock, EventClock) and clock.to_system_utc is _identity)):
         return None
     return GpuCollectWindowPlan(into, bool(ordered), clock, windower, step_id)
+
+
+@dataclass(frozen=True)
+class GpuSessionCollectWindowPlan:
+    """A ``collect_window`` over a `SessionWindower` the engine may run with ``bw_scwin_*`` (K12): ``into`` exactly
+    `list`, `set` or `dict`, and an `EventClock` with an identity ``to_system_utc`` or a `SystemClock`.  Values travel as
+    handles into a host-side dict; each session's container is built from its handles in flattened play order, with the
+    merger applied where each merged-away session's block sits.  It rides on the builder's own attribute,
+    ``_gpu_session_collect_plan``, beside ``_gpu_plan`` (which session collects never carry)."""
+
+    into: type
+    ordered: bool
+    clock: Any
+    windower: Any
+    step_id: str = ""  # the `collect_window` step id, for the reference's `dict` error message
+
+
+def _session_collect_window_plan(step_id, clock, windower, into, ordered) -> Optional[GpuSessionCollectWindowPlan]:
+    # the conditions of `_collect_window_plan`, over a session windower
+    if into not in (list, set, dict) or not isinstance(windower, SessionWindower):
+        return None
+    if not (isinstance(clock, SystemClock) or (isinstance(clock, EventClock) and clock.to_system_utc is _identity)):
+        return None
+    return GpuSessionCollectWindowPlan(into, bool(ordered), clock, windower, step_id)
 
 
 @dataclass

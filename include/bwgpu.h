@@ -669,6 +669,96 @@ bw_status bw_sjwin_advance(bw_sjwin* j, int64_t system_now_us, bw_sjwin_rows* ou
 /* End of input: every key flushes at watermark UTC_MAX (:1144-1151), so sessions with close >= UTC_MAX - gap stay open. */
 bw_status bw_sjwin_eof(bw_sjwin* j, bw_sjwin_rows* out);
 
+/* Collect within session windows (K12): `collect_window` (pysrc/bytewax/operators/windowing.py:1436-1576) into list /
+ * set / dict over `SessionWindower` (:928-950), i.e. `_WindowLogic` (:1046-1190) over `_SessionWindowerLogic` (:671-810)
+ * with `_FoldWindowLogic` (:1692-1714) per session and the collect callbacks (:1356-1384).  Values travel as u64 handles
+ * (any u64: none is reserved); the objects stay with the caller.  Per key, per call, in order: the EventClock's late
+ * test per item (:263-287; a late item gives one row, window LATE_SESSION_ID = -1, :671, :764-766, and is not queued);
+ * `_flush_queue` (:1095-1108) at the watermark after the key's last item (unordered: every queued entry in arrival order;
+ * ordered: the entries with ts <= watermark, stably sorted by ts, the rest kept queued across calls); per due value
+ * `open_for` (:731-762: the FIRST live session by id that contains ts or lies within gap of it, extended, then
+ * `_session_find_merges` :688-715; else a new session, id max_key + 1) and the folder on the session it returned, even
+ * one a merge just took away (:1064-1077); then the merge queue in discovery order (:1079-1085), each merge calling
+ * `into.state = merger(into.state, gone.state)` (:1700-1703); then `close_for` (:774-788): sessions with close <
+ * watermark - gap (UTC_MIN if that is below it) in id order, each giving its container and then its metadata row.
+ * Session state is never discarded (:798-806).  One GPU only.
+ *
+ * A session's container is rebuilt by the caller from two things per down row: its handles in FLATTENED play order (the
+ * session's own values, with each merged-away session's flattened list spliced in as one block where the merge
+ * happened), and its merge intervals: every block [start, end) of that list that came from one merged-away session,
+ * transitive merges included, ordered by (start ascending, end descending) -- the merge tree in pre-order.  Walking the
+ * handles with the folder (`append` / `add` / `d[k] = v`) and, at each interval, building the block's container
+ * recursively and applying the merger (`list.__add__`, `set.union`, `_collect_dict_merger`) repeats the reference's
+ * calls exactly.  For lists and dicts the flat walk gives the same result; for sets it does not (`a | b` iterates
+ * differently from adding b's values to a one by one). */
+typedef struct bw_scwin bw_scwin;
+typedef struct bw_scwin_spec {
+  uint32_t struct_size;
+  int32_t ordered;              /* 1: play values in timestamp order once the watermark passes them (the default) */
+  int32_t max_sessions_per_key; /* 1..64: sessions a key holds during a call (live ones, plus those merged away in it);
+                                   also the merged ids, and separately the merge intervals, its live sessions hold */
+  int32_t pad;
+  int64_t gap_us;               /* SessionWindower.gap, >= 0 (windowing.py:938-943) */
+  int64_t wait_us;              /* EventClock.wait_for_system_duration, or BW_WAIT_FOREVER */
+  uint64_t capacity_hint;       /* keys ever seen: session state is never freed (windowing.py:798-806) */
+  uint64_t max_queued_rows;     /* ordered mode: queued entries over ALL keys */
+  uint64_t max_batch_rows;
+  uint64_t max_emit_rows;       /* closed sessions, their merged ids, and their merge intervals, each retained between
+                                   bw_scwin_advance calls */
+  uint64_t max_late_rows;       /* late rows retained between bw_scwin_advance calls */
+} bw_scwin_spec;
+/* Rows handed downstream since the last advance / eof, in the reference's order: per call (activation, notify phase
+ * or EOF), ascending key string (src/operators.rs:758-767, :862-894); within a key `down` rows of the closing sessions in
+ * id order, `late` rows in arrival order.  Each down row is one closed session: its `E` row is the container of
+ * handle[down_offset[i] .. down_offset[i + 1]) with the merge intervals [merge_off[i] .. merge_off[i + 1]) (offsets into
+ * the session's own list), and its `M` row, which follows it, is WindowMetadata(open, close, merged_ids).  Host pointers
+ * into memory owned by the library, valid until the next advance / eof / destroy. */
+typedef struct bw_scwin_rows {
+  uint64_t n_down;
+  const uint64_t* down_key;
+  const int64_t* down_window_id;
+  const uint64_t* down_epoch;
+  const uint64_t* down_offset;     /* n_down + 1 entries */
+  const uint64_t* handle;          /* down_offset[n_down] entries, flattened play order */
+  const int64_t* open_us;          /* per down row: its M row's WindowMetadata(open, close, merged_ids) */
+  const int64_t* close_us;
+  const uint64_t* merged_off;      /* [n_down + 1]: row i's merged ids are merged_ids[merged_off[i] .. merged_off[i+1]) */
+  const int64_t* merged_ids;       /* ascending per row: the sessions merged directly into it */
+  const uint64_t* merge_off;       /* [n_down + 1]: row i's intervals are merge_start / merge_end[merge_off[i] ..) */
+  const uint64_t* merge_start;     /* pre-order per row: start ascending, end descending */
+  const uint64_t* merge_end;
+  uint64_t n_late;                 /* window id LATE_SESSION_ID = -1 */
+  const uint64_t* late_key;
+  const uint64_t* late_epoch;
+  const uint64_t* late_activation; /* (activation, row) name the input row (activations counted from 0) */
+  const uint64_t* late_row;
+  /* handles no session and no queue entry holds any more: each handle passed to apply is listed exactly once, in the
+   * rows of the call that closes the session holding it, a late item's in the call that received it */
+  uint64_t n_released;
+  const uint64_t* released;
+} bw_scwin_rows;
+/* windowing.py:1436-1576 (collect_window) + :1046-1190 (_WindowLogic) + :671-810 (_SessionWindowerLogic) */
+bw_status bw_scwin_create(bw_ctx* ctx, const bw_scwin_spec* spec, bw_scwin** out);
+void bw_scwin_destroy(bw_scwin* c);
+/* One activation from HOST columns (keys, handle, ts); blocks.  `system_now_us` is `now_getter()` for this activation
+ * (windowing.py:250-261; it must not go backwards; 0 throughout = a frozen clock).  The entry store, the staging and
+ * output buffers and the release buffer grow before each call to what it can add, so no call fails for lack of room
+ * there; a full key table, more than max_sessions_per_key sessions, merged ids or merge intervals for a key, or a full
+ * queue, late buffer or closed-session buffer returns BW_ERR_CAPACITY (reason in bw_last_error) and the collect refuses
+ * further calls. */
+bw_status bw_scwin_apply(bw_scwin* c, const uint64_t* keys, const uint64_t* handles, const int64_t* ts_us, uint64_t rows,
+                         uint64_t epoch, int64_t system_now_us);
+/* Same with DEVICE columns; returns once the work is enqueued (the columns must stay valid until the next call). */
+bw_status bw_scwin_apply_device(bw_scwin* c, const uint64_t* d_keys, const uint64_t* d_handles, const int64_t* d_ts_us,
+                                uint64_t rows, uint64_t epoch, int64_t system_now_us);
+/* Rows since the last call.  `system_now_us` > 0 first runs the notify phase at that system time
+ * (src/operators.rs:808-858, windowing.py:1135-1142, 1153-1180 with an identity `to_system_utc`): every key whose
+ * earliest session close + gap -- or, ordered, the ts of its FIRST queued entry -- has been reached flushes at its
+ * watermark. */
+bw_status bw_scwin_advance(bw_scwin* c, int64_t system_now_us, bw_scwin_rows* out);
+/* End of input: every key flushes at watermark UTC_MAX (:1144-1151), so sessions with close >= UTC_MAX - gap stay open. */
+bw_status bw_scwin_eof(bw_scwin* c, bw_scwin_rows* out);
+
 /* Windowed arg-max / arg-min (K11): `max_window` / `min_window` with a `by=` projection
  * (pysrc/bytewax/operators/windowing.py:2145-2236), i.e. `reduce_window(partial(max, key=by))` = `fold_window(ordered=
  * False)` (:2268-2285) with `_FoldWindowLogic` (:1692-1714) per window, over `_SlidingWindowerLogic` (:603-668; tumbling
