@@ -136,7 +136,8 @@ class _GpuWindowStep:
         return i
 
     def _key_str(self, i: int) -> str:
-        return self.id_keys.get(i) or str(i)
+        k = self.id_keys.get(i)
+        return str(i) if k is None else k  # (the empty key "" is interned too)
 
     def on_epoch(self, epoch: int, items: list) -> list:
         np, plan = self.np, self.plan
@@ -175,16 +176,36 @@ class _GpuWindowStep:
                         raise TypeError(f"step {self.step_id!r}: the CUDA fold needs numeric values in the int64 / float64 range; got {num!r}")
                     vals.append(num)
             k, t = np.array(keys, dtype=np.uint64), np.array(ts, dtype=np.int64)
-            v = np.array(vals) if vals else np.zeros(0, dtype=np.int64)
+            v = self._value_column(vals)
         if self.fold is None:
             self.float_vals = v is not None and v.dtype.kind == "f"
             self.fold = self._mk("f64" if self.float_vals else "i64")
-        if v is not None and v.dtype.kind == "f" and not self.float_vals:
-            raise TypeError(f"step {self.step_id!r}: value type changed from integer to float mid-stream")
+        if v is not None:
+            self._check_kind(v)
         self._set_now()
         self.fold.ingest(k, v, t, max(epoch, self.last_epoch))  # (the engine's frontier already keeps epochs in order)
         self.last_epoch = max(epoch, self.last_epoch)
         return self._rows(self.fold.advance(), orig)
+
+    def _value_column(self, vals: list):
+        """The values of one batch as an int64 or float64 column.  They must all be `int` or all `float` (as K11's
+        by-values): the host compares an int with a float exactly and adds ints exactly until the first float, and one
+        float64 column does neither (`2**53 + 1` becomes `2**53`).  A mix in the step's first batch sends the step to
+        the host logic; after it, a mix raises a `TypeError` naming the step."""
+        np = self.np
+        n_float = sum(isinstance(x, float) for x in vals)
+        if 0 < n_float < len(vals):
+            if self.fold is None:  # nothing folded yet: this step runs on the host logic instead
+                raise _GpuPlanUnfit("a batch mixing int and float values")
+            raise TypeError(f"step {self.step_id!r}: the CUDA fold needs all `int` or all `float` values; got a batch mixing both")
+        return np.array(vals, dtype=np.float64 if n_float else np.int64)
+
+    def _check_kind(self, v):
+        """A batch's values are of the kind the step's first batch fixed (`float_vals`), in both directions."""
+        if (v.dtype.kind == "f") != self.float_vals:
+            was, now = ("float", "int") if self.float_vals else ("int", "float")
+            raise TypeError(f"step {self.step_id!r}: value type changed from {was} to {now} mid-stream; the CUDA fold needs "
+                            f"all `int` or all `float` values")
 
     def _now_us(self):
         from bytewax_b200.operators import windowing as W
@@ -937,12 +958,11 @@ class _GpuFinalStep(_NoClock, _GpuWindowStep):
             vals.append(value)
         if not keys:
             return []
-        v = np.array(vals)
+        v = self._value_column(vals)
         if self.fold is None:
             self.float_vals = v.dtype.kind == "f"
             self.fold = self._mk("f64" if self.float_vals else "i64")
-        if v.dtype.kind == "f" and not self.float_vals:
-            raise TypeError(f"step {self.step_id!r}: value type changed from integer to float mid-stream")
+        self._check_kind(v)
         self.fold.ingest(np.array(keys, dtype=np.uint64), v, None, max(epoch, self.last_epoch))
         self.last_epoch = max(epoch, self.last_epoch)
         return []

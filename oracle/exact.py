@@ -109,3 +109,19 @@ def fold(reduction: str, length_us: int, offset_us: Optional[int], align_us: int
             for w in window_ids(t, length_us, offset_us, align_us):
                 groups.setdefault((k, w), []).append(v)
     return {kw: _reduce(reduction, dtype, vs) for kw, vs in groups.items()}
+
+
+def final(reduction: str, batches: Iterable[Tuple[Sequence[int], Optional[Sequence]]], dtype: str = "i64") -> Dict[int, object]:
+    """``key -> exact accumulator`` of a ``*_final`` fold over ``batches`` of ``(keys, vals)`` in arrival order: what
+    ``fold`` gives for window 0 with every row at the align, grouped with a stable numpy sort instead of a loop per row
+    (the same ``_reduce`` per key, on the key's values in arrival order)."""
+    import numpy as np
+
+    batches = list(batches)
+    keys = np.concatenate([np.asarray(k, dtype=np.uint64) for k, _ in batches])
+    order = np.argsort(keys, kind="stable")
+    vals = None if any(v is None for _, v in batches) else np.concatenate([np.asarray(v) for _, v in batches])[order]
+    vals = _py_values(vals, len(keys), dtype)  # grouped by key, each key's in arrival order
+    uk, start = np.unique(keys[order], return_index=True)
+    ends = np.append(start[1:], len(keys)).tolist()
+    return {k: _reduce(reduction, dtype, vals[s:e]) for k, s, e in zip(uk.tolist(), start.tolist(), ends)}

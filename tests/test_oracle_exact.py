@@ -112,3 +112,31 @@ def test_exact_rules_at_the_limits():
         one("sum", "i64", [2**63])
     with pytest.raises(ValueError):
         one("count", "i64", [1, 1], ts=[A + 5 * S, A + 4 * S])
+
+
+@pytest.mark.parametrize("dtype", ["i64", "u64", "f32", "f64"])
+@pytest.mark.parametrize("red", ["count", "sum", "min", "max", "mean"])
+def test_final_is_fold_in_window_zero(red, dtype):
+    """`exact.final` (the *_final folds' accumulators, grouped by a numpy sort) equals `exact.fold` with every row at the
+    align: the same value and type per key, the same zero sign for min / max, in any number of batches."""
+    rnd = np.random.default_rng(7)
+    batches = []
+    for n in (500, 1, 700):
+        keys = rnd.choice(np.array([0, 1, 9, 10, 2**63, 2**64 - 1], np.uint64), n)
+        if dtype == "i64":
+            vals = rnd.choice(np.array([-(2**63), 2**63 - 1, -1, 0, 5], np.int64), n)
+        elif dtype == "u64":
+            vals = rnd.choice(np.array([0, 1, 2**63, 2**64 - 1], np.uint64), n)
+        else:
+            edge = [-0.0, 0.0, -1.5, 2.5, 5e-324] + ([math.inf, -math.inf] if red in ("min", "max") else [])
+            vals = rnd.choice(np.array(edge), n)
+            vals = vals.astype(np.float32 if dtype == "f32" else np.float64)
+        batches.append((keys, vals))
+    want = exact.fold(red, 10 * S, None, A, None, [(k, np.full(len(k), A), v) for k, v in batches], dtype)
+    got = exact.final(red, batches, dtype)
+    assert {w for _k, w in want} == {0}
+    assert list(got) == sorted(got) and set(got) == {k for k, _w in want}
+    for k, e in got.items():
+        assert e == want[(k, 0)] and type(e) is type(want[(k, 0)]), k
+        if isinstance(e, float):
+            assert math.copysign(1.0, e) == math.copysign(1.0, want[(k, 0)]), k
