@@ -19,6 +19,7 @@ LIB_PATH = os.environ.get("BWGPU_LIB") or os.path.join(HERE, "libbwgpu.so")
 CSRC = os.path.join(HERE, "csrc")
 
 BW_OK = 0
+BW_ERR_STATE = 5
 STATUS_NAMES = {
     0: "BW_OK", 1: "BW_ERR_CUDA", 2: "BW_ERR_NCCL", 3: "BW_ERR_CAPACITY", 4: "BW_ERR_SPEC",
     5: "BW_ERR_STATE", 6: "BW_ERR_RANGE", 7: "BW_ERR_NOMEM",

@@ -95,8 +95,7 @@ __device__ __forceinline__ bool bw_close_key_simple(const Table& t, const FoldPa
   } else if (!p.track_wm) {
     wm = INT64_MIN;
   } else {
-    wm = bw_sub_sat(hs->max_ts, p.wait_us);
-    if (wm < BW_UTC_MIN_US_DEV) wm = BW_UTC_MIN_US_DEV;
+    wm = bw_wm_floor(bw_sub_sat(hs->max_ts, p.wait_us), p);
   }
   const i64 q0 = bw_widtag_q(tag), q1 = bw_widtag_q1(tag);
   const u64 acc0 = hs->acc0, cnt0 = ax->cnt0, seq0 = ax->seq0;
@@ -128,7 +127,9 @@ __device__ __forceinline__ bool bw_close_key_simple(const Table& t, const FoldPa
     ax->seq0 = newest_is_1 ? seq1 : seq0;
     if (both) {
       ps->acc1 = newest_is_1 ? acc0 : acc1;
-      ps->seq1 = newest_is_1 ? seq0 : seq1;
+      // seq1 != ~0 is what marks pane 1 present.  A seq_by_id fold keeps no arrival sequence (the segment fold leaves
+      // seq0 at ~0), so the pane moved down from the hot slot takes 0, as the segment fold's own re-rank gives it.
+      ps->seq1 = ordered_seq ? 0ULL : (newest_is_1 ? seq0 : seq1);
       ax->cnt1 = newest_is_1 ? cnt0 : cnt1;
       keep1 = true;
     }
@@ -158,8 +159,7 @@ __device__ void bw_close_key(const Table& t, const FoldParams& p, const EmitBufs
   } else if (!p.track_wm) {
     wm = INT64_MIN;
   } else {
-    wm = bw_sub_sat(hs->max_ts, p.wait_us);
-    if (wm < BW_UTC_MIN_US_DEV) wm = BW_UTC_MIN_US_DEV;
+    wm = bw_wm_floor(bw_sub_sat(hs->max_ts, p.wait_us), p);
   }
   // gather
   PaneRec P[BW_MAX_PANES];
@@ -260,7 +260,7 @@ __device__ void bw_close_key(const Table& t, const FoldParams& p, const EmitBufs
     if (prev) {
       const PaneRec& r1 = P[idx[1]];
       ps->acc1 = r1.acc;
-      ps->seq1 = r1.seq;
+      ps->seq1 = ordered_seq ? 0ULL : r1.seq;  // (present; see bw_close_key_simple)
       ax->cnt1 = r1.cnt;
       first_listed = 2;
     }
@@ -334,7 +334,17 @@ __global__ void k_close_wake(Table t, FoldParams p, EmitBufs e, u64 epoch, u32 c
     for (u32 nd = t.aux[s].spill_head; nd; nd = t.nodes[nd].next) q_old = min(q_old, t.nodes[nd].wid);
     i64 w_first = bw_floordiv(q_old - b + a, a);  // earliest window over the oldest pane ...
     if (!(a == 1 && b == 1) && t.closed_upto[s] != INT64_MIN && w_first <= t.closed_upto[s]) w_first = t.closed_upto[s] + 1;  // ... not yet emitted
-    if (p.align_us + w_first * p.offset_us + p.length_us > 0) continue;  // not due
+    const i64 close = p.align_us + w_first * p.offset_us + p.length_us;
+    // An ordered fold's reference also wakes a key at the timestamp of the head of its queue, the oldest arrival not
+    // yet folded (windowing.py:1154-1180), which the table does not keep.  That only changes a row when some item's
+    // event time led the system clock (max_ts > 0 here; else the head is at or before now and every key with a queue
+    // is woken) and this notify's drifted watermark closes a window: refuse that instead of guessing.  (wait == 0:
+    // every flush empties the queue.)
+    if (p.ordered && p.wait_us > 0 && h.max_ts > 0 && close <= bw_wm_floor(bw_sub_sat(h.max_ts, p.wait_us), p)) {
+      bw_raise(t.ctr, 5u);  // BW_ERR_STATE
+      continue;
+    }
+    if (close > 0) continue;  // not due
     bw_close_key(t, p, e, s, false, epoch, close_batch);
   }
 }

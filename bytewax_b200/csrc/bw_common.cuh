@@ -442,3 +442,9 @@ __host__ __device__ __forceinline__ i64 bw_sub_sat(i64 ts, i64 wait) {
   if (ts < INT64_MIN + wait) return INT64_MIN;
   return ts - wait;
 }
+// A watermark raised to the reference's floor, UTC_MIN in absolute time (a new key's watermark_base,
+// windowing.py:245-248): UTC_MIN - now in the frame of FoldParams::now_us.
+__device__ __forceinline__ i64 bw_wm_floor(i64 wm, const FoldParams& p) {
+  const i64 lo = bw_sub_sat(BW_UTC_MIN_US_DEV, p.now_us);
+  return wm < lo ? lo : wm;
+}

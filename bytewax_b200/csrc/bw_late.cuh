@@ -2,8 +2,8 @@
 //
 // Row i of key k is late iff  ts_i < wm(max(B_k, P_i)),  B_k the key's running maximum before the activation and
 // P_i the largest timestamp among the key's EARLIER rows of the activation (windowing.py:1120-1130, clock
-// windowing.py:263-287; wm(m) = max(UTC_MIN, m - wait)).  The exact path of bw_slow.cuh gets every P_i from a
-// stable sort by key over the whole activation.  But only a SUSPECT row -- one behind the running maximum G_i over
+// windowing.py:263-287; wm(m) = max(UTC_MIN, m - wait), UTC_MIN in absolute time: bw_wm_floor).  The exact path of
+// bw_slow.cuh gets every P_i from a stable sort by key over the whole activation.  But only a SUSPECT row -- one behind the running maximum G_i over
 // all keys, ts_i < wm(G_i), which is what made the verdict "not clean" -- can be late at all (P_i, B_k <= G_i), and
 // an in-order stream with stragglers has few of them.  So:
 //
@@ -58,10 +58,8 @@ struct LateBufs {
   i64* gpre;       // per tile: running maximum over everything before the tile
 };
 
-__device__ __forceinline__ i64 bw_wm_of(i64 m, i64 wait) {
-  if (m == INT64_MIN) return BW_UTC_MIN_US_DEV;
-  const i64 wm = bw_sub_sat(m, wait);
-  return wm < BW_UTC_MIN_US_DEV ? BW_UTC_MIN_US_DEV : wm;
+__device__ __forceinline__ i64 bw_wm_of(i64 m, const FoldParams& p) {
+  return bw_wm_floor(bw_sub_sat(m, p.wait_us), p);  // (m == INT64_MIN: the floor)
 }
 
 // one block: gpre[t] = max(gprev, tile_max[0..t))
@@ -205,7 +203,7 @@ __global__ void __launch_bounds__(256) k_late_suspect(BatchView bv, FoldParams p
     for (int u = 0; u < 4; ++u) {
       const u64 task = t0 + (u64)u * nw;
       if (task >= ntask) break;
-      const i64 wm0 = bw_wm_of(pre[u], p.wait_us);
+      const i64 wm0 = bw_wm_of(pre[u], p);
       const i64 nxt = __shfl_down_sync(0xffffffffu, ta[u], 1);
       const bool fine = ta[u] <= tb[u] && (lane == 31 || tb[u] <= nxt) && ta[u] >= wm0;
       if (__all_sync(0xffffffffu, fine)) continue;  // in order, and nothing behind what came before
@@ -219,8 +217,8 @@ __global__ void __launch_bounds__(256) k_late_suspect(BatchView bv, FoldParams p
       }
       const i64 prev = __shfl_up_sync(0xffffffffu, inc, 1);
       const i64 ga = (lane > 0) ? max(pre[u], prev) : pre[u];
-      if (r < n && va < bw_wm_of(ga, p.wait_us)) sus |= 1u << (2 * u);
-      if (r + 1 < n && vb < bw_wm_of(max(ga, va), p.wait_us)) sus |= 2u << (2 * u);
+      if (r < n && va < bw_wm_of(ga, p)) sus |= 1u << (2 * u);
+      if (r + 1 < n && vb < bw_wm_of(max(ga, va), p)) sus |= 2u << (2 * u);
     }
     // the warp's suspects of these four chunks: into its queue (or, too many for it, straight to the list)
     if (__any_sync(0xffffffffu, sus != 0u)) {
@@ -343,7 +341,7 @@ __global__ void __launch_bounds__(256) k_late_classify(Table t, FoldParams p, La
     const LateEnt x = L.ent[s];
     i64 m = bw_lookup_max_ts(t, x.key);
     if (x.pmax > m) m = x.pmax;
-    if (x.ts < bw_wm_of(m, p.wait_us)) {
+    if (x.ts < bw_wm_of(m, p)) {
       L.ent[s].stamp = (L.gen << 2) | 2u;
       atomicOr(&L.late_bits[x.idx >> 5], 1u << (x.idx & 31u));
     }

@@ -81,11 +81,7 @@ __global__ void k_slow_classify(Table t, FoldParams p, const u64* keys_sorted, c
   for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (u64)gridDim.x * blockDim.x) {
     i64 m = bw_lookup_max_ts(t, keys_sorted[i]);
     if (prefmax[i] > m) m = prefmax[i];
-    i64 wm = BW_UTC_MIN_US_DEV;
-    if (m != INT64_MIN) {
-      wm = bw_sub_sat(m, p.wait_us);
-      if (wm < BW_UTC_MIN_US_DEV) wm = BW_UTC_MIN_US_DEV;
-    }
+    const i64 wm = bw_wm_floor(bw_sub_sat(m, p.wait_us), p);  // (m == INT64_MIN: the floor)
     late[idx_sorted[i]] = (ts_sorted[i] < wm) ? 1 : 0;
   }
 }

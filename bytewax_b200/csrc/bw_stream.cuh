@@ -920,8 +920,9 @@ k_segfold(SegArgs A, Table t, FoldParams p, EmitBufs e) {
           if (bw_widtag_q(tag_in) == q) {
             bool open = true;
             if (WM) {
-              i64 wm = bw_sub_sat(h.max_ts, p.wait_us);
-              if (wm < BW_UTC_MIN_US_DEV) wm = BW_UTC_MIN_US_DEV;
+              // (no UTC_MIN floor: every pane holds a row at or after UTC_MIN, so its release is above the floor and
+              // a watermark under the floor decides the same as the floor itself)
+              const i64 wm = bw_sub_sat(h.max_ts, p.wait_us);
               open = wm < p.align_us + (q + 1) * p.length_us;
             }
             if (open) {
@@ -966,8 +967,7 @@ k_segfold(SegArgs A, Table t, FoldParams p, EmitBufs e) {
           }
           i64 wm = INT64_MIN;
           if (WM) {
-            wm = bw_sub_sat(h.max_ts, p.wait_us);
-            if (wm < BW_UTC_MIN_US_DEV) wm = BW_UTC_MIN_US_DEV;
+            wm = bw_sub_sat(h.max_ts, p.wait_us);  // (no floor needed: see above)
           }
           // survivors: newest and second newest
           int i0 = -1, i1 = -1, alive = 0;

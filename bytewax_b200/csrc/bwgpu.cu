@@ -1922,6 +1922,8 @@ static const char* status_name(u32 s) {
   switch (s) {
     case BW_ERR_CAPACITY: return "capacity exhausted (key table, pane pool, exchange region or emit buffer): raise capacity_hint / max_emit_rows / max_late_rows";
     case BW_ERR_RANGE: return "window id out of range (timestamp too far from align_to for this window length)";
+    case BW_ERR_STATE: return "ordered fold with event time ahead of the system clock: at this notify phase the reference would "
+                              "also wake keys at the timestamp of their oldest queued item, which the device does not keep";
     default: return "device-side failure";
   }
 }

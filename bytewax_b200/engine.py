@@ -229,7 +229,16 @@ class _GpuWindowStep:
         now = self._now_us()
         if now is None or now <= 0:
             return []
-        return self._rows(self.fold.advance(system_now_us=now), [])
+        from bytewax_b200 import _native as N
+
+        try:
+            em = self.fold.advance(system_now_us=now)
+        except N.BwError as e:
+            if e.status != N.BW_ERR_STATE:
+                raise
+            raise TypeError(f"step {self.step_id!r}: {e}; run this step with ordered=False, or keep event time at or "
+                            f"behind the system clock") from None
+        return self._rows(em, [])
 
     def on_eof(self) -> list:
         if self.fold is None:

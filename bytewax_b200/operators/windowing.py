@@ -619,12 +619,13 @@ def fold_window(step_id: str, up: KeyedStream, clock: Clock, windower: Windower,
 
 def _plan_for(reduction: str, clock, windower, ordered, value_of=_identity) -> Optional[GpuFoldPlan]:
     # (SystemClock == an event clock whose timestamps are the arrival times, wait 0: every item is at the watermark)
-    if isinstance(clock, (EventClock, SystemClock)) and isinstance(windower, (SlidingWindower, TumblingWindower)):
+    # An identity `to_system_utc` only: the device's notify phase compares a window's close, in event time, with the
+    # system clock directly, where the reference passes it through `to_system_utc` first (windowing.py:1177-1178).
+    identity_utc = isinstance(clock, SystemClock) or (isinstance(clock, EventClock) and clock.to_system_utc is _identity)
+    if identity_utc and isinstance(windower, (SlidingWindower, TumblingWindower)):
         return GpuFoldPlan(reduction, clock, windower, ordered, value_of)
-    # session windows (K7): unordered only, and an identity `to_system_utc` (the device's notify phase compares event
-    # time with the system clock directly, windowing.py:1177-1178)
-    if isinstance(windower, SessionWindower) and not ordered and (
-            isinstance(clock, SystemClock) or (isinstance(clock, EventClock) and clock.to_system_utc is _identity)):
+    # session windows (K7): unordered only, and likewise an identity `to_system_utc`
+    if isinstance(windower, SessionWindower) and not ordered and identity_utc:
         return GpuFoldPlan(reduction, clock, windower, ordered, value_of)
     return None
 
