@@ -165,7 +165,6 @@ struct ScatterArgs {
   u32 batch_no;
   u32 nstage;        // TMA stages in shared memory (2 or 3)
   u32 rec_idx;       // 1: records carry the arrival index; 0: the slot / fingerprint tag
-  u32 dbg;           // diagnostics only (env BW_SC_DBG): 1 skip the record stores, 2 skip the position atomics, 4 skip the verdict
   u32 world, nb_local;  // multi-GPU: bucket = owning rank * nb_local + segment of the key in the owner's table
   u32 stg_cap;       // records per bucket assembled in shared memory before they are written out (0: every record straight out)
   u32 stg_every;     // ... every this many tiles
@@ -345,7 +344,7 @@ __global__ void __launch_bounds__(BW_SC_THREADS, 1) k_scatter(ScatterArgs A, Fol
       }
     }
     // lateness triple of this warp's 64 consecutive rows; the last warp of the tile concatenates the tile's
-    if (TSM != 2 && !(A.dbg & 4u)) {
+    if (TSM != 2) {
       Trip ct = bw_trip_id();
       if ((u32)warp * 64u < rows) {
         const i64 nxt = __shfl_down_sync(0xffffffffu, ta, 1);
@@ -400,11 +399,10 @@ __global__ void __launch_bounds__(BW_SC_THREADS, 1) k_scatter(ScatterArgs A, Fol
         const u64 slot = bw_slot_of_khash(hh, A.cap);
         u32 b = (u32)(slot >> A.seg_shift);
         if (A.world > 1) b += bw_route_hash(bw_mix64(k), A.world) * A.nb_local;
-        const u32 pos = (A.dbg & 2u) ? (u32)(row & 7u) : bw_atoms_add_u32(lcur + 4 * b, 1u);
+        const u32 pos = bw_atoms_add_u32(lcur + 4 * b, 1u);
         const uint4 rec4 = make_uint4((u32)k, (u32)(k >> 32), (u32)rel, A.rec_idx ? (u32)row : bw_rec_tag(hh, slot, seg_mask));
         const u32 soff = pos - bw_lds_u32(fbase + 4 * b);  // rows of the bucket since the last write-out
-        if (A.dbg & 1u) stored = true;
-        else if (VB_OUT == 0 && soff < A.stg_cap && pos < A.lane_cap) {
+        if (VB_OUT == 0 && soff < A.stg_cap && pos < A.lane_cap) {
           asm volatile("st.shared.v4.u32 [%0], {%1,%2,%3,%4};" ::"r"(stg + 16 * (b * A.stg_cap + soff)), "r"(rec4.x), "r"(rec4.y), "r"(rec4.z),
                        "r"(rec4.w)
                        : "memory");

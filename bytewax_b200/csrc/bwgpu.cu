@@ -332,6 +332,7 @@ struct bw_fold {
   bw_fold_spec spec{};
   FoldParams p{};
   Table t{};
+  int force_seg_shift = -1;  // env BW_SEG_SHIFT: t.seg_shift in place of BW_SEG_SHIFT_DEFAULT (-1: not set)
   EmitBufs e{};
   Counters* d_ctr = nullptr;
   Counters* h_ctr = nullptr;  // pinned mirror
@@ -399,6 +400,8 @@ struct bw_fold {
   size_t segfold_smem = 0, scatter_smem = 0;
   int scatter_nstage = 3;
   u32 last_scatter_grid = 0, scatter_stg_cap = 0, scatter_stg_every = 1;
+  // env BW_SC_STG / BW_SC_EVERY / BW_SC_STAGES: the three above, in place of what stream_alloc picks for the shape (-1: not set)
+  int force_stg_cap = -1, force_stg_every = -1, force_nstage = -1;
   // multi-GPU streaming path: combine at the source, partials over NVLink, merge at the owner
   segfold_kernel_t combine_kernel = nullptr, merge_kernel = nullptr;
   int combine_grid = 0, merge_grid = 0;
@@ -427,8 +430,6 @@ struct bw_fold {
   void* snap_dev = nullptr;
   void* snap_host = nullptr;
   unsigned long long* d_snap_ctr = nullptr;
-  bool sub_auto = true;     // env BW_SUB_AUTO=0: never split an activation by its event-time span
-  u64 sub_rows = ~0ULL;  // optional fold + close granularity inside one activation (env BW_SUB_ROWS); measured slower on C1
   // multi-GPU exchange
   void* xchg_base = nullptr;  // one allocation, IPC-shared
   size_t xchg_bytes = 0;
@@ -695,7 +696,6 @@ static bw_status stream_alloc(bw_fold* f) {
   const int W = ctx->world;
   f->nb_local = (u32)(f->t.cap >> f->t.seg_shift);
   const u64 nb = (u64)f->nb_local * W;  // buckets of the scatter: (owning rank, segment of its table)
-  if (const char* e = getenv("BW_STREAM")) f->stream_mode = atoi(e) ? 1 : 0;
   if (!f->stream_mode || nb > BW_STREAM_MAX_NB || rows >= (1ULL << 28)) return BW_OK;
   if (W > 1 && f->spec.exchange != BW_XCHG_P2P) return BW_OK;  // the partials travel as peer stores
   // wait == forever with event time: nothing closes before EOF, every key grows an overflow list of panes --
@@ -738,9 +738,6 @@ static bw_status stream_alloc(bw_fold* f) {
   CU(ctx, own.dev(&sb.tile_max, 2 * (size_t)sb.tiles_cap));
   CU(ctx, own.dev(&sb.tile_bad, 2 * (size_t)sb.tiles_cap));
   CU(ctx, own.dev(&sb.chunk_max, 2 * (size_t)sb.tiles_cap * BW_SC_WARPS));
-  if (const char* e = getenv("BW_LATE_SPLIT")) f->late_split = atoi(e) != 0;
-  if (const char* e = getenv("BW_FLUSH")) f->flush_on = atoi(e) != 0;
-  if (const char* e = getenv("BW_TIMER_STRIDE")) f->timer_stride = (u32)std::max(1, atoi(e));
   // Shared memory of the scatter: up to 16 records per bucket assembled before they are written out (counts only: the
   // value column is not staged), then as many TMA stages of the input tile (2..4) as still fit.  Deeper staging beats
   // more stages: on C1 (489 buckets; H100 SXM, 700 W) 16 records with 2 stages take 0.309 ms, 8 records with 4 stages
@@ -753,14 +750,14 @@ static bw_status stream_alloc(bw_fold* f) {
         f->scatter_stg_cap = c;
         break;
       }
-  if (const char* e = getenv("BW_SC_STG")) f->scatter_stg_cap = (u32)std::max(0, std::min(16, atoi(e)));
+  if (f->force_stg_cap >= 0) f->scatter_stg_cap = (u32)f->force_stg_cap;
   // write out when an average bucket has assembled ~7/8 of its staging rows (C1 on an H100 SXM, 700 W, 16 records:
   // every tile 0.349 ms, every 2 tiles 0.310, every 3 -- this rule's choice -- 0.309)
   f->scatter_stg_every = (u32)std::max<double>(1.0, std::floor(0.875 * f->scatter_stg_cap * (double)sb.nb / BW_SC_TILE));
-  if (const char* e = getenv("BW_SC_EVERY")) f->scatter_stg_every = (u32)std::max(1, atoi(e));
+  if (f->force_stg_every >= 0) f->scatter_stg_every = (u32)f->force_stg_every;
   f->scatter_nstage = 4;
   while (f->scatter_nstage > 2 && bw_scatter_smem(tsm, vb_in, f->scatter_nstage, sb.nb, f->scatter_stg_cap) > smem_budget) --f->scatter_nstage;
-  if (const char* e = getenv("BW_SC_STAGES")) f->scatter_nstage = std::max(2, std::min(4, atoi(e)));
+  if (f->force_nstage >= 0) f->scatter_nstage = f->force_nstage;
   if (bw_scatter_smem(tsm, vb_in, f->scatter_nstage, sb.nb, f->scatter_stg_cap) > 216 * 1024) return BW_OK;  // too many segments
   f->scatter_smem = bw_scatter_smem(tsm, vb_in, f->scatter_nstage, sb.nb, f->scatter_stg_cap);
   // the attribute belongs to the kernel, not to this fold: folds with other table sizes share it
@@ -818,15 +815,11 @@ static bw_status stream_alloc(bw_fold* f) {
 static bw_status fold_alloc(bw_fold* f) {
   bw_ctx* ctx = f->ctx;
   const bw_fold_spec& s = f->spec;
-  // table: capacity_hint / load factor slots (load 0.5 by default, env BW_LOAD_PCT), a whole number of
-  // segments of BW_SEG_SLOTS slots: linear probing wraps inside a segment (bw_stream.cuh owns whole segments)
-  int load_pct = 50;
-  if (const char* e = getenv("BW_LOAD_PCT")) {
-    int v = atoi(e);
-    if (v >= 10 && v <= 90) load_pct = v;
-  }
+  // table: capacity_hint keys at a load of load_pct percent, in a whole number of segments of 2^seg_shift slots: linear
+  // probing wraps inside a segment (bw_stream.cuh owns whole segments)
+  const u64 load_pct = 50;
   u32 seg_shift = BW_SEG_SHIFT_DEFAULT;
-  if (const char* e = getenv("BW_SEG_SHIFT")) seg_shift = (u32)std::max(10, std::min(12, atoi(e)));
+  if (f->force_seg_shift >= 0) seg_shift = (u32)f->force_seg_shift;
   const u64 seg_slots = 1ULL << seg_shift;
   u64 cap = std::max<u64>(seg_slots, (std::max<u64>(s.capacity_hint, 1) * 100 + load_pct - 1) / load_pct);
   cap = (cap + seg_slots - 1) & ~(seg_slots - 1);
@@ -898,11 +891,6 @@ static bw_status fold_alloc(bw_fold* f) {
   // L2 for the second-pane array at window boundaries; plain LRU + evict_first input loads instead.
   int occ = 0;
   f->fold_kernel = pick_fold_kernel(f->p);
-  if (const char* e = getenv("BW_SUB_AUTO")) f->sub_auto = atoi(e) != 0;
-  if (const char* e = getenv("BW_SUB_ROWS")) {
-    long long v = atoll(e);
-    if (v >= 1024) f->sub_rows = (u64)v;
-  }
   CU(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, f->fold_kernel, BW_FOLD_THREADS, 0));
   if (occ < 1) occ = 1;
   f->fold_grid = ctx->sm_count * occ;
@@ -974,6 +962,19 @@ static bw_status xchg_setup(bw_fold* f) {
   return BW_OK;
 }
 
+// The environment switches, the library's only environment reads.  Tests and diagnostics use them to force a path or a
+// kernel configuration that production folds reach through other shapes; they are read once, when a fold is created.
+static void read_switches(bw_fold* f) {
+  if (const char* e = getenv("BW_STREAM")) f->stream_mode = atoi(e) ? 1 : 0;
+  if (const char* e = getenv("BW_LATE_SPLIT")) f->late_split = atoi(e) != 0;
+  if (const char* e = getenv("BW_FLUSH")) f->flush_on = atoi(e) != 0;
+  if (const char* e = getenv("BW_TIMER_STRIDE")) f->timer_stride = (u32)std::max(1, atoi(e));
+  if (const char* e = getenv("BW_SC_STG")) f->force_stg_cap = std::max(0, std::min(16, atoi(e)));
+  if (const char* e = getenv("BW_SC_EVERY")) f->force_stg_every = std::max(1, atoi(e));
+  if (const char* e = getenv("BW_SC_STAGES")) f->force_nstage = std::max(2, std::min(4, atoi(e)));
+  if (const char* e = getenv("BW_SEG_SHIFT")) f->force_seg_shift = std::max(10, std::min(12, atoi(e)));
+}
+
 bw_status bw_fold_create(bw_ctx* ctx, const bw_fold_spec* spec, bw_fold** out) {
   if (!ctx || !spec || !out) CTX_FAIL(ctx, BW_ERR_SPEC, "bw_fold_create: NULL argument");
   if (spec->struct_size != sizeof(bw_fold_spec))
@@ -996,6 +997,7 @@ bw_status bw_fold_create(bw_ctx* ctx, const bw_fold_spec* spec, bw_fold** out) {
   bw_fold* f = fp.get();
   f->ctx = ctx;
   f->spec = *spec;
+  read_switches(f);
   FoldParams& p = f->p;
   p.length_us = spec->length_us;
   p.offset_us = spec->offset_us;
@@ -1267,16 +1269,11 @@ static bw_status direct_fold(bw_fold* f, const BatchView& bv, u64 known, u32 bat
   // the pane holding max_ts never closes).  One sub-range per pane of event-time span, for
   // in-order streams; activations inside one pane (C1 on one GPU) are not split.
   u32 n_sub = 1;
-  if (f->sub_rows != ~0ULL) {
-    n_sub = (u32)std::min<u64>((known + f->sub_rows - 1) / f->sub_rows, 64);
-  } else if (f->sub_auto && f->p.track_wm) {
-    if (tmax > tmin) {
-      const u64 panes = (u64)(tmax - tmin) / (u64)f->p.pane_us + (((u64)(tmax - tmin) % (u64)f->p.pane_us) ? 1 : 0);
-      n_sub = (u32)std::min<u64>(panes, 8);
-      n_sub = (u32)std::min<u64>(n_sub, std::max<u64>(known >> 20, 1));  // keep sub-ranges >= 2^20 rows
-    }
+  if (f->p.track_wm && tmax > tmin) {
+    const u64 panes = (u64)(tmax - tmin) / (u64)f->p.pane_us + (((u64)(tmax - tmin) % (u64)f->p.pane_us) ? 1 : 0);
+    n_sub = (u32)std::min<u64>(panes, 8);
+    n_sub = (u32)std::min<u64>(n_sub, std::max<u64>(known >> 20, 1));  // keep sub-ranges >= 2^20 rows
   }
-  if (n_sub < 1) n_sub = 1;
   for (u32 i = 0; i < n_sub; ++i) {
     const u64 n_hi = (known * (i + 1ULL)) / n_sub, n_lo = (known * (u64)i) / n_sub;
     EventPair* ep;
@@ -1333,7 +1330,6 @@ static bw_status stream_front(bw_fold* f, const u64* d_keys, const void* d_vals,
   A.seg_shift = f->t.seg_shift;
   A.nstage = (u32)f->scatter_nstage;
   A.rec_idx = f->p.seq_by_id ? 0u : 1u;
-  if (const char* e = getenv("BW_SC_DBG")) A.dbg = (u32)atoi(e);
   A.stg_cap = f->scatter_stg_cap;
   A.stg_every = f->scatter_stg_every;
   A.batch_no = batch_no;

@@ -284,24 +284,14 @@ def test_stragglers_without_the_sort(ctx, fold_mode, red, length, offset, wait, 
     orc.close()
 
 
-@pytest.mark.parametrize("sub_rows", [None, "20000"])
-def test_activation_spanning_several_windows(ctx, fold_mode, sub_rows):
+def test_activation_spanning_several_windows(ctx, fold_mode):
     """In-order activations that each span 3.5 windows: the direct kernel folds them in sub-ranges with a
-    close in between (by event-time span, or forced every 20000 rows); rows must not change."""
+    close in between (one per pane of event-time span); rows must not change."""
     S = 1_000_000
     A = 1_640_995_200_000_000
     n, nb, n_keys = 1 << 21, 3, 5000
-    old = os.environ.get("BW_SUB_ROWS")
-    if sub_rows:
-        os.environ["BW_SUB_ROWS"] = sub_rows
-    try:
-        fold = _make_fold(ctx, dict(reduction="count", length_us=10 * S, offset_us=None, align_us=A, wait_us=2 * S, ordered=False),
-                          False, capacity_hint=8192, max_batch_rows=n, max_emit_rows=1 << 20)
-    finally:
-        if old is None:
-            os.environ.pop("BW_SUB_ROWS", None)
-        else:
-            os.environ["BW_SUB_ROWS"] = old
+    fold = _make_fold(ctx, dict(reduction="count", length_us=10 * S, offset_us=None, align_us=A, wait_us=2 * S, ordered=False),
+                      False, capacity_hint=8192, max_batch_rows=n, max_emit_rows=1 << 20)
     orc = coracle.COracle("count", 10 * S, None, A, 2 * S, False)
     rnd = np.random.default_rng(11)
     for b in range(nb):

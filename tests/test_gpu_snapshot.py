@@ -57,8 +57,7 @@ def fold_mode(request):
 
 @pytest.fixture(autouse=True)
 def default_env(monkeypatch):
-    for k in ("BW_LATE_SPLIT", "BW_SC_STG", "BW_SC_EVERY", "BW_SC_STAGES", "BW_SEG_SHIFT", "BW_SUB_ROWS", "BW_SUB_AUTO",
-              "BW_FLUSH", "BW_LOAD_PCT"):
+    for k in ("BW_LATE_SPLIT", "BW_SC_STG", "BW_SC_EVERY", "BW_SC_STAGES", "BW_SEG_SHIFT", "BW_FLUSH"):
         monkeypatch.delenv(k, raising=False)
 
 
