@@ -190,6 +190,16 @@ class BwArgwinRows(C.Structure):
                 ("n_released", C.c_uint64), ("released", C.POINTER(C.c_uint64))]
 
 
+class BwKcollectSpec(C.Structure):
+    _fields_ = [("struct_size", C.c_uint32), ("pad", C.c_int32), ("max_size", C.c_uint64), ("capacity_hint", C.c_uint64),
+                ("max_batch_rows", C.c_uint64), ("max_emit_rows", C.c_uint64)]
+
+
+class BwKcollectRows(C.Structure):
+    _fields_ = [("n", C.c_uint64), ("key", C.POINTER(C.c_uint64)), ("epoch", C.POINTER(C.c_uint64)),
+                ("offset", C.POINTER(C.c_uint64)), ("handle", C.POINTER(C.c_uint64))]
+
+
 # every symbol include/bwgpu.h declares: (restype, argtypes)
 _P = C.c_void_p
 SYMBOLS = {
@@ -267,6 +277,12 @@ SYMBOLS = {
     "bw_argwin_apply_device": (C.c_int32, [_P, _P, _P, _P, _P, C.c_uint64, C.c_uint64, C.c_int64]),
     "bw_argwin_advance": (C.c_int32, [_P, C.c_int64, C.POINTER(BwArgwinRows)]),
     "bw_argwin_eof": (C.c_int32, [_P, C.POINTER(BwArgwinRows)]),
+    "bw_kcollect_create": (C.c_int32, [_P, C.POINTER(BwKcollectSpec), C.POINTER(_P)]),
+    "bw_kcollect_destroy": (None, [_P]),
+    "bw_kcollect_apply": (C.c_int32, [_P, _P, _P, C.c_uint64, C.c_uint64, C.c_int64]),
+    "bw_kcollect_apply_device": (C.c_int32, [_P, _P, _P, C.c_uint64, C.c_uint64, C.c_int64]),
+    "bw_kcollect_advance": (C.c_int32, [_P, C.c_int64, C.POINTER(BwKcollectRows)]),
+    "bw_kcollect_eof": (C.c_int32, [_P, C.POINTER(BwKcollectRows)]),
     "bw_dev_alloc": (C.c_int32, [_P, C.c_uint64, C.POINTER(_P)]),
     "bw_dev_free": (C.c_int32, [_P, _P]),
     "bw_host_alloc": (C.c_int32, [_P, C.c_uint64, C.POINTER(_P)]),

@@ -40,6 +40,7 @@
 #include "bw_sjwin.cuh"
 #include "bw_scwin.cuh"
 #include "bw_argwin.cuh"
+#include "bw_kcollect.cuh"
 #include "bw_prepass.cuh"
 #include "bw_slow.cuh"
 #include "bw_late.cuh"
@@ -3483,16 +3484,14 @@ static cudaError_t collect_grow_keep(J* j, T** p, u64 used, u64 grow) {
   return cudaSuccess;
 }
 
-// Before a call that can play `values` values (its rows, and ordered the queued entries): compact the store once dead
-// entries outnumber live ones, then grow the store, the staging buffer and the release buffer so that nothing the call
-// can add or close overflows them.  Called after the drain: nothing on the stream reads them.  (J: bw_collect, bw_scwin)
+// Before a call that can add `adds` entries to the store: compact the store once dead entries outnumber live ones, then
+// grow the store and the staging buffer so that nothing the call can add or stage overflows them.  Called after the
+// drain: nothing on the stream reads them.  (J: bw_collect, bw_scwin, bw_kcollect)
 template <class J>
-static bw_status collect_room(J* j, u64 rows) {
+static bw_status store_room(J* j, u64 adds) {
   bw_ctx* ctx = j->ctx;
-  CwStore& es = j->es;
-  CwEmit& e = j->e;
-  bw_status st = jwin_room(j, rows);
-  if (st != BW_OK) return st;
+  auto& es = j->es;
+  auto& e = j->e;
   if (j->dead && j->dead >= j->n_store - j->dead) {  // stream compaction (entry order does not matter: each has its rank)
     const int grid = ctx->sm_count * 4;
     k_cwin_live<<<grid, 256, 0, j->s>>>(es.ref, j->d_flag, j->n_store);
@@ -3509,7 +3508,6 @@ static bw_status collect_room(J* j, u64 rows) {
     j->n_store -= j->dead;
     j->dead = 0;
   }
-  const u64 adds = (rows + (j->spec.ordered ? j->nq : 0)) * j->kmax;
   const u64 live = j->n_store - j->dead;
   if (j->n_store + adds > es.cap) {
     const u64 grow = std::max<u64>(j->n_store + adds, 2 * es.cap);
@@ -3528,6 +3526,15 @@ static bw_status collect_room(J* j, u64 rows) {
     e.max_stage = grow;
   }
   return BW_OK;
+}
+
+// Before a call that can play `rows` values (and ordered the queued entries): room in the store, the staging buffer and
+// the release buffer for all it can add or close.  (J: bw_collect, bw_scwin)
+template <class J>
+static bw_status collect_room(J* j, u64 rows) {
+  bw_status st = jwin_room(j, rows);
+  if (st != BW_OK) return st;
+  return store_room(j, (rows + (j->spec.ordered ? j->nq : 0)) * j->kmax);
 }
 
 // after the per-key kernels of a call: move the closed windows' entries out (k_cwin_gather)
@@ -4657,4 +4664,265 @@ bw_status bw_argwin_eof(bw_argwin* a, bw_argwin_rows* out) {
   bw_status st = argwin_wake(a, 1);
   if (st != BW_OK) return st;
   return argwin_collect(a, out);
+}
+
+// ===========================================================================
+// K13 host side: keyed collect (bw_kcollect.cuh)
+// ===========================================================================
+struct bw_kcollect {
+  Owner own;  // every buffer and the stream below
+  bw_ctx* ctx = nullptr;
+  bw_kcollect_spec spec{};
+  KcTable t{};
+  CwStore es{};
+  KeyedScratch k;
+  cudaStream_t s = nullptr;
+  u32* h_err = nullptr;                 // err, why
+  unsigned long long* d_cnt = nullptr;  // lists, staged handles, store entries, carried entries moved out
+  unsigned long long* h_cnt = nullptr;
+  unsigned char* d_flag = nullptr;
+  u64* d_handles = nullptr;
+  KcSeg* d_seg = nullptr;
+  KcEmit e{};
+  u64 n_store = 0, dead = 0;      // entries in the store, and how many of them are dead
+  u64 n_rows = 0, n_stage = 0;    // lists and staged handles since the last advance / eof
+  SortScratch srt;                // ordering and compaction scratch
+  u32* d_inv = nullptr;           // advance / eof: a list's place in the reference's order
+  u64 *d_cs = nullptr, *d_off = nullptr;  // its count in that order, and the exclusive scan of them
+  u64* d_out = nullptr;           // the handles in the reference's order
+  u64* h_out = nullptr;
+  u64 out_cap = 0;
+  HostCols hd;                    // key, epoch, offsets
+  bool undrained = false;         // a call whose counts are not read back yet
+  u32 batch_no = 0;
+  u64 calls = 0, first_call = 0;  // calls (activations, notify phases, EOF) so far; the first not yet collected
+  u64 last_epoch = 0;
+  bool failed = false;
+};
+
+bw_status bw_kcollect_create(bw_ctx* ctx, const bw_kcollect_spec* spec, bw_kcollect** out) {
+  if (!ctx || !spec || !out) CTX_FAIL(ctx, BW_ERR_SPEC, "bw_kcollect_create: NULL argument");
+  if (spec->struct_size != sizeof(bw_kcollect_spec)) CTX_FAIL(ctx, BW_ERR_SPEC, "bw_kcollect_spec.struct_size mismatch");
+  if (ctx->world != 1) CTX_FAIL(ctx, BW_ERR_SPEC, "keyed collects run on one GPU (world == 1)");
+  if (spec->max_size < 1) CTX_FAIL(ctx, BW_ERR_SPEC, "max_size must be at least 1");
+  if (spec->max_batch_rows == 0 || spec->max_batch_rows >= (1ULL << 31)) CTX_FAIL(ctx, BW_ERR_SPEC, "bad max_batch_rows");
+  if (spec->max_emit_rows >= (1ULL << 31)) CTX_FAIL(ctx, BW_ERR_SPEC, "max_emit_rows must be below 2^31");
+  if (spec->capacity_hint >= (1ULL << 30)) CTX_FAIL(ctx, BW_ERR_SPEC, "capacity_hint must be below 2^30");
+  CU(ctx, cudaSetDevice(ctx->device));
+  std::unique_ptr<bw_kcollect, void (*)(bw_kcollect*)> cp(new bw_kcollect(), bw_kcollect_destroy);  // torn down on every failure
+  bw_kcollect* j = cp.get();
+  Owner& own = j->own;
+  j->ctx = ctx;
+  j->spec = *spec;
+  const u64 cap = std::max<u64>(1024, 2 * std::max<u64>(spec->capacity_hint, 1));
+  KcTable& t = j->t;
+  t.cap = cap;
+  t.M = spec->max_size;
+  CU(ctx, own.stream(&j->s));
+  CU(ctx, own.dev(&t.keys, cap + 1));
+  CU(ctx, own.dev(&t.cnt, cap + 1));
+  CU(ctx, own.dev(&t.due, cap + 1));
+  CU(ctx, own.dev(&t.mv_ord, cap + 1));
+  CU(ctx, own.dev(&t.mv_base, cap + 1));
+  CU(ctx, own.dev(&t.mv_rec, cap + 1));
+  CU(ctx, own.dev(&t.err, 2));
+  t.why = t.err + 1;
+  CU(ctx, own.dev(&j->d_cnt, 4));
+  CU(ctx, cudaMemsetAsync(t.err, 0, 8, j->s));
+  CU(ctx, cudaMemsetAsync(j->d_cnt, 0, 32, j->s));
+  CU(ctx, own.host(&j->h_err, 64 / sizeof(u32)));
+  CU(ctx, own.host(&j->h_cnt, 64 / sizeof(unsigned long long)));
+  const u64 n = spec->max_batch_rows, m = std::max<u64>(spec->max_emit_rows, 1);
+  bw_status st = keyed_alloc(ctx, own, j->k, n, j->s);
+  if (st != BW_OK) return st;
+  CU(ctx, own.dev(&j->d_handles, n));
+  CU(ctx, own.dev(&j->d_seg, n));
+  KcEmit& e = j->e;
+  for (u64** c : {&e.key, &e.cnt, &e.soff, &e.epoch, &e.ord, &e.seq}) CU(ctx, own.dev(c, m));
+  CU(ctx, own.dev(&j->d_inv, m));
+  CU(ctx, own.dev(&j->d_cs, m + 1));
+  CU(ctx, own.dev(&j->d_off, m + 1));
+  // the store, the staging buffer and the output grow with what the collect holds (store_room, collect_place); they
+  // start at one batch
+  CwStore& es = j->es;
+  es.cap = n;
+  CU(ctx, own.dev(&es.ref, n));
+  CU(ctx, own.dev(&es.rank, n));
+  CU(ctx, own.dev(&es.h, n));
+  CU(ctx, own.dev(&j->d_flag, n));
+  e.max_stage = n;
+  CU(ctx, own.dev(&e.stage, n));
+  CU(ctx, own.dev(&e.stage_rec, n));
+  j->out_cap = n;
+  CU(ctx, own.dev(&j->d_out, n));
+  CU(ctx, own.host(&j->h_out, n));
+  e.max_rows = spec->max_emit_rows;
+  e.n_rows = j->d_cnt;
+  e.n_stage = j->d_cnt + 1;
+  es.n = j->d_cnt + 2;
+  e.n_moved = j->d_cnt + 3;
+  CU(ctx, j->srt.reserve(own, m, m, j->s));
+  size_t b = 0;
+  CU(ctx, cub::DeviceScan::ExclusiveSum(nullptr, b, j->d_cs, j->d_off, (int)(m + 1), j->s));
+  CU(ctx, j->srt.grow_cub(own, b + 256));
+  CU(ctx, j->hd.reserve(own, m + 1, m + 1));
+  k_kcol_init<<<ctx->sm_count * 4, 256, 0, j->s>>>(t);
+  CU(ctx, cudaGetLastError());
+  CU(ctx, cudaStreamSynchronize(j->s));
+  *out = cp.release();
+  return BW_OK;
+}
+
+void bw_kcollect_destroy(bw_kcollect* j) {
+  if (!j) return;
+  cudaSetDevice(j->ctx->device);
+  if (j->s) cudaStreamSynchronize(j->s);
+  delete j;  // j->own releases every buffer and the stream
+}
+
+static KcParams kcollect_params(bw_kcollect* j, u64 epoch, i64 timeout_at) {
+  KcParams p;
+  p.epoch = epoch;
+  p.ord = j->calls++;
+  p.timeout_at = timeout_at;
+  return p;
+}
+
+#define KCOLLECT_REFUSE_FAILED(j) \
+  if ((j)->failed) CTX_FAIL((j)->ctx, BW_ERR_STATE, "keyed collect: an earlier call failed on the device; the collect is unusable")
+
+// wait for the last call; fail on a device-side overflow; then take its counts
+static bw_status kcollect_drain(bw_kcollect* j) {
+  bw_ctx* ctx = j->ctx;
+  KCOLLECT_REFUSE_FAILED(j);
+  if (!j->undrained) return BW_OK;
+  CU(ctx, cudaMemcpyAsync(j->h_err, j->t.err, 8, cudaMemcpyDeviceToHost, j->s));
+  CU(ctx, cudaMemcpyAsync(j->h_cnt, j->d_cnt, 32, cudaMemcpyDeviceToHost, j->s));
+  CU(ctx, cudaStreamSynchronize(j->s));
+  if (j->h_err[0]) {
+    j->failed = true;
+    const u32 w = j->h_err[1];
+    CTX_FAIL(ctx, (bw_status)j->h_err[0], "keyed collect kernel ran out of capacity:%s%s%s%s",
+             w & BW_JW_FULL_TABLE ? " key table full (raise capacity_hint);" : "",
+             w & BW_JW_FULL_EMIT ? " more than max_emit_rows lists since the last advance;" : "",
+             w & BW_CW_FULL_STORE ? " carry store or staging buffer full;" : "", w ? "" : " (no reason recorded)");
+  }
+  j->n_rows = j->h_cnt[0];
+  j->n_stage = j->h_cnt[1];
+  j->n_store = j->h_cnt[2];
+  j->dead += j->h_cnt[3];
+  CU(ctx, cudaMemsetAsync(j->d_cnt + 3, 0, 8, j->s));
+  CU(ctx, cudaStreamSynchronize(j->s));
+  j->undrained = false;
+  return BW_OK;
+}
+
+// the carried entries of every key whose carry moved to a list in this call, to their staging slots (k_kcol_gather);
+// the store's entries added by this call lie past n_store and are not looked at
+static bw_status kcollect_gather(bw_kcollect* j, const KcParams& p) {
+  if (j->n_store) k_kcol_gather<<<j->ctx->sm_count * 8, 256, 0, j->s>>>(j->t, j->e, j->es, p, j->n_store);
+  CU(j->ctx, cudaGetLastError());
+  return BW_OK;
+}
+
+bw_status bw_kcollect_apply_device(bw_kcollect* j, const uint64_t* d_keys, const uint64_t* d_handles, uint64_t rows, uint64_t epoch,
+                                   int64_t timeout_at_us) {
+  if (!j) return BW_ERR_SPEC;
+  bw_ctx* ctx = j->ctx;
+  KCOLLECT_REFUSE_FAILED(j);
+  if (rows > j->spec.max_batch_rows) CTX_FAIL(ctx, BW_ERR_SPEC, "keyed collect: rows > max_batch_rows");
+  if (rows && (!d_keys || !d_handles)) CTX_FAIL(ctx, BW_ERR_SPEC, "keyed collect: NULL column");
+  if (j->batch_no && epoch < j->last_epoch) CTX_FAIL(ctx, BW_ERR_STATE, "keyed collect: epochs must not decrease");
+  CU(ctx, cudaSetDevice(ctx->device));
+  bw_status st = kcollect_drain(j);
+  if (st != BW_OK) return st;
+  j->last_epoch = epoch;
+  const KcParams p = kcollect_params(j, epoch, timeout_at_us);
+  j->batch_no++;
+  if (rows == 0) return BW_OK;
+  if ((st = store_room(j, rows)) != BW_OK) return st;
+  st = keyed_group(ctx, j->k, d_keys, rows, j->s);
+  if (st != BW_OK) return st;
+  const int grid = ctx->sm_count * 8;
+  k_kcol_keys<<<grid, 256, 0, j->s>>>(j->t, j->e, j->es, p, j->d_seg, j->k.d_ksorted, j->k.d_head, rows);
+  k_kcol_rows<<<grid, 256, 0, j->s>>>(j->t, j->e, j->es, p, j->d_seg, j->k.d_ksorted, j->k.d_isorted, j->k.d_head, d_handles, rows);
+  CU(ctx, cudaGetLastError());
+  j->undrained = true;
+  return kcollect_gather(j, p);
+}
+
+bw_status bw_kcollect_apply(bw_kcollect* j, const uint64_t* keys, const uint64_t* handles, uint64_t rows, uint64_t epoch,
+                            int64_t timeout_at_us) {
+  if (!j) return BW_ERR_SPEC;
+  bw_ctx* ctx = j->ctx;
+  if (rows > j->spec.max_batch_rows) CTX_FAIL(ctx, BW_ERR_SPEC, "keyed collect: rows > max_batch_rows");
+  if (rows && (!keys || !handles)) CTX_FAIL(ctx, BW_ERR_SPEC, "keyed collect: NULL column");
+  CU(ctx, cudaSetDevice(ctx->device));
+  bw_status st = kcollect_drain(j);
+  if (st != BW_OK) return st;
+  if (rows) {
+    CU(ctx, cudaMemcpyAsync(j->k.d_keys, keys, rows * 8, cudaMemcpyHostToDevice, j->s));
+    CU(ctx, cudaMemcpyAsync(j->d_handles, handles, rows * 8, cudaMemcpyHostToDevice, j->s));
+  }
+  st = bw_kcollect_apply_device(j, j->k.d_keys, j->d_handles, rows, epoch, timeout_at_us);
+  if (st != BW_OK) return st;
+  // the host columns may be reused by the caller once this returns
+  return kcollect_drain(j);
+}
+
+static bw_status kcollect_collect(bw_kcollect* j, bw_kcollect_rows* out) {
+  bw_ctx* ctx = j->ctx;
+  bw_status st = kcollect_drain(j);
+  if (st != BW_OK) return st;
+  const u64 nd = j->n_rows, ns = j->n_stage;  // within bounds: kcollect_drain passed
+  const KcEmit& e = j->e;
+  const u64* cols[] = {e.key, e.epoch};
+  if ((st = jwin_ship(j, nd, e.key, e.seq, e.ord, cols, 2, &j->hd)) != BW_OK) return st;
+  if ((st = collect_place(j, nd, ns, j->hd.col[2])) != BW_OK) return st;
+  CU(ctx, cudaGetLastError());
+  CU(ctx, cudaMemsetAsync(j->d_cnt, 0, 16, j->s));
+  CU(ctx, cudaStreamSynchronize(j->s));
+  j->n_rows = j->n_stage = 0;
+  j->first_call = j->calls;
+  out->n = nd;
+  out->key = j->hd.col[0];
+  out->epoch = j->hd.col[1];
+  out->offset = j->hd.col[2];
+  out->handle = j->h_out;
+  return BW_OK;
+}
+
+// notify phase or EOF: every due (EOF: every live) key's carry becomes a list
+static bw_status kcollect_wake(bw_kcollect* j, i64 now, int eof) {
+  bw_ctx* ctx = j->ctx;
+  bw_status st = kcollect_drain(j);
+  if (st != BW_OK) return st;
+  if ((st = store_room(j, 0)) != BW_OK) return st;
+  const KcParams p = kcollect_params(j, j->last_epoch, 0);
+  k_kcol_due<<<ctx->sm_count * 8, 256, 0, j->s>>>(j->t, j->e, p, now, eof);
+  CU(ctx, cudaGetLastError());
+  j->undrained = true;
+  return kcollect_gather(j, p);
+}
+
+bw_status bw_kcollect_advance(bw_kcollect* j, int64_t now_us, bw_kcollect_rows* out) {
+  if (!j || !out) return BW_ERR_SPEC;
+  bw_ctx* ctx = j->ctx;
+  KCOLLECT_REFUSE_FAILED(j);
+  CU(ctx, cudaSetDevice(ctx->device));
+  if (now_us > 0) {
+    bw_status st = kcollect_wake(j, now_us, 0);
+    if (st != BW_OK) return st;
+  }
+  return kcollect_collect(j, out);
+}
+
+bw_status bw_kcollect_eof(bw_kcollect* j, bw_kcollect_rows* out) {
+  if (!j || !out) return BW_ERR_SPEC;
+  bw_ctx* ctx = j->ctx;
+  KCOLLECT_REFUSE_FAILED(j);
+  CU(ctx, cudaSetDevice(ctx->device));
+  bw_status st = kcollect_wake(j, 0, 1);
+  if (st != BW_OK) return st;
+  return kcollect_collect(j, out);
 }

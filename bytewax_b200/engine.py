@@ -221,7 +221,7 @@ class _GpuWindowStep:
         if now is not None and now > 0:
             self.fold.set_system_now(now)
 
-    def on_notify(self) -> list:
+    def on_notify(self, now: Optional[datetime] = None) -> list:
         """The notify phase (src/operators.rs:808-858): keys whose earliest window's close time has come close what their
         watermark -- which moves with the system clock -- allows, without waiting for another item or EOF."""
         if self.fold is None:
@@ -295,7 +295,7 @@ class _GpuWindowStep:
 
 
 class _NoClock:
-    def on_notify(self) -> list:
+    def on_notify(self, now: Optional[datetime] = None) -> list:
         return []
 
 
@@ -353,7 +353,7 @@ class _GpuSessionStep(_GpuWindowStep):
         self.sess.apply(np.array(keys, dtype=np.uint64), v, np.array(ts, dtype=np.int64), self.last_epoch, now or 0)
         return self._session_rows(self.sess.advance(), orig)
 
-    def on_notify(self) -> list:
+    def on_notify(self, now: Optional[datetime] = None) -> list:
         if self.sess is None:
             return []
         now = self._now_us()
@@ -454,7 +454,7 @@ class _GpuJoinWindowStep(_GpuWindowStep):
             max_queued_rows=1 << 22 if plan.ordered else 0, max_batch_rows=int(os.environ.get("BYTEWAX_B200_BATCH", 1 << 22)),
             max_emit_rows=1 << 22, max_late_rows=1 << 22)
 
-    def on_notify(self) -> list:
+    def on_notify(self, now: Optional[datetime] = None) -> list:
         if self.jwin is None:
             return []
         now = self._now_us()
@@ -798,7 +798,7 @@ def _td_us(td: timedelta) -> int:
 
 
 def _gpu_step_for(step_id: str, plan):
-    from bytewax_b200.operators import GpuFinalPlan, GpuJoinPlan, GpuSmapPlan
+    from bytewax_b200.operators import GpuCollectPlan, GpuFinalPlan, GpuJoinPlan, GpuSmapPlan
     from bytewax_b200.operators.windowing import (GpuArgWindowPlan, GpuCollectWindowPlan, GpuJoinWindowPlan,
                                                   GpuSessionCollectWindowPlan, SessionWindower)
 
@@ -818,6 +818,8 @@ def _gpu_step_for(step_id: str, plan):
         return _GpuSmapStep(step_id, plan)
     if isinstance(plan, GpuJoinPlan):
         return _GpuJoinStep(step_id, plan)
+    if isinstance(plan, GpuCollectPlan):
+        return _GpuCollectStep(step_id, plan)
     return _GpuFinalStep(step_id, plan) if isinstance(plan, GpuFinalPlan) else _GpuWindowStep(step_id, plan)
 
 
@@ -984,6 +986,71 @@ class _GpuFinalStep(_NoClock, _GpuWindowStep):
         self.fold = None
         rows = [(self._key_str(k), acc) for k, acc in zip(em.closed_key.tolist(), em.closed_acc.tolist())]
         if self.resort:
+            rows.sort(key=lambda r: r[0])
+        return rows
+
+
+class _GpuCollectStep(_GpuJoinWindowStep):
+    """One worker's ``collect`` (``GpuCollectPlan``) on ``bw_kcollect_*`` (K13): `_CollectLogic` under `stateful`
+    (operators/__init__.py:1113-1164, 1025-1062), one call per activation.  Key interning, the handle dict and the
+    release are the join step's; each list is built here from its handles, and its objects are dropped with it.
+
+    The host logic samples ``now_getter()`` per item; this step samples it once per activation, after the batch is
+    converted, so a timeout can fire later by at most that activation's host processing time.  Rows are the host
+    engine's whenever the clock does not move within one activation."""
+
+    def __init__(self, step_id: str, plan):
+        import numpy as np
+
+        self.np, self.plan, self.step_id = np, plan, step_id
+        self.key_ids: Dict[str, int] = {}
+        self.id_keys: Dict[int, str] = {}
+        self.resort = False
+        self.last_epoch = 0
+        self.values: Dict[int, Any] = {}  # handle -> value, while the device holds the handle
+        self.next_handle = 0
+        self.jwin = None
+
+    def on_epoch(self, epoch: int, items: list) -> list:
+        from bytewax_b200 import gpu, operators
+
+        keys, handles = [], []
+        for item in items:
+            key, value = _split_item(self.step_id, item)
+            keys.append(self._key_id(key))
+            handles.append(self.next_handle)
+            self.values[self.next_handle] = value
+            self.next_handle += 1
+        try:  # the reference's own `now_getter() + timeout` (:1122), read at call time so a patched clock reaches it
+            timeout_at = operators._get_system_utc() + self.plan.timeout
+        except (OverflowError, TypeError) as ex:
+            if self.jwin is None:  # the first batch: the host logic runs it and raises its own error
+                raise _GpuPlanUnfit(f"timeout {self.plan.timeout!r}") from ex
+            raise type(ex)(f"step {self.step_id!r}: `now + timeout` is out of range: {ex}") from ex
+        if self.jwin is None:
+            self.jwin = gpu.KeyCollect(_get_gpu_ctx(), self.plan.max_size, capacity_hint=int(os.environ.get("BYTEWAX_B200_KEYS", 1 << 20)),
+                                       max_batch_rows=int(os.environ.get("BYTEWAX_B200_BATCH", 1 << 22)), max_emit_rows=1 << 22)
+        self.last_epoch = max(epoch, self.last_epoch)
+        np = self.np
+        self.jwin.apply(np.array(keys, dtype=np.uint64), np.array(handles, dtype=np.uint64), self.last_epoch, _us(timeout_at))
+        return self._lists(self.jwin.advance())
+
+    def on_notify(self, now: Optional[datetime] = None) -> list:
+        if self.jwin is None or now is None:
+            return []
+        return self._lists(self.jwin.advance(now_us=_us(now)))
+
+    def on_eof(self) -> list:
+        if self.jwin is None:
+            return []
+        out = self._lists(self.jwin.eof())
+        self.release()
+        return out
+
+    def _lists(self, out) -> list:
+        V = self.values
+        rows = [(self._key_str(k), [V.pop(h) for h in hs]) for k, hs in zip(out.key.tolist(), out.lists())]
+        if self.resort:  # interned (non-numeric) keys: restore ascending key-string order; stable
             rows.sort(key=lambda r: r[0])
         return rows
 
@@ -1251,7 +1318,7 @@ class _Run:
                             _reraise(f"error in the CUDA fold of step {st.step_id}", ex)
                     if g is not None:
                         try:
-                            self._emit(st.down, w, epoch, g.on_notify())
+                            self._emit(st.down, w, epoch, g.on_notify(now))
                         except Exception as ex:
                             _reraise(f"error in the CUDA fold of step {st.step_id}", ex)
                         continue

@@ -794,6 +794,83 @@ class CollectWindow:
 
 
 @dataclass
+class KeyCollectRows:
+    """Lists of one ``KeyCollect.advance`` / ``eof``, in the reference's downstream order: per call, ascending key string,
+    a key's lists in the order they filled.  List i is ``handle[offset[i]:offset[i + 1]]`` in arrival order; every
+    handle passed to ``apply`` comes back exactly once, in the list that holds it."""
+
+    key: np.ndarray
+    epoch: np.ndarray
+    offset: np.ndarray  # len(key) + 1
+    handle: np.ndarray
+
+    def lists(self) -> List[List[int]]:
+        """The handles of every list, in arrival order."""
+        h, o = self.handle.tolist(), self.offset.tolist()
+        return [h[o[i]:o[i + 1]] for i in range(len(o) - 1)]
+
+
+class KeyCollect:
+    """The keyed ``collect(timeout, max_size)`` (``bw_kcollect``, K13; operators/__init__.py:1113-1216).  Values travel as
+    uint64 handles; the caller keeps the objects and builds each list from its handles.  ``max_size`` must be >= 1."""
+
+    def __init__(self, ctx: Context, max_size: int, capacity_hint: int = 1 << 16, max_batch_rows: int = 1 << 20,
+                 max_emit_rows: int = 1 << 20):
+        self.ctx, self.lib = ctx, ctx.lib
+        s = N.BwKcollectSpec()
+        s.struct_size = C.sizeof(N.BwKcollectSpec)
+        s.max_size, s.capacity_hint, s.max_batch_rows, s.max_emit_rows = max_size, capacity_hint, max_batch_rows, max_emit_rows
+        self.spec = s
+        h = C.c_void_p()
+        N.check(self.lib.bw_kcollect_create(ctx.h, C.byref(s), C.byref(h)), ctx.h)
+        self.h = h
+        self._epoch = 0
+
+    def _next_epoch(self, epoch: Optional[int]) -> int:
+        if epoch is None:
+            self._epoch += 1
+            return self._epoch
+        return epoch
+
+    def apply(self, keys, handles, epoch: Optional[int] = None, timeout_at_us: int = 0):
+        """One activation from host arrays.  ``timeout_at_us``: the activation's ``now_getter() + timeout``."""
+        keys = np.ascontiguousarray(keys, dtype=np.uint64)
+        handles = np.ascontiguousarray(handles, dtype=np.uint64)
+        vp = lambda a: a.ctypes.data_as(C.c_void_p)  # noqa: E731
+        N.check(self.lib.bw_kcollect_apply(self.h, vp(keys), vp(handles), keys.shape[0], self._next_epoch(epoch), int(timeout_at_us)),
+                self.ctx.h)
+
+    def apply_device(self, d_keys: int, d_handles: int, rows: int, epoch: Optional[int] = None, timeout_at_us: int = 0):
+        N.check(self.lib.bw_kcollect_apply_device(self.h, C.c_void_p(d_keys), C.c_void_p(d_handles), rows, self._next_epoch(epoch),
+                                                  int(timeout_at_us)), self.ctx.h)
+
+    def _wrap(self, r: N.BwKcollectRows) -> KeyCollectRows:
+        n = int(r.n)
+
+        def arr(ptr, k):
+            return np.ctypeslib.as_array(ptr, shape=(k,)).copy() if k else np.zeros(0, np.uint64)
+
+        off = arr(r.offset, n + 1)
+        return KeyCollectRows(arr(r.key, n), arr(r.epoch, n), off, arr(r.handle, int(off[-1])))
+
+    def advance(self, now_us: int = 0) -> KeyCollectRows:
+        """Lists since the last call; ``now_us`` > 0 first emits every list whose timeout is <= ``now_us``."""
+        r = N.BwKcollectRows()
+        N.check(self.lib.bw_kcollect_advance(self.h, int(now_us), C.byref(r)), self.ctx.h)
+        return self._wrap(r)
+
+    def eof(self) -> KeyCollectRows:
+        r = N.BwKcollectRows()
+        N.check(self.lib.bw_kcollect_eof(self.h, C.byref(r)), self.ctx.h)
+        return self._wrap(r)
+
+    def close(self):
+        if self.h:
+            self.lib.bw_kcollect_destroy(self.h)
+            self.h = None
+
+
+@dataclass
 class SessionCollectWindowRows(CollectWindowRows):
     """Rows of one ``SessionCollectWindow.advance`` / ``eof``.  Each down row is a closed session: its handles in
     flattened play order (``lists()``), its merge intervals (``merges(i)``) and its ``M`` row's bounds and merged ids

@@ -469,6 +469,16 @@ class _CollectLogic(StatefulLogic):
         return copy.deepcopy(self.state)
 
 
+@dataclass(frozen=True)
+class GpuCollectPlan:
+    """A ``collect`` whose ``max_size`` is an ``int``: the engine may run it with ``bw_kcollect_*`` (K13).  ``max_size`` is
+    stored as ``max(1, min(max_size, 2**64 - 1))``, which splits lists exactly where the reference does; values travel as
+    handles, so they can be any Python object."""
+
+    timeout: timedelta
+    max_size: int
+
+
 @operator
 def collect(step_id: str, up: KeyedStream, timeout: timedelta, max_size: int) -> KeyedStream:
     """operators/__init__.py:1167."""
@@ -477,7 +487,8 @@ def collect(step_id: str, up: KeyedStream, timeout: timedelta, max_size: int) ->
         state = resume_state if resume_state is not None else _CollectState()
         return _CollectLogic(step_id, _get_system_utc, timeout, max_size, state)
 
-    return stateful("stateful", up, shim_builder)
+    plan = GpuCollectPlan(timeout, max(1, min(max_size, 2**64 - 1))) if isinstance(max_size, int) else None
+    return stateful("stateful", up, shim_builder, _gpu_plan=plan)
 
 
 @operator

@@ -838,6 +838,50 @@ bw_status bw_argwin_advance(bw_argwin* a, int64_t system_now_us, bw_argwin_rows*
 /* End of input: every key closes at watermark UTC_MAX (:1144-1151), so sessions with close >= UTC_MAX - gap stay open. */
 bw_status bw_argwin_eof(bw_argwin* a, bw_argwin_rows* out);
 
+/* Keyed collect (K13): `collect(step_id, up, timeout, max_size)` (pysrc/bytewax/operators/__init__.py:1106-1216), i.e.
+ * `_CollectLogic` (:1113-1164) under `stateful` (:1025-1062).  Values travel as u64 handles (any u64: none is reserved);
+ * the objects stay with the caller.  Per key, per call, in arrival order: every item appends its handle to the key's
+ * list and sets the key's timeout to the call's `timeout_at_us` (`now_getter() + timeout`, :1122); a list that reaches
+ * max_size is emitted and the key's logic discarded, so its next item, even in the same call, starts a new list
+ * (:1124-1127, :1030-1042).  A key's slot is kept after a discard.  One GPU only. */
+typedef struct bw_kcollect bw_kcollect;
+typedef struct bw_kcollect_spec {
+  uint32_t struct_size;
+  int32_t pad;
+  uint64_t max_size;        /* >= 1: a list is emitted when it holds this many handles (the engine maps max_size <= 1 to 1) */
+  uint64_t capacity_hint;   /* live keys; a key's slot is kept once seen */
+  uint64_t max_batch_rows;
+  uint64_t max_emit_rows;   /* lists retained between bw_kcollect_advance calls, < 2^31 */
+} bw_kcollect_spec;
+/* Lists handed downstream since the last advance / eof, in the reference's order: per call (activation, notify phase or
+ * EOF), ascending key string (src/operators.rs:758-767, :808-858, :862-894); a key's lists in the order they filled.
+ * List i is handle[offset[i] .. offset[i + 1]) in arrival order.  Every handle appears exactly once, in the list that
+ * holds it: that is when the caller may drop its object.  Host pointers into memory owned by the library, valid until
+ * the next advance / eof / destroy. */
+typedef struct bw_kcollect_rows {
+  uint64_t n;
+  const uint64_t* key;
+  const uint64_t* epoch;
+  const uint64_t* offset;   /* n + 1 entries */
+  const uint64_t* handle;   /* offset[n] entries */
+} bw_kcollect_rows;
+bw_status bw_kcollect_create(bw_ctx* ctx, const bw_kcollect_spec* spec, bw_kcollect** out);
+void bw_kcollect_destroy(bw_kcollect* c);
+/* One activation from HOST columns (keys, handles); blocks.  `timeout_at_us` is the activation's `now_getter() +
+ * timeout` (the reference samples the clock per item).  The carry store and the staging and output buffers grow before
+ * each call to what it can add; a full key table or more than max_emit_rows lists since the last advance returns
+ * BW_ERR_CAPACITY (reason in bw_last_error) and the collect refuses further calls. */
+bw_status bw_kcollect_apply(bw_kcollect* c, const uint64_t* keys, const uint64_t* handles, uint64_t rows, uint64_t epoch,
+                            int64_t timeout_at_us);
+/* Same with DEVICE columns; returns once the work is enqueued (the columns must stay valid until the next call). */
+bw_status bw_kcollect_apply_device(bw_kcollect* c, const uint64_t* d_keys, const uint64_t* d_handles, uint64_t rows, uint64_t epoch,
+                                   int64_t timeout_at_us);
+/* Lists since the last call.  `now_us` > 0 first runs the notify phase (src/operators.rs:808-858, `on_notify` :1132-1133):
+ * every key holding a list whose timeout is <= now_us emits it and is reset.  now_us <= 0: only the rows. */
+bw_status bw_kcollect_advance(bw_kcollect* c, int64_t now_us, bw_kcollect_rows* out);
+/* End of input: every key holding a list emits it (`on_eof` :1136-1137, src/operators.rs:862-894). */
+bw_status bw_kcollect_eof(bw_kcollect* c, bw_kcollect_rows* out);
+
 /* ---- plain device-memory helpers (tests / bench / host bindings without torch) ---- */
 bw_status bw_dev_alloc(bw_ctx* ctx, uint64_t bytes, void** out);
 bw_status bw_dev_free(bw_ctx* ctx, void* ptr);
