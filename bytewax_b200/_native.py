@@ -123,6 +123,13 @@ class BwJwinRows(C.Structure):
                 ("n_released", C.c_uint64), ("released", C.POINTER(C.c_uint64))]
 
 
+class BwPjwinSpec(C.Structure):
+    _fields_ = [("struct_size", C.c_uint32), ("emit_mode", C.c_int32), ("ordered", C.c_int32), ("sides", C.c_int32),
+                ("max_windows_per_key", C.c_int32), ("length_us", C.c_int64), ("offset_us", C.c_int64), ("align_us", C.c_int64),
+                ("wait_us", C.c_int64), ("capacity_hint", C.c_uint64), ("max_queued_rows", C.c_uint64), ("max_batch_rows", C.c_uint64),
+                ("max_emit_rows", C.c_uint64), ("max_late_rows", C.c_uint64), ("max_product_rows", C.c_uint64)]
+
+
 class BwCollectSpec(C.Structure):
     _fields_ = [("struct_size", C.c_uint32), ("ordered", C.c_int32), ("max_windows_per_key", C.c_int32), ("pad", C.c_int32),
                 ("length_us", C.c_int64), ("offset_us", C.c_int64), ("align_us", C.c_int64), ("wait_us", C.c_int64),
@@ -283,6 +290,12 @@ SYMBOLS = {
     "bw_kcollect_apply_device": (C.c_int32, [_P, _P, _P, C.c_uint64, C.c_uint64, C.c_int64]),
     "bw_kcollect_advance": (C.c_int32, [_P, C.c_int64, C.POINTER(BwKcollectRows)]),
     "bw_kcollect_eof": (C.c_int32, [_P, C.POINTER(BwKcollectRows)]),
+    "bw_pjwin_create": (C.c_int32, [_P, C.POINTER(BwPjwinSpec), C.POINTER(_P)]),
+    "bw_pjwin_destroy": (None, [_P]),
+    "bw_pjwin_apply": (C.c_int32, [_P, _P, _P, _P, _P, C.c_uint64, C.c_uint64, C.c_int64]),
+    "bw_pjwin_apply_device": (C.c_int32, [_P, _P, _P, _P, _P, C.c_uint64, C.c_uint64, C.c_int64]),
+    "bw_pjwin_advance": (C.c_int32, [_P, C.c_int64, C.POINTER(BwJwinRows)]),
+    "bw_pjwin_eof": (C.c_int32, [_P, C.POINTER(BwJwinRows)]),
     "bw_dev_alloc": (C.c_int32, [_P, C.c_uint64, C.POINTER(_P)]),
     "bw_dev_free": (C.c_int32, [_P, _P]),
     "bw_host_alloc": (C.c_int32, [_P, C.c_uint64, C.POINTER(_P)]),

@@ -41,6 +41,7 @@
 #include "bw_scwin.cuh"
 #include "bw_argwin.cuh"
 #include "bw_kcollect.cuh"
+#include "bw_pjwin.cuh"
 #include "bw_prepass.cuh"
 #include "bw_slow.cuh"
 #include "bw_late.cuh"
@@ -3027,14 +3028,15 @@ static bw_status jwin_drain(J* j) {
   if (j->h_err[0]) {
     j->failed = true;
     const u32 w = j->h_err[1];
-    CTX_FAIL(ctx, (bw_status)j->h_err[0], "%s kernel %s:%s%s%s%s%s%s%s%s", jwin_what(j),
+    CTX_FAIL(ctx, (bw_status)j->h_err[0], "%s kernel %s:%s%s%s%s%s%s%s%s%s", jwin_what(j),
              j->h_err[0] == BW_ERR_SPEC ? "rejected its input" : "ran out of capacity",
              w & BW_JW_BAD_SIDE ? " a side column value is not below sides;" : "", w & BW_JW_FULL_TABLE ? " key table full (raise capacity_hint);" : "",
              w & BW_JW_FULL_WINDOWS ? jwin_full_windows(j) : "",
              w & BW_JW_FULL_EMIT ? jwin_full_emit(j) : "",
              w & BW_JW_FULL_LATE ? " more than max_late_rows late rows since the last advance;" : "",
              w & BW_JW_FULL_QUEUE ? " more than max_queued_rows queued entries;" : "",
-             w & BW_CW_FULL_STORE ? " entry store or staging buffer full;" : "", w ? "" : " (no reason recorded)");
+             w & BW_CW_FULL_STORE ? " entry store or staging buffer full;" : "",
+             w & BW_PJ_FULL_SIDE ? " a window's side list reached 2^32 values;" : "", w ? "" : " (no reason recorded)");
   }
   const u64 nr = j->h_cnt[3];
   j->outstanding -= std::min(nr, j->outstanding);
@@ -4925,4 +4927,467 @@ bw_status bw_kcollect_eof(bw_kcollect* j, bw_kcollect_rows* out) {
   bw_status st = kcollect_wake(j, 0, 1);
   if (st != BW_OK) return st;
   return kcollect_collect(j, out);
+}
+
+// ===========================================================================
+// K14 host side: windowed product join (bw_pjwin.cuh)
+// ===========================================================================
+struct bw_pjwin {
+  Owner own;  // every buffer and the stream below
+  bw_ctx* ctx = nullptr;
+  bw_pjwin_spec spec{};
+  PjTable t{};
+  PjStore es{};
+  KeyedScratch k;
+  cudaStream_t s = nullptr;
+  u32* h_err = nullptr;  // err, why
+  // events, meta, late, released, carried-over queue entries, stage records, staged, store entries, values, dead entries
+  unsigned long long* d_cnt = nullptr;
+  unsigned long long* h_cnt = nullptr;
+  unsigned char *d_side = nullptr, *d_late = nullptr, *d_flag = nullptr, *d_vflag = nullptr;
+  u64* d_handles = nullptr;
+  i64* d_ts = nullptr;
+  PjEmit e{};
+  JwPool pool{}, pool2{};  // ordered mode: the queue, and the one the next flush writes
+  u64 nq = 0;              // entries in `pool`
+  int slot_bits = 1;
+  u64 kmax = 1;                        // entries one value can add: min(ceil(length / offset), max_windows_per_key)
+  u64 n_store = 0, dead = 0;           // entries in the store, and how many of them are dead
+  u64 n_vals = 0;                      // value slots in use (live and dead) since the last compaction
+  u64 n_rec = 0, n_meta = 0, n_stage = 0;  // stage records, meta rows and staged handles since the last advance / eof
+  SortScratch srt;                     // pool sort, ordering and compaction scratch
+  PjOrdered o{};                       // advance / eof: the events in the reference's order
+  u64* d_off = nullptr;                // the exclusive scan of their row counts
+  u64 *d_vlive = nullptr, *d_vmap = nullptr;  // value compaction: live flags and their scan
+  PjRows rows{};                       // the expanded rows
+  u64 rows_cap = 0;
+  HostCols hd[2];                      // down: key, window id, h0, h1, h2 | h3, mask, epoch
+  HostCols hm, hl;                     // meta: key, window id, epoch; late: key, window id, epoch, activation, row
+  std::vector<u64> released;           // since the last advance / eof
+  std::vector<u64> released_out;       // what the last advance / eof handed out
+  bool undrained = false;     // a call whose counts are not read back yet
+  u64 outstanding = 0;        // handles passed in and not released yet: what the next call can release, besides its own
+  u32 batch_no = 0;
+  u64 calls = 0, first_call = 0;  // calls (activations, notify phases, EOF) so far; the first not yet collected
+  u64 last_epoch = 0;
+  i64 now = INT64_MIN;
+  bool failed = false;
+};
+
+static const char* jwin_what(const bw_pjwin*) { return "windowed product join"; }
+static const char* jwin_full_windows(const bw_pjwin*) { return " a key needs more than max_windows_per_key open windows;"; }
+static const char* jwin_full_emit(const bw_pjwin*) { return " more than max_emit_rows emissions or meta rows since the last advance;"; }
+static u64 jwin_counters(const bw_pjwin*) { return 10; }
+
+bw_status bw_pjwin_create(bw_ctx* ctx, const bw_pjwin_spec* spec, bw_pjwin** out) {
+  if (!ctx || !spec || !out) CTX_FAIL(ctx, BW_ERR_SPEC, "bw_pjwin_create: NULL argument");
+  if (spec->struct_size != sizeof(bw_pjwin_spec)) CTX_FAIL(ctx, BW_ERR_SPEC, "bw_pjwin_spec.struct_size mismatch");
+  if (ctx->world != 1) CTX_FAIL(ctx, BW_ERR_SPEC, "windowed product joins run on one GPU (world == 1)");
+  if (spec->emit_mode < BW_JOIN_EMIT_COMPLETE || spec->emit_mode > BW_JOIN_EMIT_RUNNING) CTX_FAIL(ctx, BW_ERR_SPEC, "bad emit_mode");
+  if (spec->ordered != 0 && spec->ordered != 1) CTX_FAIL(ctx, BW_ERR_SPEC, "ordered must be 0 or 1");
+  if (spec->sides < 1 || spec->sides > BW_JW_MAXSIDES) CTX_FAIL(ctx, BW_ERR_SPEC, "sides must be in 1..%d", BW_JW_MAXSIDES);
+  if (spec->max_windows_per_key < 1 || spec->max_windows_per_key > BW_JW_MAXM)
+    CTX_FAIL(ctx, BW_ERR_SPEC, "max_windows_per_key must be in 1..%d", BW_JW_MAXM);
+  if (spec->length_us <= 0 || spec->length_us > BW_UTC_MAX_US - BW_UTC_MIN_US) CTX_FAIL(ctx, BW_ERR_SPEC, "length_us must be in 1..UTC_MAX - UTC_MIN");
+  if (spec->offset_us <= 0 || spec->offset_us > spec->length_us) CTX_FAIL(ctx, BW_ERR_SPEC, "offset_us must be in 1..length_us");
+  if (spec->align_us < BW_UTC_MIN_US || spec->align_us > BW_UTC_MAX_US) CTX_FAIL(ctx, BW_ERR_SPEC, "align_us out of range");
+  if (spec->wait_us < 0) CTX_FAIL(ctx, BW_ERR_SPEC, "wait_us must not be negative");
+  if (spec->max_batch_rows == 0 || spec->max_batch_rows >= (1ULL << 31)) CTX_FAIL(ctx, BW_ERR_SPEC, "bad max_batch_rows");
+  if (spec->max_queued_rows >= (1ULL << 31) - spec->max_batch_rows) CTX_FAIL(ctx, BW_ERR_SPEC, "max_queued_rows + max_batch_rows must stay below 2^31");
+  if (spec->max_emit_rows >= (1ULL << 31)) CTX_FAIL(ctx, BW_ERR_SPEC, "max_emit_rows must be below 2^31");
+  if (spec->capacity_hint >= (1ULL << 30)) CTX_FAIL(ctx, BW_ERR_SPEC, "capacity_hint must be below 2^30");
+  CU(ctx, cudaSetDevice(ctx->device));
+  std::unique_ptr<bw_pjwin, void (*)(bw_pjwin*)> jp(new bw_pjwin(), bw_pjwin_destroy);  // torn down on every failure
+  bw_pjwin* j = jp.get();
+  Owner& own = j->own;
+  j->ctx = ctx;
+  j->spec = *spec;
+  const u64 cap = std::max<u64>(1024, 2 * std::max<u64>(spec->capacity_hint, 1));
+  const int M = spec->max_windows_per_key;
+  const u64 per = (u64)((spec->length_us - 1) / spec->offset_us) + 1;
+  j->kmax = std::min<u64>(per, (u64)M);
+  PjTable& t = j->t;
+  t.j.cap = cap;
+  t.j.M = M;
+  t.j.sides = spec->sides;
+  while ((1ULL << j->slot_bits) < cap + 1) ++j->slot_bits;
+  const u64 cells = (cap + 1) * (u64)M;
+  CU(ctx, own.stream(&j->s));
+  CU(ctx, own.dev(&t.j.keys, cap + 1));
+  CU(ctx, own.dev(&t.j.st, cap + 1));
+  CU(ctx, own.dev(&t.win, cells));
+  CU(ctx, own.dev(&t.cell, cells));
+  CU(ctx, own.dev(&t.rec_ord, cells));
+  CU(ctx, own.dev(&t.rec_c, cells));
+  CU(ctx, own.dev(&t.close_ord, cells));
+  CU(ctx, own.dev(&t.j.err, 2));
+  t.j.why = t.j.err + 1;
+  t.err = t.j.err;
+  t.why = t.j.why;
+  CU(ctx, own.dev(&j->d_cnt, 10));
+  CU(ctx, cudaMemsetAsync(t.err, 0, 8, j->s));
+  CU(ctx, cudaMemsetAsync(j->d_cnt, 0, 80, j->s));
+  CU(ctx, own.host(&j->h_err, 64 / sizeof(u32)));
+  CU(ctx, own.host(&j->h_cnt, 16));
+  const u64 n = spec->max_batch_rows, m = std::max<u64>(spec->max_emit_rows, 1), l = std::max<u64>(spec->max_late_rows, 1);
+  const u64 q = spec->ordered ? spec->max_queued_rows : 0;
+  bw_status st = keyed_alloc(ctx, own, j->k, n, j->s);
+  if (st != BW_OK) return st;
+  CU(ctx, own.dev(&j->d_side, n));
+  CU(ctx, own.dev(&j->d_late, n));
+  CU(ctx, own.dev(&j->d_handles, n));
+  CU(ctx, own.dev(&j->d_ts, n));
+  if (spec->ordered) {
+    if ((st = jwin_pool_alloc(ctx, own, j->pool, q + n)) != BW_OK) return st;
+    if ((st = jwin_pool_alloc(ctx, own, j->pool2, q + n)) != BW_OK) return st;
+  }
+  PjEmit& e = j->e;
+  for (u64** c : {&e.key, &e.wid, &e.epoch, &e.ord, &e.seq, &e.rec, &e.m_key, &e.m_wid, &e.m_epoch, &e.m_ord, &e.m_seq}) CU(ctx, own.dev(c, m));
+  for (u64** c : {&e.l_key, &e.l_wid, &e.l_epoch, &e.l_act, &e.l_row, &e.l_ord, &e.l_seq}) CU(ctx, own.dev(c, l));
+  for (u32** c : {&e.lo, &e.hi, &e.rb, &e.rn}) CU(ctx, own.dev(c, 4 * m));
+  CU(ctx, own.dev(&e.rbase, 4 * m));
+  PjOrdered& o = j->o;
+  for (u64** c : {&o.cnt, &o.key, &o.wid, &o.epoch}) CU(ctx, own.dev(c, m + 1));
+  CU(ctx, own.dev(&o.base, 4 * m));
+  CU(ctx, own.dev(&o.len, 4 * m));
+  CU(ctx, own.dev(&j->d_off, m + 1));
+  // the store, the values, the staging buffer, the release buffer and the output grow with what the join holds and
+  // emits (pjwin_room, pjwin_collect); they start at one batch
+  PjStore& es = j->es;
+  es.c.cap = n;
+  CU(ctx, own.dev(&es.c.ref, n));
+  CU(ctx, own.dev(&es.c.rank, n));
+  CU(ctx, own.dev(&es.c.h, n));
+  CU(ctx, own.dev(&es.vi, n));
+  CU(ctx, own.dev(&j->d_flag, n));
+  es.vcap = n;
+  CU(ctx, own.dev(&es.vcnt, n));
+  CU(ctx, own.dev(&j->d_vlive, n));
+  CU(ctx, own.dev(&j->d_vmap, n));
+  CU(ctx, own.dev(&j->d_vflag, n));
+  e.max_stage = n;
+  CU(ctx, own.dev(&e.stage, n));
+  e.max_rel = n;
+  CU(ctx, own.dev(&e.rel, e.max_rel));
+  e.max_rows = spec->max_emit_rows;
+  e.max_late = spec->max_late_rows;
+  e.max_queue = q;
+  e.n_rows = j->d_cnt;
+  e.n_meta = j->d_cnt + 1;
+  e.n_late = j->d_cnt + 2;
+  e.n_rel = j->d_cnt + 3;
+  e.n_next = j->d_cnt + 4;
+  e.n_rec = j->d_cnt + 5;
+  e.n_stage = j->d_cnt + 6;
+  es.c.n = j->d_cnt + 7;
+  es.nv = j->d_cnt + 8;
+  es.n_dead = j->d_cnt + 9;
+  const u64 ns = std::max(std::max(m, l), q + n);
+  CU(ctx, j->srt.reserve(own, ns, ns, j->s));
+  size_t b = 0;
+  CU(ctx, cub::DeviceScan::ExclusiveScan(nullptr, b, o.cnt, j->d_off, PjSatAdd{}, (u64)0, (int)(m + 1), j->s));
+  CU(ctx, j->srt.grow_cub(own, b + 256));
+  CU(ctx, j->hm.reserve(own, m, m));
+  CU(ctx, j->hl.reserve(own, l, l));
+  k_pjwin_init<<<ctx->sm_count * 4, 256, 0, j->s>>>(t);
+  CU(ctx, cudaGetLastError());
+  CU(ctx, cudaStreamSynchronize(j->s));
+  *out = jp.release();
+  return BW_OK;
+}
+
+void bw_pjwin_destroy(bw_pjwin* j) {
+  if (!j) return;
+  cudaSetDevice(j->ctx->device);
+  if (j->s) cudaStreamSynchronize(j->s);
+  delete j;  // j->own releases every buffer and the stream
+}
+
+static JwParams pjwin_params(bw_pjwin* j, u64 epoch) {
+  JwParams p{};
+  p.emit_mode = j->spec.emit_mode;
+  p.ordered = j->spec.ordered;
+  p.length = j->spec.length_us;
+  p.offset = j->spec.offset_us;
+  p.align = j->spec.align_us;
+  p.wait = j->spec.wait_us;
+  p.now = j->now;
+  p.epoch = epoch;
+  p.ord = j->calls++;
+  p.batch_no = j->batch_no;
+  return p;
+}
+
+// K8's drain (failure, released handles, queue count), then the counts only this join keeps
+static bw_status pjwin_drain(bw_pjwin* j) {
+  const bool pending = j->undrained;
+  bw_status st = jwin_drain(j);
+  if (st != BW_OK || !pending) return st;
+  j->n_meta = j->h_cnt[1];
+  j->n_rec = j->h_cnt[5];
+  j->n_stage = j->h_cnt[6];
+  j->n_store = j->h_cnt[7];
+  j->n_vals = j->h_cnt[8];
+  j->dead += j->h_cnt[9];
+  CU(j->ctx, cudaMemsetAsync(j->d_cnt + 9, 0, 8, j->s));
+  return BW_OK;
+}
+
+// Before a call that can play `rows` values (and ordered the queued entries): compact the store and the values once dead
+// entries outnumber live ones, then grow the store, the values, the staging buffer and the release buffer so that
+// nothing the call can add, stage or release overflows them.  Called after the drain: nothing on the stream reads them.
+static bw_status pjwin_room(bw_pjwin* j, u64 rows) {
+  bw_ctx* ctx = j->ctx;
+  bw_status st = jwin_room(j, rows);
+  if (st != BW_OK) return st;
+  PjStore& es = j->es;
+  PjEmit& e = j->e;
+  const u64 vadds = rows + (j->spec.ordered ? j->nq : 0), adds = vadds * j->kmax;
+  if (j->dead && j->dead >= j->n_store - j->dead) {  // stream compaction of the values, then of the entries (both stable)
+    const int grid = ctx->sm_count * 4;
+    size_t b = 0, b2 = 0, b3 = 0;
+    CU(ctx, cub::DeviceSelect::Flagged(nullptr, b, es.c.h, j->d_flag, es.c.n, (int64_t)j->n_store, j->s));
+    CU(ctx, cub::DeviceSelect::Flagged(nullptr, b2, es.vcnt, j->d_vflag, es.nv, (int64_t)j->n_vals, j->s));
+    CU(ctx, cub::DeviceScan::ExclusiveSum(nullptr, b3, j->d_vlive, j->d_vmap, (int64_t)j->n_vals, j->s));
+    CU(ctx, j->srt.grow_cub(j->own, std::max(std::max(b, b2), b3) + 256));
+    size_t tb = j->srt.cub_bytes;
+    if (j->n_vals) {
+      k_pjwin_vlive<<<grid, 256, 0, j->s>>>(es.vcnt, j->d_vlive, j->d_vflag, j->n_vals);
+      CU(ctx, cub::DeviceScan::ExclusiveSum(j->srt.cub, tb, j->d_vlive, j->d_vmap, (int64_t)j->n_vals, j->s));
+      tb = j->srt.cub_bytes;
+      CU(ctx, cub::DeviceSelect::Flagged(j->srt.cub, tb, es.vcnt, j->d_vflag, es.nv, (int64_t)j->n_vals, j->s));
+    }
+    k_cwin_live<<<grid, 256, 0, j->s>>>(es.c.ref, j->d_flag, j->n_store);
+    for (int c = 0; c < 4; ++c) {
+      tb = j->srt.cub_bytes;
+      if (c == 0) CU(ctx, cub::DeviceSelect::Flagged(j->srt.cub, tb, es.c.h, j->d_flag, es.c.n, (int64_t)j->n_store, j->s));
+      if (c == 1) CU(ctx, cub::DeviceSelect::Flagged(j->srt.cub, tb, es.c.rank, j->d_flag, es.c.n, (int64_t)j->n_store, j->s));
+      if (c == 2) CU(ctx, cub::DeviceSelect::Flagged(j->srt.cub, tb, es.vi, j->d_flag, es.c.n, (int64_t)j->n_store, j->s));
+      if (c == 3) CU(ctx, cub::DeviceSelect::Flagged(j->srt.cub, tb, es.c.ref, j->d_flag, es.c.n, (int64_t)j->n_store, j->s));
+    }
+    j->n_store -= j->dead;
+    j->dead = 0;
+    if (j->n_vals && j->n_store) k_pjwin_remap<<<grid, 256, 0, j->s>>>(es.vi, j->d_vmap, j->n_store);
+    CU(ctx, cudaGetLastError());
+    CU(ctx, cudaMemcpyAsync(j->h_cnt + 8, es.nv, 8, cudaMemcpyDeviceToHost, j->s));
+    CU(ctx, cudaStreamSynchronize(j->s));
+    j->n_vals = j->n_vals ? j->h_cnt[8] : 0;
+  }
+  const u64 live = j->n_store - j->dead;
+  if (j->n_store + adds > es.c.cap) {
+    const u64 grow = std::max<u64>(j->n_store + adds, 2 * es.c.cap);
+    es.c.cap = 0;  // (a failed regrow leaves the store unusable: the next call fails here again)
+    CU(ctx, collect_grow_keep(j, &es.c.ref, j->n_store, grow));
+    CU(ctx, collect_grow_keep(j, &es.c.rank, j->n_store, grow));
+    CU(ctx, collect_grow_keep(j, &es.c.h, j->n_store, grow));
+    CU(ctx, collect_grow_keep(j, &es.vi, j->n_store, grow));
+    CU(ctx, j->own.regrow(Owner::DEV, &j->d_flag, grow));
+    es.c.cap = grow;
+  }
+  if (j->n_vals + vadds > es.vcap) {
+    const u64 grow = std::max<u64>(j->n_vals + vadds, 2 * es.vcap);
+    es.vcap = 0;
+    CU(ctx, collect_grow_keep(j, &es.vcnt, j->n_vals, grow));
+    CU(ctx, j->own.regrow(Owner::DEV, &j->d_vlive, grow));
+    CU(ctx, j->own.regrow(Owner::DEV, &j->d_vmap, grow));
+    CU(ctx, j->own.regrow(Owner::DEV, &j->d_vflag, grow));
+    es.vcap = grow;
+  }
+  if (j->n_stage + live + adds > e.max_stage) {
+    const u64 grow = std::max<u64>(j->n_stage + live + adds, 2 * e.max_stage);
+    e.max_stage = 0;
+    CU(ctx, collect_grow_keep(j, &e.stage, j->n_stage, grow));
+    e.max_stage = grow;
+  }
+  return BW_OK;
+}
+
+#define PJWIN_REFUSE_FAILED(j) \
+  if ((j)->failed) CTX_FAIL((j)->ctx, BW_ERR_STATE, "windowed product join: an earlier call failed on the device; the join is unusable")
+
+// after the per-key kernels of a call: stage the emitting windows' lists, kill dead entries, release (k_pjwin_gather)
+static bw_status pjwin_gather(bw_pjwin* j, const JwParams& p) {
+  k_pjwin_gather<<<j->ctx->sm_count * 8, 256, 0, j->s>>>(j->t, j->e, j->es, p, j->n_rec, j->n_meta);
+  CU(j->ctx, cudaGetLastError());
+  return BW_OK;
+}
+
+// ordered mode: sort the pool's due entries into play order (K8's sort); then flush every woken key (k_pjwin_flush)
+static bw_status pjwin_flush(bw_pjwin* j, const JwParams& p, u64 n) {
+  bw_ctx* ctx = j->ctx;
+  bw_status st = j->spec.ordered ? jwin_sort_pool(j, j->t.j, p, n) : BW_OK;
+  if (st != BW_OK) return st;
+  PjEmit e = j->e;
+  e.next = j->pool2;
+  k_pjwin_flush<<<ctx->sm_count * 8, 256, 0, j->s>>>(j->t, e, j->es, p, j->pool, j->srt.perm);
+  CU(ctx, cudaGetLastError());
+  if (j->spec.ordered) std::swap(j->pool, j->pool2);  // the next call reads what this flush carried over (count: jwin_drain)
+  return pjwin_gather(j, p);
+}
+
+bw_status bw_pjwin_apply_device(bw_pjwin* j, const uint64_t* d_keys, const uint8_t* d_side, const uint64_t* d_handles, const int64_t* d_ts_us,
+                                uint64_t rows, uint64_t epoch, int64_t system_now_us) {
+  if (!j) return BW_ERR_SPEC;
+  bw_ctx* ctx = j->ctx;
+  PJWIN_REFUSE_FAILED(j);
+  if (rows > j->spec.max_batch_rows) CTX_FAIL(ctx, BW_ERR_SPEC, "windowed product join: rows > max_batch_rows");
+  if (rows && (!d_keys || !d_side || !d_handles || !d_ts_us)) CTX_FAIL(ctx, BW_ERR_SPEC, "windowed product join: NULL column");
+  if (j->batch_no && epoch < j->last_epoch) CTX_FAIL(ctx, BW_ERR_STATE, "windowed product join: epochs must not decrease");
+  CU(ctx, cudaSetDevice(ctx->device));
+  bw_status st = pjwin_drain(j);
+  if (st != BW_OK) return st;
+  j->last_epoch = epoch;
+  if (system_now_us > j->now) j->now = system_now_us;  // `now_getter()` never goes backwards (windowing.py:250-261)
+  const JwParams p = pjwin_params(j, epoch);
+  j->batch_no++;
+  if (rows == 0) return BW_OK;
+  if ((st = pjwin_room(j, rows)) != BW_OK) return st;
+  j->outstanding += rows;
+  st = keyed_group(ctx, j->k, d_keys, rows, j->s);
+  if (st != BW_OK) return st;
+  k_pjwin_apply<<<ctx->sm_count * 8, 256, 0, j->s>>>(j->t, j->e, j->es, p, j->pool, j->nq, j->k.d_ksorted, j->k.d_isorted, j->k.d_head,
+                                                     d_handles, d_side, d_ts_us, j->d_late, rows);
+  CU(ctx, cudaGetLastError());
+  j->undrained = true;
+  if (j->spec.ordered) return pjwin_flush(j, p, j->nq + rows);
+  return pjwin_gather(j, p);
+}
+
+static bw_status pjwin_apply_device_fn(bw_pjwin* j, const uint64_t* d_keys, const uint8_t* d_side, const uint64_t* d_handles,
+                                       const int64_t* d_ts_us, uint64_t rows, uint64_t epoch, int64_t system_now_us) {
+  bw_status st = bw_pjwin_apply_device(j, d_keys, d_side, d_handles, d_ts_us, rows, epoch, system_now_us);
+  if (st != BW_OK) return st;
+  return pjwin_drain(j);  // (jwin_apply_host drains once more: then nothing is pending)
+}
+
+bw_status bw_pjwin_apply(bw_pjwin* j, const uint64_t* keys, const uint8_t* side, const uint64_t* handles, const int64_t* ts_us, uint64_t rows,
+                         uint64_t epoch, int64_t system_now_us) {
+  if (j) {
+    PJWIN_REFUSE_FAILED(j);
+    bw_status st = pjwin_drain(j);  // (before jwin_apply_host's own drain, which would skip this join's counts)
+    if (st != BW_OK) return st;
+  }
+  return jwin_apply_host(j, keys, side, handles, ts_us, rows, epoch, system_now_us, pjwin_apply_device_fn);
+}
+
+// advance / eof: the events in the reference's order (order_perm), their row counts and the saturating scan of them;
+// the host grows the output to the total; k_pjwin_expand writes every row in that order
+static bw_status pjwin_expand(bw_pjwin* j, u64 nd, u64* total) {
+  bw_ctx* ctx = j->ctx;
+  *total = 0;
+  if (!nd) return BW_OK;
+  SortScratch& x = j->srt;
+  bw_status st = order_perm(ctx, x, j->s, nd, j->e.key, j->e.seq, j->e.ord, nullptr, std::max<u64>(j->calls - j->first_call, 1), j->first_call,
+                            nullptr);
+  if (st != BW_OK) return st;
+  const int grid = ctx->sm_count * 4;
+  PjOrdered o = j->o;
+  k_pjwin_count<<<grid, 256, 0, j->s>>>(j->e, o, j->spec.sides, x.perm, nd);
+  CU(ctx, cudaMemsetAsync(o.cnt + nd, 0, 8, j->s));
+  size_t tb = x.cub_bytes;
+  CU(ctx, cub::DeviceScan::ExclusiveScan(x.cub, tb, o.cnt, j->d_off, PjSatAdd{}, (u64)0, (int)(nd + 1), j->s));
+  CU(ctx, cudaMemcpyAsync(j->h_cnt + 12, j->d_off + nd, 8, cudaMemcpyDeviceToHost, j->s));
+  CU(ctx, cudaStreamSynchronize(j->s));
+  const u64 n = j->h_cnt[12];
+  if (n > j->spec.max_product_rows) {
+    j->failed = true;
+    CTX_FAIL(ctx, BW_ERR_CAPACITY, "windowed product join ran out of capacity: %llu product rows since the last advance, more than "
+             "max_product_rows (%llu)", (unsigned long long)n, (unsigned long long)j->spec.max_product_rows);
+  }
+  if (n > j->rows_cap) {
+    j->rows_cap = 0;
+    for (u64** c : {&j->rows.key, &j->rows.wid, &j->rows.h0, &j->rows.h1, &j->rows.h2, &j->rows.h3, &j->rows.mask, &j->rows.epoch})
+      CU(ctx, j->own.regrow(Owner::DEV, c, n));
+    j->rows_cap = n;
+  }
+  CU(ctx, j->hd[0].reserve(j->own, n, n));
+  CU(ctx, j->hd[1].reserve(j->own, n, n));
+  k_pjwin_expand<<<ctx->sm_count * 8, 256, 0, j->s>>>(o, j->d_off, nd, j->spec.sides, j->e.stage, j->rows, n);
+  const u64* src[] = {j->rows.key, j->rows.wid, j->rows.h0, j->rows.h1, j->rows.h2, j->rows.h3, j->rows.mask, j->rows.epoch};
+  for (int c = 0; c < 8; ++c) CU(ctx, cudaMemcpyAsync(j->hd[c / 5].col[c % 5], src[c], n * 8, cudaMemcpyDeviceToHost, j->s));
+  *total = n;
+  return BW_OK;
+}
+
+static bw_status pjwin_collect(bw_pjwin* j, bw_jwin_rows* out) {
+  bw_ctx* ctx = j->ctx;
+  bw_status st = pjwin_drain(j);
+  if (st != BW_OK) return st;
+  CU(ctx, cudaMemcpyAsync(j->h_cnt, j->d_cnt, 24, cudaMemcpyDeviceToHost, j->s));
+  CU(ctx, cudaStreamSynchronize(j->s));
+  const u64 nd = j->h_cnt[0], nm = j->h_cnt[1], nl = j->h_cnt[2];  // all within bounds: jwin_drain passed
+  u64 n = 0;
+  if ((st = pjwin_expand(j, nd, &n)) != BW_OK) return st;
+  const PjEmit& e = j->e;
+  const u64* meta[] = {e.m_key, e.m_wid, e.m_epoch};
+  const u64* late[] = {e.l_key, e.l_wid, e.l_epoch, e.l_act, e.l_row};
+  if ((st = jwin_ship(j, nm, e.m_key, e.m_seq, e.m_ord, meta, 3, &j->hm)) != BW_OK) return st;
+  if ((st = jwin_ship(j, nl, e.l_key, e.l_seq, e.l_ord, late, 5, &j->hl)) != BW_OK) return st;
+  CU(ctx, cudaGetLastError());
+  CU(ctx, cudaMemsetAsync(j->d_cnt, 0, 24, j->s));
+  CU(ctx, cudaMemsetAsync(j->d_cnt + 5, 0, 16, j->s));
+  CU(ctx, cudaStreamSynchronize(j->s));
+  j->n_rec = j->n_meta = j->n_stage = 0;
+  j->first_call = j->calls;
+  out->n_down = n;
+  out->down_key = j->hd[0].col[0];
+  out->down_window_id = (const int64_t*)j->hd[0].col[1];
+  out->down_handle[0] = j->hd[0].col[2];
+  out->down_handle[1] = j->hd[0].col[3];
+  out->down_handle[2] = j->hd[0].col[4];
+  out->down_handle[3] = j->hd[1].col[0];
+  out->down_mask = j->hd[1].col[1];
+  out->down_epoch = j->hd[1].col[2];
+  out->n_meta = nm;
+  out->meta_key = j->hm.col[0];
+  out->meta_window_id = (const int64_t*)j->hm.col[1];
+  out->meta_epoch = j->hm.col[2];
+  out->n_late = nl;
+  out->late_key = j->hl.col[0];
+  out->late_window_id = (const int64_t*)j->hl.col[1];
+  out->late_epoch = j->hl.col[2];
+  out->late_activation = j->hl.col[3];
+  out->late_row = j->hl.col[4];
+  // handed out until the next advance / eof, then cleared
+  j->released.swap(j->released_out);
+  j->released.clear();
+  out->n_released = j->released_out.size();
+  out->released = j->released_out.data();
+  return BW_OK;
+}
+
+// notify phase or EOF: wake the keys (K8's k_jwin_mark), then flush them (ordered: through the pool)
+static bw_status pjwin_wake(bw_pjwin* j, int eof) {
+  bw_ctx* ctx = j->ctx;
+  bw_status st = pjwin_drain(j);
+  if (st != BW_OK) return st;
+  if ((st = pjwin_room(j, 0)) != BW_OK) return st;
+  const JwParams p = pjwin_params(j, j->last_epoch);
+  k_jwin_mark<<<ctx->sm_count * 8, 256, 0, j->s>>>(j->t.j, j->t.win, p, eof);
+  CU(ctx, cudaGetLastError());
+  j->undrained = true;
+  return pjwin_flush(j, p, j->nq);
+}
+
+bw_status bw_pjwin_advance(bw_pjwin* j, int64_t system_now_us, bw_jwin_rows* out) {
+  if (!j || !out) return BW_ERR_SPEC;
+  bw_ctx* ctx = j->ctx;
+  PJWIN_REFUSE_FAILED(j);
+  CU(ctx, cudaSetDevice(ctx->device));
+  if (system_now_us > 0) {
+    if (system_now_us > j->now) j->now = system_now_us;
+    bw_status st = pjwin_wake(j, 0);
+    if (st != BW_OK) return st;
+  }
+  return pjwin_collect(j, out);
+}
+
+bw_status bw_pjwin_eof(bw_pjwin* j, bw_jwin_rows* out) {
+  if (!j || !out) return BW_ERR_SPEC;
+  bw_ctx* ctx = j->ctx;
+  PJWIN_REFUSE_FAILED(j);
+  CU(ctx, cudaSetDevice(ctx->device));
+  bw_status st = pjwin_wake(j, 1);
+  if (st != BW_OK) return st;
+  return pjwin_collect(j, out);
 }

@@ -495,6 +495,22 @@ class _GpuJoinWindowStep(_GpuWindowStep):
         return rows
 
 
+class _GpuProductJoinWindowStep(_GpuJoinWindowStep):
+    """One worker's ``join_window(insert_mode="product")`` over a tumbling or sliding windower (``GpuJoinWindowPlan``) on
+    ``bw_pjwin_*`` (K14).  Ingest, handles, clock sampling, notify, EOF, the key re-sort and the rows are the join step's;
+    each down row is one tuple of an emission's product, expanded on the device."""
+
+    def _make(self):
+        from bytewax_b200 import gpu
+
+        plan = self.plan
+        return gpu.ProductJoinWindow(
+            _get_gpu_ctx(), plan.emit_mode, plan.ordered, plan.sides, self.length_us, self.offset_us, self.align_us, self.wait_us,
+            capacity_hint=int(os.environ.get("BYTEWAX_B200_KEYS", 1 << 20)), max_windows_per_key=64,
+            max_queued_rows=1 << 22 if plan.ordered else 0, max_batch_rows=int(os.environ.get("BYTEWAX_B200_BATCH", 1 << 22)),
+            max_emit_rows=1 << 22, max_late_rows=1 << 22, max_product_rows=1 << 28)
+
+
 class _GpuSessionJoinWindowStep(_GpuJoinWindowStep):
     """One worker's ``join_window`` over a ``SessionWindower`` (``GpuJoinWindowPlan``) on ``bw_sjwin_*`` (K10):
     `_WindowLogic` over `_SessionWindowerLogic` with `_JoinWindowLogic` per session (windowing.py:671-810, 1046-1190,
@@ -803,6 +819,8 @@ def _gpu_step_for(step_id: str, plan):
                                                   GpuSessionCollectWindowPlan, SessionWindower)
 
     if isinstance(plan, GpuJoinWindowPlan):
+        if plan.insert_mode == "product":
+            return _GpuProductJoinWindowStep(step_id, plan)
         if isinstance(plan.windower, SessionWindower):
             return _GpuSessionJoinWindowStep(step_id, plan)
         return _GpuJoinWindowStep(step_id, plan)

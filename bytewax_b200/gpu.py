@@ -643,6 +643,31 @@ class JoinWindow(_HandleJoin):
                               arr(r.late_activation, nl), arr(r.late_row, nl), arr(r.released, nr))
 
 
+class ProductJoinWindow(JoinWindow):
+    """``join_window`` with insert mode product over tumbling or sliding windows (``bw_pjwin``, K14;
+    windowing.py:1046-1190, 1849-1902, ``_JoinState`` operators/__init__.py:2072-2120).  Each down row is one tuple of an
+    emission's ``itertools.product``, expanded on the device; values travel as uint64 handles, and each comes back in
+    ``released`` once no window list and no queue entry holds it."""
+
+    _PREFIX, _ROWS = "bw_pjwin", N.BwJwinRows
+
+    def __init__(self, ctx: Context, emit_mode: str = "final", ordered: bool = True, sides: int = 2, length_us: int = 10_000_000,
+                 offset_us: Optional[int] = None, align_us: int = 0, wait_us: Optional[int] = 0, capacity_hint: int = 1 << 16,
+                 max_windows_per_key: int = 16, max_queued_rows: int = 1 << 20, max_batch_rows: int = 1 << 20,
+                 max_emit_rows: int = 1 << 20, max_late_rows: int = 1 << 20, max_product_rows: int = 1 << 26):
+        """``offset_us=None``: tumbling.  ``wait_us=None``: the watermark never advances on data (``BW_WAIT_FOREVER``).
+        ``max_product_rows``: down rows one ``advance`` / ``eof`` may hand out."""
+        s = N.BwPjwinSpec()
+        s.struct_size = C.sizeof(N.BwPjwinSpec)
+        s.emit_mode = self.EMIT.get(emit_mode, -1)
+        s.ordered, s.sides, s.max_windows_per_key = int(ordered), sides, max_windows_per_key
+        s.length_us, s.offset_us, s.align_us = length_us, length_us if offset_us is None else offset_us, align_us
+        s.wait_us = N.BW_WAIT_FOREVER if wait_us is None else wait_us
+        s.capacity_hint, s.max_queued_rows, s.max_batch_rows = capacity_hint, max_queued_rows, max_batch_rows
+        s.max_emit_rows, s.max_late_rows, s.max_product_rows = max_emit_rows, max_late_rows, max_product_rows
+        self._create(ctx, s, sides)
+
+
 @dataclass
 class SessionJoinWindowRows(JoinWindowRows):
     """Rows of one ``SessionJoinWindow.advance`` / ``eof``: the join's streams, with each meta row's session bounds and

@@ -887,9 +887,10 @@ def join_window(step_id: str, clock: Clock, windower: Windower, *sides: KeyedStr
 
 @dataclass(frozen=True)
 class GpuJoinWindowPlan:
-    """A ``join_window`` the engine may run with ``bw_jwin_*`` (K8, tumbling or sliding windower) or ``bw_sjwin_*`` (K10,
-    `SessionWindower`): insert mode first / last, 1 to 4 sides, and an `EventClock` with an identity ``to_system_utc`` or a
-    `SystemClock`.  Values travel as handles into a host-side dict, so they can be any Python object."""
+    """A ``join_window`` the engine may run on the device: insert mode first / last with ``bw_jwin_*`` (K8, tumbling or
+    sliding windower) or ``bw_sjwin_*`` (K10, `SessionWindower`), insert mode product with ``bw_pjwin_*`` (K14, tumbling or
+    sliding windower only); 1 to 4 sides, and an `EventClock` with an identity ``to_system_utc`` or a `SystemClock`.
+    Values travel as handles into a host-side dict, so they can be any Python object."""
 
     insert_mode: str
     emit_mode: str
@@ -900,11 +901,13 @@ class GpuJoinWindowPlan:
 
 
 def _join_window_plan(clock, windower, side_count, insert_mode, emit_mode, ordered) -> Optional[GpuJoinWindowPlan]:
-    # product keeps lists per side: host engine.  A custom `to_system_utc` moves the notify time away from the event
-    # time the device compares with the system clock (windowing.py:1177-1178): host engine.
-    if insert_mode not in ("first", "last") or not 1 <= side_count <= 4:
+    # product over sessions stays on the host engine: a merge concatenates the side lists (`self.state += original.state`).
+    # A custom `to_system_utc` moves the notify time away from the event time the device compares with the system clock
+    # (windowing.py:1177-1178): host engine.
+    if insert_mode not in ("first", "last", "product") or not 1 <= side_count <= 4:
         return None
-    if not isinstance(windower, (SlidingWindower, TumblingWindower, SessionWindower)):
+    windowers = (SlidingWindower, TumblingWindower) if insert_mode == "product" else (SlidingWindower, TumblingWindower, SessionWindower)
+    if not isinstance(windower, windowers):
         return None
     if not (isinstance(clock, SystemClock) or (isinstance(clock, EventClock) and clock.to_system_utc is _identity)):
         return None

@@ -341,7 +341,8 @@ bw_status bw_smap_sync(bw_smap* m);
 
 /* Two-sided keyed join: `_JoinLogic.on_item` / `on_eof` (operators/__init__.py:2157-2190) over the
  * side-labelled merged stream of `_join_label_merge` (:2193-2204); insert modes first / last,
- * emit modes complete / final / running (`product` keeps lists per side: host path only). */
+ * emit modes complete / final / running (`product` keeps lists per side: host path only; windowed product joins:
+ * bw_pjwin_*, K14). */
 typedef enum { BW_JOIN_INSERT_FIRST = 0, BW_JOIN_INSERT_LAST = 1 } bw_join_insert;
 typedef enum { BW_JOIN_EMIT_COMPLETE = 0, BW_JOIN_EMIT_FINAL = 1, BW_JOIN_EMIT_RUNNING = 2 } bw_join_emit_mode;
 typedef struct bw_join bw_join;
@@ -455,7 +456,7 @@ bw_status bw_session_eof(bw_session* s, bw_session_rows* out);
 typedef struct bw_jwin bw_jwin;
 typedef struct bw_jwin_spec {
   uint32_t struct_size;
-  int32_t insert_mode;          /* BW_JOIN_INSERT_FIRST / LAST (product keeps lists per side: host engine) */
+  int32_t insert_mode;          /* BW_JOIN_INSERT_FIRST / LAST (product: bw_pjwin_*, K14) */
   int32_t emit_mode;            /* BW_JOIN_EMIT_COMPLETE / FINAL / RUNNING */
   int32_t ordered;              /* 1: play values in timestamp order once the watermark passes them (the default) */
   int32_t sides;                /* 1..4 joined streams */
@@ -512,6 +513,50 @@ bw_status bw_jwin_apply_device(bw_jwin* j, const uint64_t* d_keys, const uint8_t
 bw_status bw_jwin_advance(bw_jwin* j, int64_t system_now_us, bw_jwin_rows* out);
 /* End of input: every key flushes at watermark UTC_MAX (:1144-1151). */
 bw_status bw_jwin_eof(bw_jwin* j, bw_jwin_rows* out);
+
+/* Windowed product join (K14): `join_window(insert_mode="product")` over tumbling and sliding windows -- K8's steps
+ * (late test, queue, ordered play, `open_for` in ascending id, close in first-opened order, notify, EOF at UTC_MAX,
+ * discard of an empty key) with `_JoinState` keeping one list per side (operators/__init__.py:2072-2120): a value is
+ * appended to its side's list in every window of `open_for(ts)`; "complete" emits the product once every side is
+ * non-empty and then clears every list (the lists refill within the window; a cleared window emits nothing at close);
+ * "running" emits the product after every value; "final" at the close.  A product is `itertools.product` of the lists,
+ * the last side varying fastest, each list in play order, an empty list giving one None: one `down` row per tuple, so
+ * an emission whose lists hold n_0 .. n_{sides-1} values gives prod max(1, n_s) rows.  The rows are expanded on the
+ * device at advance / eof.  One GPU only. */
+typedef struct bw_pjwin bw_pjwin;
+typedef struct bw_pjwin_spec {
+  uint32_t struct_size;
+  int32_t emit_mode;            /* BW_JOIN_EMIT_COMPLETE / FINAL / RUNNING */
+  int32_t ordered;              /* 1: play values in timestamp order once the watermark passes them (the default) */
+  int32_t sides;                /* 1..4 joined streams */
+  int32_t max_windows_per_key;  /* 1..64 open windows per key */
+  int64_t length_us;            /* window length, > 0 */
+  int64_t offset_us;            /* 0 < offset <= length (TumblingWindower: == length) */
+  int64_t align_us;             /* align_to */
+  int64_t wait_us;              /* EventClock.wait_for_system_duration, or BW_WAIT_FOREVER */
+  uint64_t capacity_hint;       /* live keys; a key's slot is kept once seen */
+  uint64_t max_queued_rows;     /* ordered mode: queued entries over ALL keys */
+  uint64_t max_batch_rows;
+  uint64_t max_emit_rows;       /* < 2^31: emissions (each one product), and meta rows, retained between advances */
+  uint64_t max_late_rows;       /* late rows retained between bw_pjwin_advance calls */
+  uint64_t max_product_rows;    /* down rows one advance / eof may hand out (the sum of the emissions' products) */
+} bw_pjwin_spec;
+bw_status bw_pjwin_create(bw_ctx* ctx, const bw_pjwin_spec* spec, bw_pjwin** out);
+void bw_pjwin_destroy(bw_pjwin* j);
+/* One activation from HOST columns (keys, side 0..sides-1, handle, ts); blocks.  `system_now_us` as bw_jwin_apply. */
+bw_status bw_pjwin_apply(bw_pjwin* j, const uint64_t* keys, const uint8_t* side, const uint64_t* handles, const int64_t* ts_us,
+                         uint64_t rows, uint64_t epoch, int64_t system_now_us);
+/* Same with DEVICE columns; returns once the work is enqueued (the columns must stay valid until the next call).  A side
+ * value >= sides is not played: the next call returns BW_ERR_SPEC and the join refuses further calls. */
+bw_status bw_pjwin_apply_device(bw_pjwin* j, const uint64_t* d_keys, const uint8_t* d_side, const uint64_t* d_handles,
+                                const int64_t* d_ts_us, uint64_t rows, uint64_t epoch, int64_t system_now_us);
+/* Rows since the last call, as bw_jwin_advance: `down` rows are the product tuples, each emission's rows in product
+ * order (down_mask bit s is set iff side s's list was non-empty).  More than max_product_rows rows fails with
+ * BW_ERR_CAPACITY and the join refuses further calls.  Each handle is released once, in the call after which no window
+ * list and no queue entry holds it. */
+bw_status bw_pjwin_advance(bw_pjwin* j, int64_t system_now_us, bw_jwin_rows* out);
+/* End of input: every key flushes at watermark UTC_MAX. */
+bw_status bw_pjwin_eof(bw_pjwin* j, bw_jwin_rows* out);
 
 /* Windowed collect (K9): `collect_window` (pysrc/bytewax/operators/windowing.py:1436-1576) into list / set / dict,
  * i.e. `_WindowLogic` (:1046-1190) over `_SlidingWindowerLogic` (:603-668; tumbling == offset equal to length,
@@ -603,7 +648,8 @@ bw_status bw_collect_eof(bw_collect* c, bw_collect_rows* out);
 typedef struct bw_sjwin bw_sjwin;
 typedef struct bw_sjwin_spec {
   uint32_t struct_size;
-  int32_t insert_mode;          /* BW_JOIN_INSERT_FIRST / LAST (product keeps lists per side: host engine) */
+  int32_t insert_mode;          /* BW_JOIN_INSERT_FIRST / LAST (product over sessions: host engine; over tumbling and
+                                   sliding windows: bw_pjwin_*, K14) */
   int32_t emit_mode;            /* BW_JOIN_EMIT_COMPLETE / FINAL / RUNNING */
   int32_t ordered;              /* 1: play values in timestamp order once the watermark passes them (the default) */
   int32_t sides;                /* 1..4 joined streams */
