@@ -207,6 +207,18 @@ class BwKcollectRows(C.Structure):
                 ("offset", C.POINTER(C.c_uint64)), ("handle", C.POINTER(C.c_uint64))]
 
 
+class BwKjoinSpec(C.Structure):
+    _fields_ = [("struct_size", C.c_uint32), ("insert_mode", C.c_int32), ("emit_mode", C.c_int32), ("sides", C.c_int32),
+                ("capacity_hint", C.c_uint64), ("max_batch_rows", C.c_uint64), ("max_emit_rows", C.c_uint64),
+                ("max_product_rows", C.c_uint64)]
+
+
+class BwKjoinRows(C.Structure):
+    _fields_ = [("n", C.c_uint64), ("key", C.POINTER(C.c_uint64)), ("handle", C.POINTER(C.c_uint64) * 4),
+                ("mask", C.POINTER(C.c_uint64)), ("epoch", C.POINTER(C.c_uint64)), ("n_released", C.c_uint64),
+                ("released", C.POINTER(C.c_uint64))]
+
+
 # every symbol include/bwgpu.h declares: (restype, argtypes)
 _P = C.c_void_p
 SYMBOLS = {
@@ -296,6 +308,12 @@ SYMBOLS = {
     "bw_pjwin_apply_device": (C.c_int32, [_P, _P, _P, _P, _P, C.c_uint64, C.c_uint64, C.c_int64]),
     "bw_pjwin_advance": (C.c_int32, [_P, C.c_int64, C.POINTER(BwJwinRows)]),
     "bw_pjwin_eof": (C.c_int32, [_P, C.POINTER(BwJwinRows)]),
+    "bw_kjoin_create": (C.c_int32, [_P, C.POINTER(BwKjoinSpec), C.POINTER(_P)]),
+    "bw_kjoin_destroy": (None, [_P]),
+    "bw_kjoin_apply": (C.c_int32, [_P, _P, _P, _P, C.c_uint64, C.c_uint64]),
+    "bw_kjoin_apply_device": (C.c_int32, [_P, _P, _P, _P, C.c_uint64, C.c_uint64]),
+    "bw_kjoin_advance": (C.c_int32, [_P, C.POINTER(BwKjoinRows)]),
+    "bw_kjoin_eof": (C.c_int32, [_P, C.POINTER(BwKjoinRows)]),
     "bw_dev_alloc": (C.c_int32, [_P, C.c_uint64, C.POINTER(_P)]),
     "bw_dev_free": (C.c_int32, [_P, _P]),
     "bw_host_alloc": (C.c_int32, [_P, C.c_uint64, C.POINTER(_P)]),

@@ -42,6 +42,7 @@
 #include "bw_argwin.cuh"
 #include "bw_kcollect.cuh"
 #include "bw_pjwin.cuh"
+#include "bw_kjoin.cuh"
 #include "bw_prepass.cuh"
 #include "bw_slow.cuh"
 #include "bw_late.cuh"
@@ -3486,9 +3487,15 @@ static cudaError_t collect_grow_keep(J* j, T** p, u64 used, u64 grow) {
   return cudaSuccess;
 }
 
+// emit buffers whose staging buffer has a record column (K9, K12, K13; K15 stages by rank ranges and has none)
+template <class E, class = void>
+struct HasStageRec : std::false_type {};
+template <class E>
+struct HasStageRec<E, std::void_t<decltype(&E::stage_rec)>> : std::true_type {};
+
 // Before a call that can add `adds` entries to the store: compact the store once dead entries outnumber live ones, then
 // grow the store and the staging buffer so that nothing the call can add or stage overflows them.  Called after the
-// drain: nothing on the stream reads them.  (J: bw_collect, bw_scwin, bw_kcollect)
+// drain: nothing on the stream reads them.  (J: bw_collect, bw_scwin, bw_kcollect, bw_kjoin)
 template <class J>
 static bw_status store_room(J* j, u64 adds) {
   bw_ctx* ctx = j->ctx;
@@ -3524,7 +3531,7 @@ static bw_status store_room(J* j, u64 adds) {
     const u64 grow = std::max<u64>(j->n_stage + live + adds, 2 * e.max_stage);
     e.max_stage = 0;
     CU(ctx, collect_grow_keep(j, &e.stage, j->n_stage, grow));
-    CU(ctx, collect_grow_keep(j, &e.stage_rec, j->n_stage, grow));
+    if constexpr (HasStageRec<std::decay_t<decltype(e)>>::value) CU(ctx, collect_grow_keep(j, &e.stage_rec, j->n_stage, grow));
     e.max_stage = grow;
   }
   return BW_OK;
@@ -5390,4 +5397,335 @@ bw_status bw_pjwin_eof(bw_pjwin* j, bw_jwin_rows* out) {
   bw_status st = pjwin_wake(j, 1);
   if (st != BW_OK) return st;
   return pjwin_collect(j, out);
+}
+
+// ===========================================================================
+// K15 host side: keyed join (bw_kjoin.cuh)
+// ===========================================================================
+struct bw_kjoin {
+  Owner own;  // every buffer and the stream below
+  bw_ctx* ctx = nullptr;
+  bw_kjoin_spec spec{};
+  KjTable t{};
+  CwStore es{};
+  KeyedScratch k;
+  cudaStream_t s = nullptr;
+  u32* h_err = nullptr;  // err, why
+  // events, released, stage records, staged, store entries, dead entries, killed entries
+  unsigned long long* d_cnt = nullptr;
+  unsigned long long* h_cnt = nullptr;
+  unsigned char *d_side = nullptr, *d_flag = nullptr;
+  u64* d_handles = nullptr;
+  KjEmit e{};
+  u64 n_store = 0, dead = 0;   // entries in the store, and how many of them are dead
+  u64 n_rec = 0, n_stage = 0;  // stage records and staged handles since the last advance / eof
+  SortScratch srt;             // ordering and compaction scratch
+  PjOrdered o{};               // advance / eof: the events in the reference's order
+  u64* d_off = nullptr;        // the exclusive scan of their row counts
+  u64* d_zero = nullptr;       // the window-id column K14's count kernel reads: zeros
+  PjRows rows{};               // the expanded rows (its window-id column is not copied out)
+  u64 rows_cap = 0;
+  HostCols hd[2];              // key, h0, h1, h2, h3 | mask, epoch
+  std::vector<u64> released;      // since the last advance / eof
+  std::vector<u64> released_out;  // what the last advance / eof handed out
+  bool undrained = false;         // a call whose counts are not read back yet
+  u64 outstanding = 0;            // handles passed in and not released yet: what the next call can release, besides its own
+  u32 batch_no = 0;
+  u64 calls = 0, first_call = 0;  // calls (activations, EOF) so far; the first not yet collected
+  u64 last_epoch = 0;
+  bool failed = false;
+};
+
+bw_status bw_kjoin_create(bw_ctx* ctx, const bw_kjoin_spec* spec, bw_kjoin** out) {
+  if (!ctx || !spec || !out) CTX_FAIL(ctx, BW_ERR_SPEC, "bw_kjoin_create: NULL argument");
+  if (spec->struct_size != sizeof(bw_kjoin_spec)) CTX_FAIL(ctx, BW_ERR_SPEC, "bw_kjoin_spec.struct_size mismatch");
+  if (ctx->world != 1) CTX_FAIL(ctx, BW_ERR_SPEC, "keyed joins run on one GPU (world == 1)");
+  if (spec->insert_mode < BW_JOIN_INSERT_FIRST || spec->insert_mode > BW_JOIN_INSERT_PRODUCT) CTX_FAIL(ctx, BW_ERR_SPEC, "bad insert_mode");
+  if (spec->emit_mode < BW_JOIN_EMIT_COMPLETE || spec->emit_mode > BW_JOIN_EMIT_RUNNING) CTX_FAIL(ctx, BW_ERR_SPEC, "bad emit_mode");
+  if (spec->sides < 1 || spec->sides > BW_JW_MAXSIDES) CTX_FAIL(ctx, BW_ERR_SPEC, "sides must be in 1..%d", BW_JW_MAXSIDES);
+  if (spec->max_batch_rows == 0 || spec->max_batch_rows >= (1ULL << 31)) CTX_FAIL(ctx, BW_ERR_SPEC, "bad max_batch_rows");
+  if (spec->max_emit_rows >= (1ULL << 31)) CTX_FAIL(ctx, BW_ERR_SPEC, "max_emit_rows must be below 2^31");
+  if (spec->capacity_hint >= (1ULL << 30)) CTX_FAIL(ctx, BW_ERR_SPEC, "capacity_hint must be below 2^30");
+  CU(ctx, cudaSetDevice(ctx->device));
+  std::unique_ptr<bw_kjoin, void (*)(bw_kjoin*)> jp(new bw_kjoin(), bw_kjoin_destroy);  // torn down on every failure
+  bw_kjoin* j = jp.get();
+  Owner& own = j->own;
+  j->ctx = ctx;
+  j->spec = *spec;
+  const u64 cap = std::max<u64>(1024, 2 * std::max<u64>(spec->capacity_hint, 1));
+  KjTable& t = j->t;
+  t.cap = cap;
+  t.sides = spec->sides;
+  t.insert_mode = spec->insert_mode;
+  t.emit_mode = spec->emit_mode;
+  CU(ctx, own.stream(&j->s));
+  CU(ctx, own.dev(&t.keys, cap + 1));
+  CU(ctx, own.dev(&t.cell, cap + 1));
+  CU(ctx, own.dev(&t.live, cap + 1));
+  CU(ctx, own.dev(&t.rec_ord, cap + 1));
+  CU(ctx, own.dev(&t.rec_c, cap + 1));
+  CU(ctx, own.dev(&t.err, 2));
+  t.why = t.err + 1;
+  CU(ctx, own.dev(&j->d_cnt, 7));
+  CU(ctx, cudaMemsetAsync(t.err, 0, 8, j->s));
+  CU(ctx, cudaMemsetAsync(j->d_cnt, 0, 56, j->s));
+  CU(ctx, own.host(&j->h_err, 64 / sizeof(u32)));
+  CU(ctx, own.host(&j->h_cnt, 16));
+  const u64 n = spec->max_batch_rows, m = std::max<u64>(spec->max_emit_rows, 1);
+  bw_status st = keyed_alloc(ctx, own, j->k, n, j->s);
+  if (st != BW_OK) return st;
+  CU(ctx, own.dev(&j->d_side, n));
+  CU(ctx, own.dev(&j->d_handles, n));
+  KjEmit& e = j->e;
+  for (u64** c : {&e.key, &e.epoch, &e.ord, &e.seq, &e.rec}) CU(ctx, own.dev(c, m));
+  for (u32** c : {&e.lo, &e.hi, &e.rb, &e.rn}) CU(ctx, own.dev(c, 4 * m));
+  CU(ctx, own.dev(&e.rbase, 4 * m));
+  PjOrdered& o = j->o;
+  for (u64** c : {&o.cnt, &o.key, &o.wid, &o.epoch}) CU(ctx, own.dev(c, m + 1));
+  CU(ctx, own.dev(&o.base, 4 * m));
+  CU(ctx, own.dev(&o.len, 4 * m));
+  CU(ctx, own.dev(&j->d_off, m + 1));
+  CU(ctx, own.dev(&j->d_zero, m));
+  CU(ctx, cudaMemsetAsync(j->d_zero, 0, m * 8, j->s));
+  // the store, the staging buffer, the release buffer and the output grow with what the join holds and emits
+  // (store_room, jwin_room, kjoin_expand); they start at one batch
+  CwStore& es = j->es;
+  es.cap = n;
+  CU(ctx, own.dev(&es.ref, n));
+  CU(ctx, own.dev(&es.rank, n));
+  CU(ctx, own.dev(&es.h, n));
+  CU(ctx, own.dev(&j->d_flag, n));
+  e.max_stage = n;
+  CU(ctx, own.dev(&e.stage, n));
+  e.max_rel = n;
+  CU(ctx, own.dev(&e.rel, e.max_rel));
+  e.max_rows = spec->max_emit_rows;
+  e.n_rows = j->d_cnt;
+  e.n_rel = j->d_cnt + 1;
+  e.n_rec = j->d_cnt + 2;
+  e.n_stage = j->d_cnt + 3;
+  es.n = j->d_cnt + 4;
+  e.n_kill = j->d_cnt + 6;
+  CU(ctx, j->srt.reserve(own, m, m, j->s));
+  size_t b = 0;
+  CU(ctx, cub::DeviceScan::ExclusiveScan(nullptr, b, o.cnt, j->d_off, PjSatAdd{}, (u64)0, (int)(m + 1), j->s));
+  CU(ctx, j->srt.grow_cub(own, b + 256));
+  k_kjoin_init<<<ctx->sm_count * 4, 256, 0, j->s>>>(t);
+  CU(ctx, cudaGetLastError());
+  CU(ctx, cudaStreamSynchronize(j->s));
+  *out = jp.release();
+  return BW_OK;
+}
+
+void bw_kjoin_destroy(bw_kjoin* j) {
+  if (!j) return;
+  cudaSetDevice(j->ctx->device);
+  if (j->s) cudaStreamSynchronize(j->s);
+  delete j;  // j->own releases every buffer and the stream
+}
+
+static KjParams kjoin_params(bw_kjoin* j, u64 epoch, int eof) {
+  KjParams p;
+  p.epoch = epoch;
+  p.ord = j->calls++;
+  p.eof = eof;
+  return p;
+}
+
+#define KJOIN_REFUSE_FAILED(j) \
+  if ((j)->failed) CTX_FAIL((j)->ctx, BW_ERR_STATE, "keyed join: an earlier call failed on the device; the join is unusable")
+
+// wait for the last call; fail on a device-side overflow or a bad side; then take its released handles and its counts,
+// so the device buffer only ever holds one call's releases
+static bw_status kjoin_drain(bw_kjoin* j) {
+  bw_ctx* ctx = j->ctx;
+  KJOIN_REFUSE_FAILED(j);
+  if (!j->undrained) return BW_OK;
+  CU(ctx, cudaMemcpyAsync(j->h_err, j->t.err, 8, cudaMemcpyDeviceToHost, j->s));
+  CU(ctx, cudaMemcpyAsync(j->h_cnt, j->d_cnt, 56, cudaMemcpyDeviceToHost, j->s));
+  CU(ctx, cudaStreamSynchronize(j->s));
+  if (j->h_err[0]) {
+    j->failed = true;
+    const u32 w = j->h_err[1];
+    CTX_FAIL(ctx, (bw_status)j->h_err[0], "keyed join kernel %s:%s%s%s%s%s%s",
+             j->h_err[0] == BW_ERR_SPEC ? "rejected its input" : "ran out of capacity",
+             w & BW_JW_BAD_SIDE ? " a side column value is not below sides;" : "", w & BW_JW_FULL_TABLE ? " key table full (raise capacity_hint);" : "",
+             w & BW_JW_FULL_EMIT ? " more than max_emit_rows emissions since the last advance;" : "",
+             w & BW_CW_FULL_STORE ? " entry store or staging buffer full;" : "",
+             w & BW_PJ_FULL_SIDE ? " a key's side list reached 2^32 values;" : "", w ? "" : " (no reason recorded)");
+  }
+  const u64 nr = j->h_cnt[1];
+  j->outstanding -= std::min(nr, j->outstanding);
+  if (nr) {
+    const size_t at = j->released.size();
+    j->released.resize(at + nr);
+    CU(ctx, cudaMemcpyAsync(j->released.data() + at, j->e.rel, nr * 8, cudaMemcpyDeviceToHost, j->s));
+  }
+  j->n_rec = j->h_cnt[2];
+  j->n_stage = j->h_cnt[3];
+  j->n_store = j->h_cnt[4];
+  j->dead += j->h_cnt[5];
+  CU(ctx, cudaMemsetAsync(j->d_cnt + 5, 0, 16, j->s));
+  CU(ctx, cudaMemsetAsync(j->d_cnt + 1, 0, 8, j->s));
+  CU(ctx, cudaStreamSynchronize(j->s));
+  j->undrained = false;
+  return BW_OK;
+}
+
+// after the per-key kernel of a call: stage the emitting keys' lists, kill dead entries, release (k_kjoin_gather)
+static bw_status kjoin_gather(bw_kjoin* j, const KjParams& p) {
+  k_kjoin_gather<<<j->ctx->sm_count * 8, 256, 0, j->s>>>(j->t, j->e, j->es, p, j->n_rec, j->d_cnt + 5);
+  CU(j->ctx, cudaGetLastError());
+  return BW_OK;
+}
+
+bw_status bw_kjoin_apply_device(bw_kjoin* j, const uint64_t* d_keys, const uint8_t* d_side, const uint64_t* d_handles, uint64_t rows,
+                                uint64_t epoch) {
+  if (!j) return BW_ERR_SPEC;
+  bw_ctx* ctx = j->ctx;
+  KJOIN_REFUSE_FAILED(j);
+  if (rows > j->spec.max_batch_rows) CTX_FAIL(ctx, BW_ERR_SPEC, "keyed join: rows > max_batch_rows");
+  if (rows && (!d_keys || !d_side || !d_handles)) CTX_FAIL(ctx, BW_ERR_SPEC, "keyed join: NULL column");
+  if (j->batch_no && epoch < j->last_epoch) CTX_FAIL(ctx, BW_ERR_STATE, "keyed join: epochs must not decrease");
+  CU(ctx, cudaSetDevice(ctx->device));
+  bw_status st = kjoin_drain(j);
+  if (st != BW_OK) return st;
+  j->last_epoch = epoch;
+  const KjParams p = kjoin_params(j, epoch, 0);
+  j->batch_no++;
+  if (rows == 0) return BW_OK;
+  if ((st = jwin_room(j, rows)) != BW_OK) return st;
+  if ((st = store_room(j, rows)) != BW_OK) return st;  // (a value adds at most one entry)
+  j->outstanding += rows;
+  st = keyed_group(ctx, j->k, d_keys, rows, j->s);
+  if (st != BW_OK) return st;
+  k_kjoin_apply<<<ctx->sm_count * 8, 256, 0, j->s>>>(j->t, j->e, j->es, p, j->k.d_ksorted, j->k.d_isorted, j->k.d_head, d_handles, d_side,
+                                                     rows);
+  CU(ctx, cudaGetLastError());
+  j->undrained = true;
+  return kjoin_gather(j, p);
+}
+
+bw_status bw_kjoin_apply(bw_kjoin* j, const uint64_t* keys, const uint8_t* side, const uint64_t* handles, uint64_t rows, uint64_t epoch) {
+  if (!j) return BW_ERR_SPEC;
+  bw_ctx* ctx = j->ctx;
+  KJOIN_REFUSE_FAILED(j);
+  if (rows > j->spec.max_batch_rows) CTX_FAIL(ctx, BW_ERR_SPEC, "keyed join: rows > max_batch_rows");
+  if (rows && (!keys || !side || !handles)) CTX_FAIL(ctx, BW_ERR_SPEC, "keyed join: NULL column");
+  for (u64 i = 0; i < rows; ++i)
+    if (side[i] >= (u32)j->spec.sides)
+      CTX_FAIL(ctx, BW_ERR_SPEC, "keyed join: side %u of row %llu is not below sides", side[i], (unsigned long long)i);
+  CU(ctx, cudaSetDevice(ctx->device));
+  bw_status st = kjoin_drain(j);
+  if (st != BW_OK) return st;
+  if (rows) {
+    CU(ctx, cudaMemcpyAsync(j->k.d_keys, keys, rows * 8, cudaMemcpyHostToDevice, j->s));
+    CU(ctx, cudaMemcpyAsync(j->d_side, side, rows, cudaMemcpyHostToDevice, j->s));
+    CU(ctx, cudaMemcpyAsync(j->d_handles, handles, rows * 8, cudaMemcpyHostToDevice, j->s));
+  }
+  st = bw_kjoin_apply_device(j, j->k.d_keys, j->d_side, j->d_handles, rows, epoch);
+  if (st != BW_OK) return st;
+  // the host columns may be reused by the caller once this returns
+  return kjoin_drain(j);
+}
+
+// advance / eof: the events in the reference's order (order_perm), their row counts and the saturating scan of them
+// (K14's k_pjwin_count, over a zero window-id column); the host grows the output to the total; K14's k_pjwin_expand
+// writes every row in that order
+static bw_status kjoin_expand(bw_kjoin* j, u64 nd, u64* total) {
+  bw_ctx* ctx = j->ctx;
+  *total = 0;
+  if (!nd) return BW_OK;
+  SortScratch& x = j->srt;
+  const KjEmit& e = j->e;
+  bw_status st = order_perm(ctx, x, j->s, nd, e.key, e.seq, e.ord, nullptr, std::max<u64>(j->calls - j->first_call, 1), j->first_call,
+                            nullptr);
+  if (st != BW_OK) return st;
+  PjEmit v{};  // the event columns as K14 lays them out
+  v.key = e.key;
+  v.wid = j->d_zero;
+  v.epoch = e.epoch;
+  v.rec = e.rec;
+  v.lo = e.lo;
+  v.hi = e.hi;
+  v.rb = e.rb;
+  v.rn = e.rn;
+  v.rbase = e.rbase;
+  const PjOrdered o = j->o;
+  k_pjwin_count<<<ctx->sm_count * 4, 256, 0, j->s>>>(v, o, j->spec.sides, x.perm, nd);
+  CU(ctx, cudaMemsetAsync(o.cnt + nd, 0, 8, j->s));
+  size_t tb = x.cub_bytes;
+  CU(ctx, cub::DeviceScan::ExclusiveScan(x.cub, tb, o.cnt, j->d_off, PjSatAdd{}, (u64)0, (int)(nd + 1), j->s));
+  CU(ctx, cudaMemcpyAsync(j->h_cnt + 8, j->d_off + nd, 8, cudaMemcpyDeviceToHost, j->s));
+  CU(ctx, cudaStreamSynchronize(j->s));
+  const u64 n = j->h_cnt[8];
+  if (n > j->spec.max_product_rows) {
+    j->failed = true;
+    CTX_FAIL(ctx, BW_ERR_CAPACITY, "keyed join ran out of capacity: %llu product rows since the last advance, more than max_product_rows "
+             "(%llu)", (unsigned long long)n, (unsigned long long)j->spec.max_product_rows);
+  }
+  if (n > j->rows_cap) {
+    j->rows_cap = 0;
+    for (u64** c : {&j->rows.key, &j->rows.wid, &j->rows.h0, &j->rows.h1, &j->rows.h2, &j->rows.h3, &j->rows.mask, &j->rows.epoch})
+      CU(ctx, j->own.regrow(Owner::DEV, c, n));
+    j->rows_cap = n;
+  }
+  CU(ctx, j->hd[0].reserve(j->own, n, n));
+  CU(ctx, j->hd[1].reserve(j->own, n, n));
+  k_pjwin_expand<<<ctx->sm_count * 8, 256, 0, j->s>>>(o, j->d_off, nd, j->spec.sides, e.stage, j->rows, n);
+  const u64* src[] = {j->rows.key, j->rows.h0, j->rows.h1, j->rows.h2, j->rows.h3, j->rows.mask, j->rows.epoch};
+  for (int c = 0; c < 7; ++c) CU(ctx, cudaMemcpyAsync(j->hd[c / 5].col[c % 5], src[c], n * 8, cudaMemcpyDeviceToHost, j->s));
+  *total = n;
+  return BW_OK;
+}
+
+static bw_status kjoin_collect(bw_kjoin* j, bw_kjoin_rows* out) {
+  bw_ctx* ctx = j->ctx;
+  bw_status st = kjoin_drain(j);
+  if (st != BW_OK) return st;
+  CU(ctx, cudaMemcpyAsync(j->h_cnt, j->d_cnt, 8, cudaMemcpyDeviceToHost, j->s));
+  CU(ctx, cudaStreamSynchronize(j->s));
+  const u64 nd = j->h_cnt[0];  // within bounds: kjoin_drain passed
+  u64 n = 0;
+  if ((st = kjoin_expand(j, nd, &n)) != BW_OK) return st;
+  CU(ctx, cudaGetLastError());
+  CU(ctx, cudaMemsetAsync(j->d_cnt, 0, 8, j->s));
+  CU(ctx, cudaMemsetAsync(j->d_cnt + 2, 0, 16, j->s));
+  CU(ctx, cudaStreamSynchronize(j->s));
+  j->n_rec = j->n_stage = 0;
+  j->first_call = j->calls;
+  out->n = n;
+  out->key = j->hd[0].col[0];
+  for (int s = 0; s < 4; ++s) out->handle[s] = j->hd[0].col[1 + s];
+  out->mask = j->hd[1].col[0];
+  out->epoch = j->hd[1].col[1];
+  // handed out until the next advance / eof, then cleared
+  j->released.swap(j->released_out);
+  j->released.clear();
+  out->n_released = j->released_out.size();
+  out->released = j->released_out.data();
+  return BW_OK;
+}
+
+bw_status bw_kjoin_advance(bw_kjoin* j, bw_kjoin_rows* out) {
+  if (!j || !out) return BW_ERR_SPEC;
+  KJOIN_REFUSE_FAILED(j);
+  CU(j->ctx, cudaSetDevice(j->ctx->device));
+  return kjoin_collect(j, out);
+}
+
+bw_status bw_kjoin_eof(bw_kjoin* j, bw_kjoin_rows* out) {
+  if (!j || !out) return BW_ERR_SPEC;
+  bw_ctx* ctx = j->ctx;
+  KJOIN_REFUSE_FAILED(j);
+  CU(ctx, cudaSetDevice(ctx->device));
+  bw_status st = kjoin_drain(j);
+  if (st != BW_OK) return st;
+  if ((st = store_room(j, 0)) != BW_OK) return st;  // (staging for every entry held)
+  const KjParams p = kjoin_params(j, j->last_epoch, 1);
+  k_kjoin_eof<<<ctx->sm_count * 8, 256, 0, j->s>>>(j->t, j->e, p);
+  CU(ctx, cudaGetLastError());
+  j->undrained = true;
+  if ((st = kjoin_gather(j, p)) != BW_OK) return st;
+  return kjoin_collect(j, out);
 }

@@ -814,7 +814,7 @@ def _td_us(td: timedelta) -> int:
 
 
 def _gpu_step_for(step_id: str, plan):
-    from bytewax_b200.operators import GpuCollectPlan, GpuFinalPlan, GpuJoinPlan, GpuSmapPlan
+    from bytewax_b200.operators import GpuCollectPlan, GpuFinalPlan, GpuJoinPlan, GpuKeyJoinPlan, GpuSmapPlan
     from bytewax_b200.operators.windowing import (GpuArgWindowPlan, GpuCollectWindowPlan, GpuJoinWindowPlan,
                                                   GpuSessionCollectWindowPlan, SessionWindower)
 
@@ -836,6 +836,8 @@ def _gpu_step_for(step_id: str, plan):
         return _GpuSmapStep(step_id, plan)
     if isinstance(plan, GpuJoinPlan):
         return _GpuJoinStep(step_id, plan)
+    if isinstance(plan, GpuKeyJoinPlan):
+        return _GpuKeyJoinStep(step_id, plan)
     if isinstance(plan, GpuCollectPlan):
         return _GpuCollectStep(step_id, plan)
     return _GpuFinalStep(step_id, plan) if isinstance(plan, GpuFinalPlan) else _GpuWindowStep(step_id, plan)
@@ -1070,6 +1072,60 @@ class _GpuCollectStep(_GpuJoinWindowStep):
         rows = [(self._key_str(k), [V.pop(h) for h in hs]) for k, hs in zip(out.key.tolist(), out.lists())]
         if self.resort:  # interned (non-numeric) keys: restore ascending key-string order; stable
             rows.sort(key=lambda r: r[0])
+        return rows
+
+
+class _GpuKeyJoinStep(_NoClock, _GpuJoinWindowStep):
+    """One worker's ``join`` (``GpuKeyJoinPlan``: product inserts, or first / last with 1, 3 or 4 sides) on
+    ``bw_kjoin_*`` (K15): `_JoinLogic` under `stateful` (operators/__init__.py:2076-2190, 1025-1062), one call per
+    activation.  Items are ``(key, (side, value))`` from ``_join_label_merge``.  Key interning, the handle dict, the key
+    re-sort and the release are the join-window step's; there is no clock, so no notify phase.  Each row is one tuple
+    of an emission's product, expanded on the device."""
+
+    def __init__(self, step_id: str, plan):
+        import numpy as np
+
+        self.np, self.plan, self.step_id = np, plan, step_id
+        self.key_ids: Dict[str, int] = {}
+        self.id_keys: Dict[int, str] = {}
+        self.resort = False
+        self.last_epoch = 0
+        self.values: Dict[int, Any] = {}  # handle -> value, while the device holds the handle
+        self.next_handle = 0
+        self.jwin = None
+
+    def on_epoch(self, epoch: int, items: list) -> list:
+        np = self.np
+        keys, sides, handles = [], [], []
+        for item in items:
+            key, (side, value) = _split_item(self.step_id, item)
+            keys.append(self._key_id(key))
+            sides.append(side)
+            handles.append(self.next_handle)
+            self.values[self.next_handle] = value
+            self.next_handle += 1
+        if self.jwin is None:
+            self.jwin = self._make()
+        self.last_epoch = max(epoch, self.last_epoch)
+        self.jwin.apply(np.array(keys, dtype=np.uint64), np.array(sides, dtype=np.uint8), np.array(handles, dtype=np.uint64), self.last_epoch)
+        return self._jwin_rows(self.jwin.advance(), None)
+
+    def _make(self):
+        from bytewax_b200 import gpu
+
+        plan = self.plan
+        return gpu.KeyJoin(_get_gpu_ctx(), plan.insert_mode, plan.emit_mode, plan.sides,
+                           capacity_hint=int(os.environ.get("BYTEWAX_B200_KEYS", 1 << 20)),
+                           max_batch_rows=int(os.environ.get("BYTEWAX_B200_BATCH", 1 << 22)), max_emit_rows=1 << 22,
+                           max_product_rows=1 << 28)
+
+    def _jwin_rows(self, out, _labelled) -> list:
+        V = self.values
+        rows = [(self._key_str(k), tuple(None if h is None else V[h] for h in t)) for k, t in zip(out.key.tolist(), out.tuples())]
+        if self.resort:  # interned (non-numeric) keys: restore ascending key-string order; stable
+            rows.sort(key=lambda r: r[0])
+        for h in out.released.tolist():  # after this call's rows are built: no later row can name these
+            del V[h]
         return rows
 
 

@@ -896,6 +896,91 @@ class KeyCollect:
 
 
 @dataclass
+class KeyJoinRows:
+    """Rows of one ``KeyJoin.advance`` / ``eof`` in the reference's downstream order: per call, ascending key string, a
+    key's emissions in item order, each emission's tuples in ``itertools.product`` order; and the handles released since
+    the previous one."""
+
+    key: np.ndarray
+    handles: np.ndarray  # [rows, sides] uint64; valid where the side's bit of mask is set
+    mask: np.ndarray
+    epoch: np.ndarray
+    released: np.ndarray  # uint64, in no particular order
+
+    def tuples(self) -> List[tuple]:
+        """The joined tuple of every row: a handle per side, None where the side's list was empty."""
+        m = self.mask.tolist()
+        return [tuple(int(h[s]) if mk >> s & 1 else None for s in range(len(h))) for h, mk in zip(self.handles.tolist(), m)]
+
+
+class KeyJoin:
+    """The keyed ``op.join`` with 1 to 4 sides and any insert mode (``bw_kjoin``, K15; ``_JoinLogic`` + ``_JoinState``,
+    operators/__init__.py:2076-2190).  Each row is one tuple of an emission's ``itertools.product``, expanded on the
+    device; values travel as uint64 handles, and each comes back in ``released`` once no list holds it."""
+
+    INSERT = {"first": 0, "last": 1, "product": 2}
+    EMIT = {"complete": 0, "final": 1, "running": 2}
+
+    def __init__(self, ctx: Context, insert_mode: str = "product", emit_mode: str = "final", sides: int = 2, capacity_hint: int = 1 << 16,
+                 max_batch_rows: int = 1 << 20, max_emit_rows: int = 1 << 20, max_product_rows: int = 1 << 26):
+        """``max_product_rows``: rows one ``advance`` / ``eof`` may hand out."""
+        self.ctx, self.lib, self.sides = ctx, ctx.lib, sides
+        s = N.BwKjoinSpec()
+        s.struct_size = C.sizeof(N.BwKjoinSpec)
+        s.insert_mode, s.emit_mode, s.sides = self.INSERT.get(insert_mode, -1), self.EMIT.get(emit_mode, -1), sides
+        s.capacity_hint, s.max_batch_rows, s.max_emit_rows, s.max_product_rows = capacity_hint, max_batch_rows, max_emit_rows, max_product_rows
+        self.spec = s
+        h = C.c_void_p()
+        N.check(self.lib.bw_kjoin_create(ctx.h, C.byref(s), C.byref(h)), ctx.h)
+        self.h = h
+        self._epoch = 0
+
+    def _next_epoch(self, epoch: Optional[int]) -> int:
+        if epoch is None:
+            self._epoch += 1
+            return self._epoch
+        return epoch
+
+    def apply(self, keys, sides, handles, epoch: Optional[int] = None):
+        """One activation from host arrays: ``sides[i]`` is the side (0 .. sides-1) of item i."""
+        keys = np.ascontiguousarray(keys, dtype=np.uint64)
+        sides = np.ascontiguousarray(sides, dtype=np.uint8)
+        handles = np.ascontiguousarray(handles, dtype=np.uint64)
+        vp = lambda a: a.ctypes.data_as(C.c_void_p)  # noqa: E731
+        N.check(self.lib.bw_kjoin_apply(self.h, vp(keys), vp(sides), vp(handles), keys.shape[0], self._next_epoch(epoch)), self.ctx.h)
+
+    def apply_device(self, d_keys: int, d_sides: int, d_handles: int, rows: int, epoch: Optional[int] = None):
+        N.check(self.lib.bw_kjoin_apply_device(self.h, C.c_void_p(d_keys), C.c_void_p(d_sides), C.c_void_p(d_handles), rows,
+                                               self._next_epoch(epoch)), self.ctx.h)
+
+    def _wrap(self, r: N.BwKjoinRows) -> KeyJoinRows:
+        n, nr = int(r.n), int(r.n_released)
+
+        def arr(ptr, k):
+            return np.ctypeslib.as_array(ptr, shape=(k,)).copy() if k else np.zeros(0, np.uint64)
+
+        hs = np.stack([arr(r.handle[s], n) for s in range(self.sides)], axis=1) if n else np.zeros((0, self.sides), np.uint64)
+        return KeyJoinRows(arr(r.key, n), hs, arr(r.mask, n), arr(r.epoch, n), arr(r.released, nr))
+
+    def advance(self) -> KeyJoinRows:
+        """Rows since the last call."""
+        r = N.BwKjoinRows()
+        N.check(self.lib.bw_kjoin_advance(self.h, C.byref(r)), self.ctx.h)
+        return self._wrap(r)
+
+    def eof(self) -> KeyJoinRows:
+        """End of input: "final" emits every key's product; every handle still held is released."""
+        r = N.BwKjoinRows()
+        N.check(self.lib.bw_kjoin_eof(self.h, C.byref(r)), self.ctx.h)
+        return self._wrap(r)
+
+    def close(self):
+        if self.h:
+            self.lib.bw_kjoin_destroy(self.h)
+            self.h = None
+
+
+@dataclass
 class SessionCollectWindowRows(CollectWindowRows):
     """Rows of one ``SessionCollectWindow.advance`` / ``eof``.  Each down row is a closed session: its handles in
     flattened play order (``lists()``), its merge intervals (``merges(i)``) and its ``M`` row's bounds and merged ids

@@ -621,6 +621,17 @@ class GpuJoinPlan:
     emit_mode: str
 
 
+@dataclass(frozen=True)
+class GpuKeyJoinPlan:
+    """A ``join`` with 1 to 4 sides that `GpuJoinPlan` does not cover -- product inserts, and first / last with 1, 3 or 4
+    sides: the engine may run it with ``bw_kjoin_*`` (K15); values travel as handles into a host-side dict, so they can
+    be any Python object."""
+
+    insert_mode: str
+    emit_mode: str
+    sides: int
+
+
 @operator
 def stateful_map(step_id: str, up: KeyedStream, mapper: Callable[[Optional[Any], Any], Tuple[Optional[Any], Any]]) -> KeyedStream:
     """operators/__init__.py:2920."""
@@ -738,5 +749,9 @@ def join(step_id: str, *sides: KeyedStream, insert_mode: str = "last", emit_mode
         return _JoinLogic(insert_mode, emit_mode, state)
 
     merged = _join_label_merge("add_names", *sides)
-    plan = GpuJoinPlan(insert_mode, emit_mode) if side_count == 2 and insert_mode in ("first", "last") else None
+    plan = None
+    if side_count == 2 and insert_mode in ("first", "last"):
+        plan = GpuJoinPlan(insert_mode, emit_mode)
+    elif 1 <= side_count <= 4:  # (more sides stay on the host engine)
+        plan = GpuKeyJoinPlan(insert_mode, emit_mode, side_count)
     return stateful("join", merged, shim_builder, _gpu_plan=plan)

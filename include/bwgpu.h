@@ -341,9 +341,9 @@ bw_status bw_smap_sync(bw_smap* m);
 
 /* Two-sided keyed join: `_JoinLogic.on_item` / `on_eof` (operators/__init__.py:2157-2190) over the
  * side-labelled merged stream of `_join_label_merge` (:2193-2204); insert modes first / last,
- * emit modes complete / final / running (`product` keeps lists per side: host path only; windowed product joins:
- * bw_pjwin_*, K14). */
-typedef enum { BW_JOIN_INSERT_FIRST = 0, BW_JOIN_INSERT_LAST = 1 } bw_join_insert;
+ * emit modes complete / final / running.  Product inserts, and first / last with 1, 3 or 4 sides: bw_kjoin_*, K15;
+ * windowed product joins: bw_pjwin_*, K14. */
+typedef enum { BW_JOIN_INSERT_FIRST = 0, BW_JOIN_INSERT_LAST = 1, BW_JOIN_INSERT_PRODUCT = 2 } bw_join_insert;
 typedef enum { BW_JOIN_EMIT_COMPLETE = 0, BW_JOIN_EMIT_FINAL = 1, BW_JOIN_EMIT_RUNNING = 2 } bw_join_emit_mode;
 typedef struct bw_join bw_join;
 typedef struct bw_join_spec {
@@ -927,6 +927,59 @@ bw_status bw_kcollect_apply_device(bw_kcollect* c, const uint64_t* d_keys, const
 bw_status bw_kcollect_advance(bw_kcollect* c, int64_t now_us, bw_kcollect_rows* out);
 /* End of input: every key holding a list emits it (`on_eof` :1136-1137, src/operators.rs:862-894). */
 bw_status bw_kcollect_eof(bw_kcollect* c, bw_kcollect_rows* out);
+
+/* Keyed join (K15): `op.join` (pysrc/bytewax/operators/__init__.py:2324-2372) with 1 to 4 sides, i.e. `_JoinLogic` +
+ * `_JoinState` (:2076-2190) under `_StatefulLogic.on_batch` (:1030-1042) over the `(key, (side, value))` stream of
+ * `_join_label_merge`.  Per key, per call, in arrival order: "product" appends the value to its side's list, "last"
+ * replaces the list with [value], "first" sets it only while it is empty; "complete" emits the product once every side
+ * is non-empty and discards the key's lists (its next item, even in the same call, starts from empty lists); "running"
+ * emits the product after every item; "final" emits it at EOF for every key with a logic.  A product is
+ * `itertools.product` of the lists, the last side varying fastest, each list in arrival order, an empty list giving one
+ * None: an emission whose lists hold n_0 .. n_{sides-1} values gives prod max(1, n_s) rows, expanded on the device at
+ * advance / eof.  Values travel as u64 handles (any u64: none is reserved).  A key's slot is kept once seen, so
+ * capacity_hint covers every key ever seen.  One GPU only.  (The two-sided first / last join also runs on bw_join_*, K6.) */
+typedef struct bw_kjoin bw_kjoin;
+typedef struct bw_kjoin_spec {
+  uint32_t struct_size;
+  int32_t insert_mode;        /* BW_JOIN_INSERT_FIRST / LAST / PRODUCT */
+  int32_t emit_mode;          /* BW_JOIN_EMIT_COMPLETE / FINAL / RUNNING */
+  int32_t sides;              /* 1..4 joined streams */
+  uint64_t capacity_hint;     /* keys ever seen, < 2^30 */
+  uint64_t max_batch_rows;    /* < 2^31 */
+  uint64_t max_emit_rows;     /* < 2^31: emissions (each one product) retained between advances */
+  uint64_t max_product_rows;  /* down rows one advance / eof may hand out (the sum of the emissions' products) */
+} bw_kjoin_spec;
+/* Rows handed downstream since the last advance / eof, in the reference's order: per call (activation or EOF), ascending
+ * key string (src/operators.rs:758-767, :862-894), a key's emissions in item order, each emission's tuples in product
+ * order.  handle[s] is valid where mask bit s is set (else the side's list was empty: None).  `released` are the
+ * handles no list holds any more, each exactly once, in the call after which nothing holds it: the caller may drop
+ * their objects once it has built this call's rows.  Host pointers into memory owned by the library, valid until the
+ * next advance / eof / destroy. */
+typedef struct bw_kjoin_rows {
+  uint64_t n;
+  const uint64_t* key;
+  const uint64_t* handle[4];
+  const uint64_t* mask;
+  const uint64_t* epoch;
+  uint64_t n_released;
+  const uint64_t* released;
+} bw_kjoin_rows;
+bw_status bw_kjoin_create(bw_ctx* ctx, const bw_kjoin_spec* spec, bw_kjoin** out);
+void bw_kjoin_destroy(bw_kjoin* j);
+/* One activation from HOST columns (keys, side 0..sides-1, handles); blocks.  The entry store and the staging, release
+ * and output buffers grow before each call to what it can add.  A full key table, more than max_emit_rows emissions
+ * since the last advance, or a side list at 2^32 values returns BW_ERR_CAPACITY (reason in bw_last_error) and the join
+ * refuses further calls. */
+bw_status bw_kjoin_apply(bw_kjoin* j, const uint64_t* keys, const uint8_t* side, const uint64_t* handles, uint64_t rows, uint64_t epoch);
+/* Same with DEVICE columns; returns once the work is enqueued (the columns must stay valid until the next call).  A side
+ * value >= sides is not played: the next call returns BW_ERR_SPEC and the join refuses further calls. */
+bw_status bw_kjoin_apply_device(bw_kjoin* j, const uint64_t* d_keys, const uint8_t* d_side, const uint64_t* d_handles, uint64_t rows,
+                                uint64_t epoch);
+/* Rows since the last call.  More than max_product_rows rows fails with BW_ERR_CAPACITY and the join refuses further
+ * calls. */
+bw_status bw_kjoin_advance(bw_kjoin* j, bw_kjoin_rows* out);
+/* End of input: "final" emits every key that has a logic (`on_eof`); every handle still held is released. */
+bw_status bw_kjoin_eof(bw_kjoin* j, bw_kjoin_rows* out);
 
 /* ---- plain device-memory helpers (tests / bench / host bindings without torch) ---- */
 bw_status bw_dev_alloc(bw_ctx* ctx, uint64_t bytes, void** out);
