@@ -219,6 +219,13 @@ class BwKjoinRows(C.Structure):
                 ("released", C.POINTER(C.c_uint64))]
 
 
+class BwSpjwinSpec(C.Structure):
+    _fields_ = [("struct_size", C.c_uint32), ("emit_mode", C.c_int32), ("ordered", C.c_int32), ("sides", C.c_int32),
+                ("max_sessions_per_key", C.c_int32), ("pad", C.c_int32), ("gap_us", C.c_int64), ("wait_us", C.c_int64),
+                ("capacity_hint", C.c_uint64), ("max_queued_rows", C.c_uint64), ("max_batch_rows", C.c_uint64),
+                ("max_emit_rows", C.c_uint64), ("max_late_rows", C.c_uint64), ("max_product_rows", C.c_uint64)]
+
+
 # every symbol include/bwgpu.h declares: (restype, argtypes)
 _P = C.c_void_p
 SYMBOLS = {
@@ -314,6 +321,12 @@ SYMBOLS = {
     "bw_kjoin_apply_device": (C.c_int32, [_P, _P, _P, _P, C.c_uint64, C.c_uint64]),
     "bw_kjoin_advance": (C.c_int32, [_P, C.POINTER(BwKjoinRows)]),
     "bw_kjoin_eof": (C.c_int32, [_P, C.POINTER(BwKjoinRows)]),
+    "bw_spjwin_create": (C.c_int32, [_P, C.POINTER(BwSpjwinSpec), C.POINTER(_P)]),
+    "bw_spjwin_destroy": (None, [_P]),
+    "bw_spjwin_apply": (C.c_int32, [_P, _P, _P, _P, _P, C.c_uint64, C.c_uint64, C.c_int64]),
+    "bw_spjwin_apply_device": (C.c_int32, [_P, _P, _P, _P, _P, C.c_uint64, C.c_uint64, C.c_int64]),
+    "bw_spjwin_advance": (C.c_int32, [_P, C.c_int64, C.POINTER(BwSjwinRows)]),
+    "bw_spjwin_eof": (C.c_int32, [_P, C.POINTER(BwSjwinRows)]),
     "bw_dev_alloc": (C.c_int32, [_P, C.c_uint64, C.POINTER(_P)]),
     "bw_dev_free": (C.c_int32, [_P, _P]),
     "bw_host_alloc": (C.c_int32, [_P, C.c_uint64, C.POINTER(_P)]),

@@ -43,6 +43,7 @@
 #include "bw_kcollect.cuh"
 #include "bw_pjwin.cuh"
 #include "bw_kjoin.cuh"
+#include "bw_spjwin.cuh"
 #include "bw_prepass.cuh"
 #include "bw_slow.cuh"
 #include "bw_late.cuh"
@@ -5728,4 +5729,447 @@ bw_status bw_kjoin_eof(bw_kjoin* j, bw_kjoin_rows* out) {
   j->undrained = true;
   if ((st = kjoin_gather(j, p)) != BW_OK) return st;
   return kjoin_collect(j, out);
+}
+
+// ===========================================================================
+// K16 host side: windowed product join over session windows (bw_spjwin.cuh)
+// ===========================================================================
+// K9's store growth and compaction (store_room), K8's drain, release-buffer growth and pool sort (jwin_drain, jwin_room,
+// jwin_sort_pool, jwin_ship) and K14's expansion read these members by the names bw_pjwin / bw_kjoin give them.
+struct bw_spjwin {
+  Owner own;  // every buffer and the stream below
+  bw_ctx* ctx = nullptr;
+  bw_spjwin_spec spec{};
+  SpTable t{};
+  CwStore es{};
+  KeyedScratch k;
+  cudaStream_t s = nullptr;
+  u32* h_err = nullptr;  // err, why
+  // events, meta, late, released, carried-over queue entries, stage records, staged, store entries, dead entries, merged
+  // ids, merges
+  unsigned long long* d_cnt = nullptr;
+  unsigned long long* h_cnt = nullptr;
+  unsigned char *d_side = nullptr, *d_late = nullptr, *d_flag = nullptr;
+  u64* d_handles = nullptr;
+  i64* d_ts = nullptr;
+  SpEmit e{};
+  JwPool pool{}, pool2{};  // ordered mode: the queue, and the one the next flush writes
+  u64 nq = 0;              // entries in `pool`
+  int slot_bits = 1;
+  u64 n_store = 0, dead = 0;               // entries in the store, and how many of them are dead
+  u64 n_rec = 0, n_meta = 0, n_stage = 0;  // stage records, meta rows and staged handles since the last advance / eof
+  u64 n_mrg = 0;                           // keys that merged, so far
+  SortScratch srt;                         // pool sort, ordering and compaction scratch
+  PjOrdered o{};                           // advance / eof: the events in the reference's order
+  u64* d_off = nullptr;                    // the exclusive scan of their row counts
+  PjRows rows{};                           // the expanded rows
+  u64 rows_cap = 0;
+  HostCols hd[2];  // down: key, window id, h0, h1, h2 | h3, mask, epoch
+  HostCols hm[2];  // meta: key, window id, open, close, epoch | merged count, merged offset
+  HostCols hl;     // late: key, window id, epoch, activation, row
+  i64* h_mids = nullptr;
+  std::vector<u64> merged_off;
+  std::vector<i64> merged_ids;
+  std::vector<u64> released;      // since the last advance / eof
+  std::vector<u64> released_out;  // what the last advance / eof handed out
+  bool undrained = false;     // a call whose counts are not read back yet
+  u64 outstanding = 0;        // handles passed in and not released yet: what the next call can release, besides its own
+  u32 batch_no = 0;
+  u64 calls = 0, first_call = 0;  // calls (activations, notify phases, EOF) so far; the first not yet collected
+  u64 last_epoch = 0;
+  i64 now = INT64_MIN;
+  bool failed = false;
+};
+
+static const char* jwin_what(const bw_spjwin*) { return "session product join"; }
+static const char* jwin_full_windows(const bw_spjwin*) { return " a key needs more than max_sessions_per_key sessions or merged ids;"; }
+static const char* jwin_full_emit(const bw_spjwin*) {
+  return " more than max_emit_rows emissions, meta rows or merged ids since the last advance;";
+}
+static u64 jwin_counters(const bw_spjwin*) { return 11; }
+
+bw_status bw_spjwin_create(bw_ctx* ctx, const bw_spjwin_spec* spec, bw_spjwin** out) {
+  if (!ctx || !spec || !out) CTX_FAIL(ctx, BW_ERR_SPEC, "bw_spjwin_create: NULL argument");
+  if (spec->struct_size != sizeof(bw_spjwin_spec)) CTX_FAIL(ctx, BW_ERR_SPEC, "bw_spjwin_spec.struct_size mismatch");
+  if (ctx->world != 1) CTX_FAIL(ctx, BW_ERR_SPEC, "session product joins run on one GPU (world == 1)");
+  if (spec->emit_mode < BW_JOIN_EMIT_COMPLETE || spec->emit_mode > BW_JOIN_EMIT_RUNNING) CTX_FAIL(ctx, BW_ERR_SPEC, "bad emit_mode");
+  if (spec->ordered != 0 && spec->ordered != 1) CTX_FAIL(ctx, BW_ERR_SPEC, "ordered must be 0 or 1");
+  if (spec->sides < 1 || spec->sides > BW_JW_MAXSIDES) CTX_FAIL(ctx, BW_ERR_SPEC, "sides must be in 1..%d", BW_JW_MAXSIDES);
+  if (spec->max_sessions_per_key < 1 || spec->max_sessions_per_key > BW_SESS_MAXM)
+    CTX_FAIL(ctx, BW_ERR_SPEC, "max_sessions_per_key must be in 1..%d", BW_SESS_MAXM);
+  if (spec->gap_us < 0 || spec->gap_us > BW_UTC_MAX_US - BW_UTC_MIN_US) CTX_FAIL(ctx, BW_ERR_SPEC, "gap_us must be in 0..UTC_MAX - UTC_MIN");
+  if (spec->wait_us < 0) CTX_FAIL(ctx, BW_ERR_SPEC, "wait_us must not be negative");
+  if (spec->max_batch_rows == 0 || spec->max_batch_rows >= (1ULL << 31)) CTX_FAIL(ctx, BW_ERR_SPEC, "bad max_batch_rows");
+  if (spec->max_queued_rows >= (1ULL << 31) - spec->max_batch_rows) CTX_FAIL(ctx, BW_ERR_SPEC, "max_queued_rows + max_batch_rows must stay below 2^31");
+  if (spec->max_emit_rows >= (1ULL << 31)) CTX_FAIL(ctx, BW_ERR_SPEC, "max_emit_rows must be below 2^31");
+  if (spec->capacity_hint >= (1ULL << 30)) CTX_FAIL(ctx, BW_ERR_SPEC, "capacity_hint must be below 2^30");
+  CU(ctx, cudaSetDevice(ctx->device));
+  std::unique_ptr<bw_spjwin, void (*)(bw_spjwin*)> jp(new bw_spjwin(), bw_spjwin_destroy);  // torn down on every failure
+  bw_spjwin* j = jp.get();
+  Owner& own = j->own;
+  j->ctx = ctx;
+  j->spec = *spec;
+  const u64 cap = std::max<u64>(1024, 2 * std::max<u64>(spec->capacity_hint, 1));
+  const int M = spec->max_sessions_per_key;
+  const u64 cells = (cap + 1) * (u64)M;
+  SpTable& t = j->t;
+  t.j.cap = cap;
+  t.j.M = M;
+  t.j.sides = spec->sides;
+  t.gap = spec->gap_us;
+  while ((1ULL << j->slot_bits) < cap + 1) ++j->slot_bits;
+  CU(ctx, own.stream(&j->s));
+  CU(ctx, own.dev(&t.j.keys, cap + 1));
+  CU(ctx, own.dev(&t.j.st, cap + 1));
+  CU(ctx, own.dev(&t.kx, cap + 1));
+  CU(ctx, own.dev(&t.rec, cells));
+  CU(ctx, own.dev(&t.mrg, 2 * cells));
+  CU(ctx, own.dev(&t.cell, cells));
+  CU(ctx, own.dev(&t.rec_ord, cells));
+  CU(ctx, own.dev(&t.rec_c, cells));
+  CU(ctx, own.dev(&t.close_ord, cells));
+  CU(ctx, own.dev(&t.mord, cells));
+  CU(ctx, own.dev(&t.hop, cells));
+  t.j.win = nullptr;  // (K8's window records and K14's: sessions live in rec)
+  t.win = nullptr;
+  CU(ctx, own.dev(&t.j.err, 2));
+  t.j.why = t.j.err + 1;
+  t.err = t.j.err;
+  t.why = t.j.why;
+  CU(ctx, own.dev(&j->d_cnt, 11));
+  CU(ctx, cudaMemsetAsync(t.err, 0, 8, j->s));
+  CU(ctx, cudaMemsetAsync(j->d_cnt, 0, 88, j->s));
+  CU(ctx, own.host(&j->h_err, 64 / sizeof(u32)));
+  CU(ctx, own.host(&j->h_cnt, 16));
+  const u64 n = spec->max_batch_rows, m = std::max<u64>(spec->max_emit_rows, 1), l = std::max<u64>(spec->max_late_rows, 1);
+  const u64 q = spec->ordered ? spec->max_queued_rows : 0;
+  bw_status st = keyed_alloc(ctx, own, j->k, n, j->s);
+  if (st != BW_OK) return st;
+  CU(ctx, own.dev(&j->d_side, n));
+  CU(ctx, own.dev(&j->d_late, n));
+  CU(ctx, own.dev(&j->d_handles, n));
+  CU(ctx, own.dev(&j->d_ts, n));
+  if (spec->ordered) {
+    if ((st = jwin_pool_alloc(ctx, own, j->pool, q + n)) != BW_OK) return st;
+    if ((st = jwin_pool_alloc(ctx, own, j->pool2, q + n)) != BW_OK) return st;
+  }
+  SpEmit& e = j->e;
+  for (u64** c : {&e.key, &e.wid, &e.epoch, &e.ord, &e.seq, &e.rec, &e.m_key, &e.m_wid, &e.m_epoch, &e.m_ord, &e.m_seq, &e.m_moff, &e.m_mcnt})
+    CU(ctx, own.dev(c, m));
+  for (i64** c : {&e.m_open, &e.m_close, &e.mids}) CU(ctx, own.dev(c, m));
+  for (u64** c : {&e.l_key, &e.l_wid, &e.l_epoch, &e.l_act, &e.l_row, &e.l_ord, &e.l_seq}) CU(ctx, own.dev(c, l));
+  for (u32** c : {&e.lo, &e.hi, &e.rb, &e.rn}) CU(ctx, own.dev(c, 4 * m));
+  CU(ctx, own.dev(&e.rbase, 4 * m));
+  PjOrdered& o = j->o;
+  for (u64** c : {&o.cnt, &o.key, &o.wid, &o.epoch}) CU(ctx, own.dev(c, m + 1));
+  CU(ctx, own.dev(&o.base, 4 * m));
+  CU(ctx, own.dev(&o.len, 4 * m));
+  CU(ctx, own.dev(&j->d_off, m + 1));
+  // the store, the staging buffer, the release buffer and the output grow with what the join holds and emits
+  // (spjwin_room, spjwin_gather, spjwin_expand); they start at one batch
+  CwStore& es = j->es;
+  es.cap = n;
+  CU(ctx, own.dev(&es.ref, n));
+  CU(ctx, own.dev(&es.rank, n));
+  CU(ctx, own.dev(&es.h, n));
+  CU(ctx, own.dev(&j->d_flag, n));
+  e.max_stage = n;
+  CU(ctx, own.dev(&e.stage, n));
+  e.max_rel = n;
+  CU(ctx, own.dev(&e.rel, e.max_rel));
+  e.max_rows = spec->max_emit_rows;
+  e.max_late = spec->max_late_rows;
+  e.max_queue = q;
+  e.n_rows = j->d_cnt;
+  e.n_meta = j->d_cnt + 1;
+  e.n_late = j->d_cnt + 2;
+  e.n_rel = j->d_cnt + 3;  // (jwin_drain reads these two)
+  e.n_next = j->d_cnt + 4;
+  e.n_rec = j->d_cnt + 5;
+  e.n_stage = j->d_cnt + 6;
+  es.n = j->d_cnt + 7;     // (d_cnt + 8: entries that died in the call)
+  e.n_mids = j->d_cnt + 9;
+  e.n_mrg = j->d_cnt + 10;
+  const u64 ns = std::max(std::max(m, l), q + n);
+  CU(ctx, j->srt.reserve(own, ns, ns, j->s));
+  size_t b = 0;
+  CU(ctx, cub::DeviceScan::ExclusiveScan(nullptr, b, o.cnt, j->d_off, PjSatAdd{}, (u64)0, (int)(m + 1), j->s));
+  CU(ctx, j->srt.grow_cub(own, b + 256));
+  CU(ctx, j->hm[0].reserve(own, m, m));
+  CU(ctx, j->hm[1].reserve(own, m, m));
+  CU(ctx, j->hl.reserve(own, l, l));
+  CU(ctx, own.host(&j->h_mids, m));
+  k_spjwin_init<<<ctx->sm_count * 4, 256, 0, j->s>>>(t);
+  CU(ctx, cudaGetLastError());
+  CU(ctx, cudaStreamSynchronize(j->s));
+  *out = jp.release();
+  return BW_OK;
+}
+
+void bw_spjwin_destroy(bw_spjwin* j) {
+  if (!j) return;
+  cudaSetDevice(j->ctx->device);
+  if (j->s) cudaStreamSynchronize(j->s);
+  delete j;  // j->own releases every buffer and the stream
+}
+
+static JwParams spjwin_params(bw_spjwin* j, u64 epoch) {
+  JwParams p{};
+  p.emit_mode = j->spec.emit_mode;
+  p.ordered = j->spec.ordered;
+  p.wait = j->spec.wait_us;
+  p.now = j->now;
+  p.epoch = epoch;
+  p.ord = j->calls++;
+  p.batch_no = j->batch_no;
+  return p;
+}
+
+#define SPJWIN_REFUSE_FAILED(j) \
+  if ((j)->failed) CTX_FAIL((j)->ctx, BW_ERR_STATE, "session product join: an earlier call failed on the device; the join is unusable")
+
+// K8's drain (failure, released handles, queue count), then the counts only this join keeps
+static bw_status spjwin_drain(bw_spjwin* j) {
+  const bool pending = j->undrained;
+  bw_status st = jwin_drain(j);
+  if (st != BW_OK || !pending) return st;
+  j->n_meta = j->h_cnt[1];
+  j->n_rec = j->h_cnt[5];
+  j->n_stage = j->h_cnt[6];
+  j->n_store = j->h_cnt[7];
+  j->dead += j->h_cnt[8];
+  j->n_mrg = j->h_cnt[10];
+  CU(j->ctx, cudaMemsetAsync(j->d_cnt + 8, 0, 8, j->s));
+  return BW_OK;
+}
+
+// Before a call that can play `rows` values (and ordered the queued entries): room in the release buffer, and in the
+// store for one entry per value (K9's compaction and growth).  Called after the drain: nothing on the stream reads them.
+static bw_status spjwin_room(bw_spjwin* j, u64 rows) {
+  bw_status st = jwin_room(j, rows);
+  if (st != BW_OK) return st;
+  return store_room(j, rows + (j->spec.ordered ? j->nq : 0));
+}
+
+// The emit buffers the per-key kernels see.  One entry may be staged once per hop of a merge chain, so no bound on a
+// call's staging is known before it runs: the kernels' stage records only reserve their ranges (no limit checked here),
+// and spjwin_gather grows the buffer to what they reserved before anything is written there.
+static SpEmit spjwin_walk_emit(const bw_spjwin* j) {
+  SpEmit e = j->e;
+  e.max_stage = ~0ULL;
+  return e;
+}
+
+// after the per-key kernels of a call: room in staging for their stage records (what earlier calls staged is kept), then
+// stage, retag and kill along every hop, and release (k_spjwin_gather)
+static bw_status spjwin_gather(bw_spjwin* j, const JwParams& p) {
+  bw_ctx* ctx = j->ctx;
+  SpEmit& e = j->e;
+  CU(ctx, cudaMemcpyAsync(j->h_cnt + 13, e.n_stage, 8, cudaMemcpyDeviceToHost, j->s));
+  CU(ctx, cudaMemcpyAsync(j->h_err + 2, j->t.err, 4, cudaMemcpyDeviceToHost, j->s));
+  CU(ctx, cudaStreamSynchronize(j->s));
+  const u64 need = j->h_cnt[13];
+  if (!j->h_err[2] && need > e.max_stage) {  // (after a failed call the gather does nothing and the drain reports it)
+    const u64 grow = std::max<u64>(need, 2 * e.max_stage);
+    e.max_stage = 0;
+    CU(ctx, collect_grow_keep(j, &e.stage, j->n_stage, grow));
+    e.max_stage = grow;
+  }
+  k_spjwin_gather<<<ctx->sm_count * 8, 256, 0, j->s>>>(j->t, e, j->es, p, j->n_rec, j->n_meta, j->n_mrg, j->d_cnt + 8);
+  CU(ctx, cudaGetLastError());
+  return BW_OK;
+}
+
+// ordered mode: sort the pool's due entries into play order (K8's sort); then flush every woken key (k_spjwin_flush)
+static bw_status spjwin_flush(bw_spjwin* j, const JwParams& p, u64 n) {
+  bw_ctx* ctx = j->ctx;
+  bw_status st = j->spec.ordered ? jwin_sort_pool(j, j->t.j, p, n) : BW_OK;
+  if (st != BW_OK) return st;
+  SpEmit e = spjwin_walk_emit(j);
+  e.next = j->pool2;
+  k_spjwin_flush<<<ctx->sm_count * 8, 256, 0, j->s>>>(j->t, e, j->es, p, j->pool, j->srt.perm);
+  CU(ctx, cudaGetLastError());
+  if (j->spec.ordered) std::swap(j->pool, j->pool2);  // the next call reads what this flush carried over (count: jwin_drain)
+  return spjwin_gather(j, p);
+}
+
+bw_status bw_spjwin_apply_device(bw_spjwin* j, const uint64_t* d_keys, const uint8_t* d_side, const uint64_t* d_handles,
+                                 const int64_t* d_ts_us, uint64_t rows, uint64_t epoch, int64_t system_now_us) {
+  if (!j) return BW_ERR_SPEC;
+  bw_ctx* ctx = j->ctx;
+  SPJWIN_REFUSE_FAILED(j);
+  if (rows > j->spec.max_batch_rows) CTX_FAIL(ctx, BW_ERR_SPEC, "session product join: rows > max_batch_rows");
+  if (rows && (!d_keys || !d_side || !d_handles || !d_ts_us)) CTX_FAIL(ctx, BW_ERR_SPEC, "session product join: NULL column");
+  if (j->batch_no && epoch < j->last_epoch) CTX_FAIL(ctx, BW_ERR_STATE, "session product join: epochs must not decrease");
+  CU(ctx, cudaSetDevice(ctx->device));
+  bw_status st = spjwin_drain(j);
+  if (st != BW_OK) return st;
+  j->last_epoch = epoch;
+  if (system_now_us > j->now) j->now = system_now_us;  // `now_getter()` never goes backwards (windowing.py:250-261)
+  const JwParams p = spjwin_params(j, epoch);
+  j->batch_no++;
+  if (rows == 0) return BW_OK;
+  if ((st = spjwin_room(j, rows)) != BW_OK) return st;
+  j->outstanding += rows;
+  st = keyed_group(ctx, j->k, d_keys, rows, j->s);
+  if (st != BW_OK) return st;
+  k_spjwin_apply<<<ctx->sm_count * 8, 256, 0, j->s>>>(j->t, spjwin_walk_emit(j), j->es, p, j->pool, j->nq, j->k.d_ksorted, j->k.d_isorted,
+                                                      j->k.d_head, d_handles, d_side, d_ts_us, j->d_late, rows);
+  CU(ctx, cudaGetLastError());
+  j->undrained = true;
+  if (j->spec.ordered) return spjwin_flush(j, p, j->nq + rows);
+  return spjwin_gather(j, p);
+}
+
+static bw_status spjwin_apply_device_fn(bw_spjwin* j, const uint64_t* d_keys, const uint8_t* d_side, const uint64_t* d_handles,
+                                        const int64_t* d_ts_us, uint64_t rows, uint64_t epoch, int64_t system_now_us) {
+  bw_status st = bw_spjwin_apply_device(j, d_keys, d_side, d_handles, d_ts_us, rows, epoch, system_now_us);
+  if (st != BW_OK) return st;
+  return spjwin_drain(j);  // (jwin_apply_host drains once more: then nothing is pending)
+}
+
+bw_status bw_spjwin_apply(bw_spjwin* j, const uint64_t* keys, const uint8_t* side, const uint64_t* handles, const int64_t* ts_us,
+                          uint64_t rows, uint64_t epoch, int64_t system_now_us) {
+  if (j) {
+    SPJWIN_REFUSE_FAILED(j);
+    bw_status st = spjwin_drain(j);  // (before jwin_apply_host's own drain, which would skip this join's counts)
+    if (st != BW_OK) return st;
+  }
+  return jwin_apply_host(j, keys, side, handles, ts_us, rows, epoch, system_now_us, spjwin_apply_device_fn);
+}
+
+// advance / eof: the events in the reference's order (order_perm), K14's row counts and saturating scan; the host grows
+// the output to the total; K14's k_pjwin_expand writes every row in that order
+static bw_status spjwin_expand(bw_spjwin* j, u64 nd, u64* total) {
+  bw_ctx* ctx = j->ctx;
+  *total = 0;
+  if (!nd) return BW_OK;
+  SortScratch& x = j->srt;
+  bw_status st = order_perm(ctx, x, j->s, nd, j->e.key, j->e.seq, j->e.ord, nullptr, std::max<u64>(j->calls - j->first_call, 1), j->first_call,
+                            nullptr);
+  if (st != BW_OK) return st;
+  const int grid = ctx->sm_count * 4;
+  const PjOrdered o = j->o;
+  k_pjwin_count<<<grid, 256, 0, j->s>>>(j->e, o, j->spec.sides, x.perm, nd);
+  CU(ctx, cudaMemsetAsync(o.cnt + nd, 0, 8, j->s));
+  size_t tb = x.cub_bytes;
+  CU(ctx, cub::DeviceScan::ExclusiveScan(x.cub, tb, o.cnt, j->d_off, PjSatAdd{}, (u64)0, (int)(nd + 1), j->s));
+  CU(ctx, cudaMemcpyAsync(j->h_cnt + 12, j->d_off + nd, 8, cudaMemcpyDeviceToHost, j->s));
+  CU(ctx, cudaStreamSynchronize(j->s));
+  const u64 n = j->h_cnt[12];
+  if (n > j->spec.max_product_rows) {
+    j->failed = true;
+    CTX_FAIL(ctx, BW_ERR_CAPACITY, "session product join ran out of capacity: %llu product rows since the last advance, more than "
+             "max_product_rows (%llu)", (unsigned long long)n, (unsigned long long)j->spec.max_product_rows);
+  }
+  if (n > j->rows_cap) {
+    j->rows_cap = 0;
+    for (u64** c : {&j->rows.key, &j->rows.wid, &j->rows.h0, &j->rows.h1, &j->rows.h2, &j->rows.h3, &j->rows.mask, &j->rows.epoch})
+      CU(ctx, j->own.regrow(Owner::DEV, c, n));
+    j->rows_cap = n;
+  }
+  CU(ctx, j->hd[0].reserve(j->own, n, n));
+  CU(ctx, j->hd[1].reserve(j->own, n, n));
+  k_pjwin_expand<<<ctx->sm_count * 8, 256, 0, j->s>>>(o, j->d_off, nd, j->spec.sides, j->e.stage, j->rows, n);
+  const u64* src[] = {j->rows.key, j->rows.wid, j->rows.h0, j->rows.h1, j->rows.h2, j->rows.h3, j->rows.mask, j->rows.epoch};
+  for (int c = 0; c < 8; ++c) CU(ctx, cudaMemcpyAsync(j->hd[c / 5].col[c % 5], src[c], n * 8, cudaMemcpyDeviceToHost, j->s));
+  *total = n;
+  return BW_OK;
+}
+
+static bw_status spjwin_collect(bw_spjwin* j, bw_sjwin_rows* out) {
+  bw_ctx* ctx = j->ctx;
+  bw_status st = spjwin_drain(j);
+  if (st != BW_OK) return st;
+  CU(ctx, cudaMemcpyAsync(j->h_cnt, j->d_cnt, 88, cudaMemcpyDeviceToHost, j->s));
+  CU(ctx, cudaStreamSynchronize(j->s));
+  const u64 nd = j->h_cnt[0], nm = j->h_cnt[1], nl = j->h_cnt[2], nmid = j->h_cnt[9];  // all within bounds: the drain passed
+  u64 n = 0;
+  if ((st = spjwin_expand(j, nd, &n)) != BW_OK) return st;
+  const SpEmit& e = j->e;
+  const u64* meta[] = {e.m_key, e.m_wid, (const u64*)e.m_open, (const u64*)e.m_close, e.m_epoch, e.m_mcnt, e.m_moff};
+  const u64* late[] = {e.l_key, e.l_wid, e.l_epoch, e.l_act, e.l_row};
+  if ((st = jwin_ship(j, nm, e.m_key, e.m_seq, e.m_ord, meta, 7, j->hm)) != BW_OK) return st;
+  if ((st = jwin_ship(j, nl, e.l_key, e.l_seq, e.l_ord, late, 5, &j->hl)) != BW_OK) return st;
+  if (nmid) CU(ctx, cudaMemcpyAsync(j->h_mids, e.mids, nmid * 8, cudaMemcpyDeviceToHost, j->s));
+  CU(ctx, cudaGetLastError());
+  CU(ctx, cudaMemsetAsync(j->d_cnt, 0, 24, j->s));
+  CU(ctx, cudaMemsetAsync(j->d_cnt + 5, 0, 16, j->s));
+  CU(ctx, cudaMemsetAsync(j->d_cnt + 9, 0, 8, j->s));
+  CU(ctx, cudaStreamSynchronize(j->s));
+  j->n_rec = j->n_meta = j->n_stage = 0;
+  // merged ids in meta row order
+  j->merged_off.assign(nm + 1, 0);
+  j->merged_ids.resize(nmid);
+  const u64 *cnt = j->hm[1].col[0], *off = j->hm[1].col[1];
+  for (u64 r = 0; r < nm; ++r) {
+    j->merged_off[r + 1] = j->merged_off[r] + cnt[r];
+    std::copy(j->h_mids + off[r], j->h_mids + off[r] + cnt[r], j->merged_ids.begin() + j->merged_off[r]);
+  }
+  j->first_call = j->calls;
+  out->n_down = n;
+  out->down_key = j->hd[0].col[0];
+  out->down_window_id = (const int64_t*)j->hd[0].col[1];
+  out->down_handle[0] = j->hd[0].col[2];
+  out->down_handle[1] = j->hd[0].col[3];
+  out->down_handle[2] = j->hd[0].col[4];
+  out->down_handle[3] = j->hd[1].col[0];
+  out->down_mask = j->hd[1].col[1];
+  out->down_epoch = j->hd[1].col[2];
+  out->n_meta = nm;
+  out->meta_key = j->hm[0].col[0];
+  out->meta_window_id = (const int64_t*)j->hm[0].col[1];
+  out->meta_open_us = (const int64_t*)j->hm[0].col[2];
+  out->meta_close_us = (const int64_t*)j->hm[0].col[3];
+  out->meta_epoch = j->hm[0].col[4];
+  out->merged_off = j->merged_off.data();
+  out->merged_ids = j->merged_ids.data();
+  out->n_late = nl;
+  out->late_key = j->hl.col[0];
+  out->late_epoch = j->hl.col[2];
+  out->late_activation = j->hl.col[3];
+  out->late_row = j->hl.col[4];
+  // handed out until the next advance / eof, then cleared
+  j->released.swap(j->released_out);
+  j->released.clear();
+  out->n_released = j->released_out.size();
+  out->released = j->released_out.data();
+  return BW_OK;
+}
+
+// notify phase or EOF: wake the keys (K8's k_jwin_mark with the session notify_at), then flush them (ordered: through
+// the pool)
+static bw_status spjwin_wake(bw_spjwin* j, int eof) {
+  bw_ctx* ctx = j->ctx;
+  bw_status st = spjwin_drain(j);
+  if (st != BW_OK) return st;
+  if ((st = spjwin_room(j, 0)) != BW_OK) return st;
+  const JwParams p = spjwin_params(j, j->last_epoch);
+  k_jwin_mark<<<ctx->sm_count * 8, 256, 0, j->s>>>(j->t.j, (const SpRec*)j->t.rec, p, eof, SjNotifyAt{j->t.gap});
+  CU(ctx, cudaGetLastError());
+  j->undrained = true;
+  return spjwin_flush(j, p, j->nq);
+}
+
+bw_status bw_spjwin_advance(bw_spjwin* j, int64_t system_now_us, bw_sjwin_rows* out) {
+  if (!j || !out) return BW_ERR_SPEC;
+  bw_ctx* ctx = j->ctx;
+  SPJWIN_REFUSE_FAILED(j);
+  CU(ctx, cudaSetDevice(ctx->device));
+  if (system_now_us > 0) {
+    if (system_now_us > j->now) j->now = system_now_us;
+    bw_status st = spjwin_wake(j, 0);
+    if (st != BW_OK) return st;
+  }
+  return spjwin_collect(j, out);
+}
+
+bw_status bw_spjwin_eof(bw_spjwin* j, bw_sjwin_rows* out) {
+  if (!j || !out) return BW_ERR_SPEC;
+  bw_ctx* ctx = j->ctx;
+  SPJWIN_REFUSE_FAILED(j);
+  CU(ctx, cudaSetDevice(ctx->device));
+  bw_status st = spjwin_wake(j, 1);
+  if (st != BW_OK) return st;
+  return spjwin_collect(j, out);
 }

@@ -551,6 +551,22 @@ class _GpuSessionJoinWindowStep(_GpuJoinWindowStep):
         return rows
 
 
+class _GpuSessionProductJoinWindowStep(_GpuSessionJoinWindowStep):
+    """One worker's ``join_window(insert_mode="product")`` over a ``SessionWindower`` (``GpuJoinWindowPlan``) on
+    ``bw_spjwin_*`` (K16).  Ingest, handles, clock sampling, notify, EOF, the key re-sort and the rows (merged ids
+    included) are the session join step's; each down row is one tuple of an emission's product, expanded on the device."""
+
+    def _make(self):
+        from bytewax_b200 import gpu
+
+        plan = self.plan
+        return gpu.SessionProductJoinWindow(
+            _get_gpu_ctx(), plan.emit_mode, plan.ordered, plan.sides, self.gap_us, self.wait_us,
+            capacity_hint=int(os.environ.get("BYTEWAX_B200_KEYS", 1 << 20)), max_sessions_per_key=int(os.environ.get("BYTEWAX_B200_SESSIONS", 64)),
+            max_queued_rows=1 << 22 if plan.ordered else 0, max_batch_rows=int(os.environ.get("BYTEWAX_B200_BATCH", 1 << 22)),
+            max_emit_rows=1 << 22, max_late_rows=1 << 22, max_product_rows=1 << 28)
+
+
 class _GpuCollectWindowStep(_GpuJoinWindowStep):
     """One worker's ``collect_window`` (``GpuCollectWindowPlan``) on ``bw_collect_*`` (K9): `_WindowLogic` over a tumbling
     or sliding windower with the collect folder per window (windowing.py:1046-1190, 1356-1384, 1436-1576), one call per
@@ -819,6 +835,8 @@ def _gpu_step_for(step_id: str, plan):
                                                   GpuSessionCollectWindowPlan, SessionWindower)
 
     if isinstance(plan, GpuJoinWindowPlan):
+        if plan.insert_mode == "product" and isinstance(plan.windower, SessionWindower):
+            return _GpuSessionProductJoinWindowStep(step_id, plan)
         if plan.insert_mode == "product":
             return _GpuProductJoinWindowStep(step_id, plan)
         if isinstance(plan.windower, SessionWindower):

@@ -719,6 +719,31 @@ class SessionJoinWindow(_HandleJoin):
                                      arr(r.merged_ids, int(off[-1]), np.int64))
 
 
+class SessionProductJoinWindow(SessionJoinWindow):
+    """``join_window`` with insert mode product over session windows (``bw_spjwin``, K16; windowing.py:671-810,
+    1046-1190, 1849-1902, ``_JoinState`` operators/__init__.py:2072-2120).  Each down row is one tuple of an emission's
+    ``itertools.product``, expanded on the device; a merge appends the merged-away session's lists to the survivor's.
+    Values travel as uint64 handles, and each comes back in ``released`` once no session list and no queue entry holds
+    it.  Session bounds and merged ids come with each meta row."""
+
+    _PREFIX, _ROWS = "bw_spjwin", N.BwSjwinRows
+
+    def __init__(self, ctx: Context, emit_mode: str = "final", ordered: bool = True, sides: int = 2, gap_us: int = 10_000_000,
+                 wait_us: Optional[int] = 0, capacity_hint: int = 1 << 16, max_sessions_per_key: int = 16, max_queued_rows: int = 1 << 20,
+                 max_batch_rows: int = 1 << 20, max_emit_rows: int = 1 << 20, max_late_rows: int = 1 << 20,
+                 max_product_rows: int = 1 << 26):
+        """``wait_us=None``: the watermark never advances on data (``BW_WAIT_FOREVER``).  ``max_product_rows``: down rows
+        one ``advance`` / ``eof`` may hand out."""
+        s = N.BwSpjwinSpec()
+        s.struct_size = C.sizeof(N.BwSpjwinSpec)
+        s.emit_mode = self.EMIT.get(emit_mode, -1)
+        s.ordered, s.sides, s.max_sessions_per_key = int(ordered), sides, max_sessions_per_key
+        s.gap_us, s.wait_us = gap_us, N.BW_WAIT_FOREVER if wait_us is None else wait_us
+        s.capacity_hint, s.max_queued_rows, s.max_batch_rows = capacity_hint, max_queued_rows, max_batch_rows
+        s.max_emit_rows, s.max_late_rows, s.max_product_rows = max_emit_rows, max_late_rows, max_product_rows
+        self._create(ctx, s, sides)
+
+
 @dataclass
 class CollectWindowRows:
     """Rows of one ``CollectWindow.advance`` / ``eof``, each stream in the reference's downstream order, and the handles

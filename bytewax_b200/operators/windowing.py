@@ -876,7 +876,8 @@ def join_window(step_id: str, clock: Clock, windower: Windower, *sides: KeyedStr
         state = resume_state if resume_state is not None else _JoinState.for_side_count(side_count)
         return _JoinWindowLogic(insert_mode, emit_mode, state)
 
-    plan = _join_window_plan(clock, windower, side_count, insert_mode, emit_mode, ordered)
+    plan = (_join_window_plan(clock, windower, side_count, insert_mode, emit_mode, ordered)
+            or _session_product_join_window_plan(clock, windower, side_count, insert_mode, emit_mode, ordered))
     # items reach the clock as (side, value): unwrap for the user's ts_getter
     if isinstance(clock, EventClock):
         inner = clock.ts_getter
@@ -889,8 +890,9 @@ def join_window(step_id: str, clock: Clock, windower: Windower, *sides: KeyedStr
 class GpuJoinWindowPlan:
     """A ``join_window`` the engine may run on the device: insert mode first / last with ``bw_jwin_*`` (K8, tumbling or
     sliding windower) or ``bw_sjwin_*`` (K10, `SessionWindower`), insert mode product with ``bw_pjwin_*`` (K14, tumbling or
-    sliding windower only); 1 to 4 sides, and an `EventClock` with an identity ``to_system_utc`` or a `SystemClock`.
-    Values travel as handles into a host-side dict, so they can be any Python object."""
+    sliding windower) or ``bw_spjwin_*`` (K16, `SessionWindower`); 1 to 4 sides, and an `EventClock` with an identity
+    ``to_system_utc`` or a `SystemClock`.  Values travel as handles into a host-side dict, so they can be any Python
+    object."""
 
     insert_mode: str
     emit_mode: str
@@ -901,13 +903,23 @@ class GpuJoinWindowPlan:
 
 
 def _join_window_plan(clock, windower, side_count, insert_mode, emit_mode, ordered) -> Optional[GpuJoinWindowPlan]:
-    # product over sessions stays on the host engine: a merge concatenates the side lists (`self.state += original.state`).
+    # the plans of K8, K10 and K14; product over sessions, where a merge concatenates the side lists
+    # (`self.state += original.state`), is K16's: `_session_product_join_window_plan`.
     # A custom `to_system_utc` moves the notify time away from the event time the device compares with the system clock
     # (windowing.py:1177-1178): host engine.
     if insert_mode not in ("first", "last", "product") or not 1 <= side_count <= 4:
         return None
     windowers = (SlidingWindower, TumblingWindower) if insert_mode == "product" else (SlidingWindower, TumblingWindower, SessionWindower)
     if not isinstance(windower, windowers):
+        return None
+    if not (isinstance(clock, SystemClock) or (isinstance(clock, EventClock) and clock.to_system_utc is _identity)):
+        return None
+    return GpuJoinWindowPlan(insert_mode, emit_mode, bool(ordered), side_count, clock, windower)
+
+
+def _session_product_join_window_plan(clock, windower, side_count, insert_mode, emit_mode, ordered) -> Optional[GpuJoinWindowPlan]:
+    # product over a `SessionWindower` (K16): 1 to 4 sides; a custom `to_system_utc` stays on the host engine, as above
+    if insert_mode != "product" or not 1 <= side_count <= 4 or not isinstance(windower, SessionWindower):
         return None
     if not (isinstance(clock, SystemClock) or (isinstance(clock, EventClock) and clock.to_system_utc is _identity)):
         return None

@@ -648,8 +648,8 @@ bw_status bw_collect_eof(bw_collect* c, bw_collect_rows* out);
 typedef struct bw_sjwin bw_sjwin;
 typedef struct bw_sjwin_spec {
   uint32_t struct_size;
-  int32_t insert_mode;          /* BW_JOIN_INSERT_FIRST / LAST (product over sessions: host engine; over tumbling and
-                                   sliding windows: bw_pjwin_*, K14) */
+  int32_t insert_mode;          /* BW_JOIN_INSERT_FIRST / LAST (product over sessions: bw_spjwin_*, K16; over tumbling
+                                   and sliding windows: bw_pjwin_*, K14) */
   int32_t emit_mode;            /* BW_JOIN_EMIT_COMPLETE / FINAL / RUNNING */
   int32_t ordered;              /* 1: play values in timestamp order once the watermark passes them (the default) */
   int32_t sides;                /* 1..4 joined streams */
@@ -714,6 +714,58 @@ bw_status bw_sjwin_apply_device(bw_sjwin* j, const uint64_t* d_keys, const uint8
 bw_status bw_sjwin_advance(bw_sjwin* j, int64_t system_now_us, bw_sjwin_rows* out);
 /* End of input: every key flushes at watermark UTC_MAX (:1144-1151), so sessions with close >= UTC_MAX - gap stay open. */
 bw_status bw_sjwin_eof(bw_sjwin* j, bw_sjwin_rows* out);
+
+/* Windowed product join over session windows (K16): `join_window(insert_mode="product")` over `SessionWindower` -- K10's
+ * steps (late test, queue, ordered play, `open_for` with `_session_find_merges`, the merge queue, `close_for`, notify,
+ * EOF at UTC_MAX) with `_JoinState` keeping one list per side (operators/__init__.py:2072-2120), as K14: a value is
+ * appended to its side's list in the session `open_for` returned; "complete" emits the product once every side is
+ * non-empty and then clears every list; "running" emits the product after every value; "final" at the close.  A merge
+ * (`on_merge`, windowing.py:1879-1891) makes each of the survivor's lists its own values followed by the merged-away
+ * session's (`_JoinState.__iadd__`, operators/__init__.py:2106-2112), then "complete" / "running" act as after a value,
+ * under the survivor's id.  A product is `itertools.product` of the lists, the last side varying fastest, each list in
+ * its order, an empty list giving one None: an emission whose lists hold n_0 .. n_{sides-1} values gives
+ * prod max(1, n_s) `down` rows, expanded on the device at advance / eof.  Session state is never discarded (:798-806).
+ * One GPU only. */
+typedef struct bw_spjwin bw_spjwin;
+typedef struct bw_spjwin_spec {
+  uint32_t struct_size;
+  int32_t emit_mode;            /* BW_JOIN_EMIT_COMPLETE / FINAL / RUNNING */
+  int32_t ordered;              /* 1: play values in timestamp order once the watermark passes them (the default) */
+  int32_t sides;                /* 1..4 joined streams */
+  int32_t max_sessions_per_key; /* 1..64: sessions a key holds during a call (live ones, plus those merged away in it),
+                                   and also the merged ids its live sessions hold */
+  int32_t pad;
+  int64_t gap_us;               /* SessionWindower.gap, >= 0 (windowing.py:938-943) */
+  int64_t wait_us;              /* EventClock.wait_for_system_duration, or BW_WAIT_FOREVER */
+  uint64_t capacity_hint;       /* keys ever seen: session state is never freed (windowing.py:798-806) */
+  uint64_t max_queued_rows;     /* ordered mode: queued entries over ALL keys */
+  uint64_t max_batch_rows;
+  uint64_t max_emit_rows;       /* < 2^31: emissions (each one product), meta rows, and meta rows' merged ids, retained
+                                   between advances */
+  uint64_t max_late_rows;       /* late rows retained between bw_spjwin_advance calls */
+  uint64_t max_product_rows;    /* down rows one advance / eof may hand out (the sum of the emissions' products) */
+} bw_spjwin_spec;
+bw_status bw_spjwin_create(bw_ctx* ctx, const bw_spjwin_spec* spec, bw_spjwin** out);
+void bw_spjwin_destroy(bw_spjwin* j);
+/* One activation from HOST columns (keys, side 0..sides-1, handle, ts); blocks.  `system_now_us` as bw_sjwin_apply.  The
+ * entry store, the staging, release and output buffers grow before each call to what it can add; a full key table, more
+ * than max_sessions_per_key sessions or merged ids, a full queue, emit or late buffer, or a side list at 2^32 values
+ * returns BW_ERR_CAPACITY (reason in bw_last_error) and the join refuses further calls. */
+bw_status bw_spjwin_apply(bw_spjwin* j, const uint64_t* keys, const uint8_t* side, const uint64_t* handles, const int64_t* ts_us,
+                          uint64_t rows, uint64_t epoch, int64_t system_now_us);
+/* Same with DEVICE columns; returns once the work is enqueued (the columns must stay valid until the next call).  A side
+ * value >= sides is not played: the next call returns BW_ERR_SPEC and the join refuses further calls. */
+bw_status bw_spjwin_apply_device(bw_spjwin* j, const uint64_t* d_keys, const uint8_t* d_side, const uint64_t* d_handles,
+                                 const int64_t* d_ts_us, uint64_t rows, uint64_t epoch, int64_t system_now_us);
+/* Rows since the last call, as bw_sjwin_advance: within a key `down` rows of the inserts in play order, then of the
+ * merges in merge-queue order (under the survivor's id), then the `final` rows of the closing sessions in id order, each
+ * emission's rows in product order (down_mask bit s is set iff side s's list was non-empty); `meta` rows with the session
+ * bounds and merged ids; `late` rows (window id -1).  More than max_product_rows rows fails with BW_ERR_CAPACITY and the
+ * join refuses further calls.  Each handle is released once, in the call after which no session list and no queue entry
+ * holds it: a late item's in the call that received it, a value's in the call that cleared it or closed its session. */
+bw_status bw_spjwin_advance(bw_spjwin* j, int64_t system_now_us, bw_sjwin_rows* out);
+/* End of input: every key flushes at watermark UTC_MAX, so sessions with close >= UTC_MAX - gap stay open. */
+bw_status bw_spjwin_eof(bw_spjwin* j, bw_sjwin_rows* out);
 
 /* Collect within session windows (K12): `collect_window` (pysrc/bytewax/operators/windowing.py:1436-1576) into list /
  * set / dict over `SessionWindower` (:928-950), i.e. `_WindowLogic` (:1046-1190) over `_SessionWindowerLogic` (:671-810)
