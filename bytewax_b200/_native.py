@@ -254,6 +254,8 @@ SYMBOLS = {
     "bw_fold_reset_timers": (C.c_int32, [_P]),
     "bw_fold_sync": (C.c_int32, [_P]),
     "bw_fold_stream": (_P, [_P]),
+    "bw_fold_set_segfold_parts": (C.c_int32, [_P, C.c_uint32]),
+    "bw_fold_check_key_column": (C.c_int32, [_P, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
     "bw_fold_time_begin": (C.c_int32, [_P]),
     "bw_fold_time_end": (C.c_int32, [_P, C.POINTER(C.c_float)]),
     "bw_gen_c1": (C.c_int32, [_P, _P, _P, C.c_uint64, C.c_uint64, C.c_uint64]),

@@ -167,6 +167,8 @@ struct FoldParams {
 
 struct Table {
   HotSlot* hot;
+  u64* keys;       // dense copy of hot[].key (cap + 1): the segment fold reads a segment's keys from here, 8 B per slot
+                   // instead of a 32-byte sector; written only through bw_key_claim / bw_key_put
   P1Slot* p1;
   AuxSlot* aux;
   i64* closed_upto;  // sliding windows: window ids <= this were already emitted for this key incarnation
@@ -218,6 +220,20 @@ __host__ __device__ __forceinline__ u64 bw_slot_of_hash(u64 h, u64 cap) {
 #endif
 }
 __device__ __forceinline__ void bw_raise(Counters* c, u32 status) { atomicCAS(&c->err, 0u, status); }
+
+// The only writers of a slot's key: the hot slot's key and the dense column Table::keys change together.  A key is set
+// once (free -> key) and stays until the table is reset, so the column equals hot[].key whenever no kernel runs.
+// Claim a free slot among concurrent claimers: the old key (BW_EMPTY_KEY: the slot is now `key`'s).
+__device__ __forceinline__ u64 bw_key_claim(const Table& t, u64 s, u64 key) {
+  const u64 old = atomicCAS((unsigned long long*)&t.hot[s].key, (unsigned long long)BW_EMPTY_KEY, (unsigned long long)key);
+  if (old == BW_EMPTY_KEY) t.keys[s] = key;
+  return old;
+}
+// Set the key of a slot the caller owns alone; the caller stores `h` to hot[s].
+__device__ __forceinline__ void bw_key_put(const Table& t, HotSlot& h, u64 s, u64 key) {
+  h.key = key;
+  t.keys[s] = key;
+}
 
 // up to BW_MAX_WORLD column segments forming one activation in arrival order
 struct BatchView {

@@ -142,7 +142,7 @@ __device__ __forceinline__ u64 bw_find_slot(const Table& t, DirtySink* sk, u64 k
       return sj;
     }
     HotSlot* hs = t.hot + sj;
-    u64 old = atomicCAS((unsigned long long*)&hs->key, (unsigned long long)BW_EMPTY_KEY, (unsigned long long)key);
+    const u64 old = bw_key_claim(t, sj, key);
     if (old == BW_EMPTY_KEY) {
       // a free slot is always in the reset state; nobody else touches it before the key is set
       atomicAdd(&sk->n_new_keys, 1u);

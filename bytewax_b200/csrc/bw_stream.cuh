@@ -563,7 +563,10 @@ struct SegArgs {
                 // between (what the direct path's sub-ranges do; exact because the activation is clean)
   u32 batch_no;
   u64 epoch;
+  u32 parts;    // BW_SF_* below: the parts of the segment fold that are switched on (all, unless a measurement turns one off)
 };
+#define BW_SF_KEYCOL 1u     // read the segment's keys from the dense column (Table::keys), not from the hot slots
+#define BW_SF_ALL BW_SF_KEYCOL
 
 // One accumulator op on a shared-memory delta (32-bit shared-window address)
 template <int OP>
@@ -659,15 +662,43 @@ k_segfold(SegArgs A, Table t, FoldParams p, EmitBufs e) {
     const u64 slot_base = (u64)b << A.seg_shift;
     __syncthreads();  // the previous segment's merge is done with shared memory
     if (MODE == 1 && threadIdx.x == 0) part_n = 0u;
-    for (u32 i = threadIdx.x; i < S / 4; i += BW_SF_THREADS) {  // four slots per thread: one 32-bit word of fingerprints
-      u32 w = 0;
+    {
+      // The segment's keys from the dense column: coalesced 16-byte loads, 32 KB for 4096 slots where the hot slots'
+      // keys cost a 32-byte sector each (128 KB).  Four slots per group (one 32-bit word of fingerprints); every load
+      // of the thread is issued before its first shared-memory store (the stores are compiler barriers).  MODE 1: a
+      // source rank combines its slice from an empty segment.
+      constexpr u32 KG = (1u << BW_SEG_SHIFT_DEFAULT) / 4 / BW_SF_THREADS;  // groups per thread at the largest segment
+      u64 kv[KG][4];
 #pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        const u64 key = (MODE == 1) ? BW_EMPTY_KEY : t.hot[slot_base + 4 * i + k].key;
-        bw_sts_u64(a_key + 8 * (4 * i + k), key);
-        if (key != BW_EMPTY_KEY) w |= bw_fp_of(bw_khash(key)) << (8 * k);
+      for (u32 j = 0; j < KG; ++j) {
+        const u32 i = threadIdx.x + j * BW_SF_THREADS;
+#pragma unroll
+        for (int k = 0; k < 4; ++k) kv[j][k] = BW_EMPTY_KEY;
+        if (MODE == 1 || i >= S / 4) continue;
+        const u64 s0 = slot_base + 4 * i;
+        if (A.parts & BW_SF_KEYCOL) {
+          const ulonglong2 lo = *(const ulonglong2*)(t.keys + s0), hi = *(const ulonglong2*)(t.keys + s0 + 2);
+          kv[j][0] = lo.x;
+          kv[j][1] = lo.y;
+          kv[j][2] = hi.x;
+          kv[j][3] = hi.y;
+        } else {
+#pragma unroll
+          for (int k = 0; k < 4; ++k) kv[j][k] = t.hot[s0 + k].key;
+        }
       }
-      bw_sts_u32(a_fp + 4 * i, w);
+#pragma unroll
+      for (u32 j = 0; j < KG; ++j) {
+        const u32 i = threadIdx.x + j * BW_SF_THREADS;
+        if (i >= S / 4) continue;
+        u32 w = 0;
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          bw_sts_u64(a_key + 8 * (4 * i + k), kv[j][k]);
+          if (kv[j][k] != BW_EMPTY_KEY) w |= bw_fp_of(bw_khash(kv[j][k])) << (8 * k);
+        }
+        bw_sts_u32(a_fp + 4 * i, w);
+      }
     }
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     for (u32 pass = 0; pass < A.npass; ++pass) {
@@ -885,7 +916,7 @@ k_segfold(SegArgs A, Table t, FoldParams p, EmitBufs e) {
         HotSlot h = t.hot[s];
         if (h.key == BW_EMPTY_KEY) {
           atomicAdd(&sink.n_new_keys, 1u);
-          h.key = key;
+          bw_key_put(t, h, s, key);
         }
         const u64 dv[2] = {SO::load(a_d0 + DTB * ls), SO::load(a_d1 + DTB * ls)};
         bool touched[2];
@@ -983,6 +1014,7 @@ k_segfold(SegArgs A, Table t, FoldParams p, EmitBufs e) {
           }
           if (!range_ok) {
             bw_raise(t.ctr, 6u);
+            t.hot[s].key = h.key;  // (a key claimed above keeps its slot, with its old state: the column already has it)
             continue;
           }
           if (alive <= 1 || (alive == 2 && P[i1].q == P[i0].q - 1)) {

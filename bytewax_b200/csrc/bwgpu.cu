@@ -337,6 +337,7 @@ struct bw_fold {
   FoldParams p{};
   Table t{};
   int force_seg_shift = -1;  // env BW_SEG_SHIFT: t.seg_shift in place of BW_SEG_SHIFT_DEFAULT (-1: not set)
+  u32 segfold_parts = BW_SF_ALL;  // BW_SF_*: bw_fold_set_segfold_parts measures what each part of the segment fold is worth
   EmitBufs e{};
   Counters* d_ctr = nullptr;
   Counters* h_ctr = nullptr;  // pinned mirror
@@ -464,7 +465,7 @@ __global__ void k_init_table(Table t, u64 acc_identity) {
   const u64 n = t.cap + 1;
   for (u64 s = (u64)blockIdx.x * blockDim.x + threadIdx.x; s < n; s += (u64)gridDim.x * blockDim.x) {
     HotSlot h;
-    h.key = BW_EMPTY_KEY;
+    bw_key_put(t, h, s, BW_EMPTY_KEY);
     h.max_ts = INT64_MIN;
     h.wt0 = BW_EMPTY_WIDTAG;
     h.acc0 = acc_identity;
@@ -846,6 +847,7 @@ static bw_status fold_alloc(bw_fold* f) {
   }
   Owner& own = f->own;
   CU(ctx, own.dev(&f->t.hot, cap + 1));
+  CU(ctx, own.dev(&f->t.keys, cap + 1));
   CU(ctx, own.dev(&f->t.p1, cap + 1));
   CU(ctx, own.dev(&f->t.closed_upto, cap + 1));
   CU(ctx, own.dev(&f->t.aux, cap + 1));
@@ -1398,6 +1400,7 @@ static SegArgs seg_args(const bw_fold* f, const Deferred& d) {
   A.seg_shift = f->t.seg_shift;
   A.batch_no = d.batch_no;
   A.epoch = d.ord;
+  A.parts = f->segfold_parts;
   return A;
 }
 
@@ -2276,6 +2279,44 @@ bw_status bw_fold_sync(bw_fold* f) {
   if (!f) return BW_ERR_SPEC;
   CU(f->ctx, cudaSetDevice(f->ctx->device));
   return resolve_and_sync(f, true);
+}
+
+bw_status bw_fold_set_segfold_parts(bw_fold* f, uint32_t parts) {
+  if (!f) return BW_ERR_SPEC;
+  if (parts & ~BW_SF_ALL) FAIL(f, BW_ERR_SPEC, "bw_fold_set_segfold_parts: unknown bits 0x%x", parts & ~BW_SF_ALL);
+  f->segfold_parts = parts;
+  return BW_OK;
+}
+
+// out[0]: slots (the alias slot included) whose dense key differs from hot[].key, out[1]: slots holding a key
+__global__ void k_check_key_column(Table t, unsigned long long* out) {
+  unsigned long long bad = 0, used = 0;
+  for (u64 s = (u64)blockIdx.x * blockDim.x + threadIdx.x; s <= t.cap; s += (u64)gridDim.x * blockDim.x) {
+    const u64 k = t.hot[s].key;
+    bad += t.keys[s] != k;
+    used += k != BW_EMPTY_KEY;
+  }
+  if (bad) atomicAdd(out, bad);
+  if (used) atomicAdd(out + 1, used);
+}
+
+bw_status bw_fold_check_key_column(bw_fold* f, uint64_t* mismatches, uint64_t* keys) {
+  if (!f || !mismatches || !keys) return BW_ERR_SPEC;
+  bw_ctx* ctx = f->ctx;
+  CU(ctx, cudaSetDevice(ctx->device));
+  bw_status st = resolve_and_sync(f, true);
+  if (st != BW_OK) return st;
+  cudaStream_t s = f->s_compute;
+  if (!f->d_snap_ctr) CU(ctx, f->own.dev(&f->d_snap_ctr, 2));  // (the snapshot's two counters: free between calls)
+  CU(ctx, cudaMemsetAsync(f->d_snap_ctr, 0, 2 * sizeof(unsigned long long), s));
+  k_check_key_column<<<ctx->sm_count * 4, 256, 0, s>>>(f->t, f->d_snap_ctr);
+  CU(ctx, cudaGetLastError());
+  unsigned long long h[2];
+  CU(ctx, cudaMemcpyAsync(h, f->d_snap_ctr, sizeof h, cudaMemcpyDeviceToHost, s));
+  CU(ctx, cudaStreamSynchronize(s));
+  *mismatches = h[0];
+  *keys = h[1];
+  return BW_OK;
 }
 bw_status bw_fold_time_begin(bw_fold* f) {
   if (!f) return BW_ERR_SPEC;

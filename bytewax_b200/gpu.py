@@ -321,6 +321,16 @@ class WindowFold:
     def sync(self):
         N.check(self.lib.bw_fold_sync(self.h), self.ctx.h)
 
+    def set_segfold_parts(self, parts: int):
+        """Measurement: which parts of the segment fold run (``bw_fold_set_segfold_parts``)."""
+        N.check(self.lib.bw_fold_set_segfold_parts(self.h, parts), self.ctx.h)
+
+    def check_key_column(self) -> Tuple[int, int]:
+        """(slots whose dense key differs from the hot slot's key, slots holding a key), after the work in flight."""
+        bad, used = C.c_uint64(), C.c_uint64()
+        N.check(self.lib.bw_fold_check_key_column(self.h, C.byref(bad), C.byref(used)), self.ctx.h)
+        return bad.value, used.value
+
     def close(self):
         if self.h:
             self.lib.bw_fold_destroy(self.h)

@@ -304,6 +304,13 @@ bw_status bw_fold_time_begin(bw_fold* fold);
 bw_status bw_fold_time_end(bw_fold* fold, float* ms);
 /* cudaStream_t (as void*) that the fold / partition kernels are launched on. */
 void* bw_fold_stream(bw_fold* fold);
+/* Measurement: switch parts of the segment fold on or off (bit 1: the segment's keys are read from the dense key
+ * column instead of the hot slots; on by default).  Results do not depend on it; the activations launched from now
+ * on use it. */
+bw_status bw_fold_set_segfold_parts(bw_fold* fold, uint32_t parts);
+/* Test: after the work in flight, the slots whose dense key column entry differs from the hot slot's key, and the
+ * slots that hold a key. */
+bw_status bw_fold_check_key_column(bw_fold* fold, uint64_t* mismatches, uint64_t* keys);
 
 /* Fill device columns with SURVEY.md section 8(d) config C1 rows
  * [start, start+rows): key = splitmix64(0x5EED ^ i) mod n_keys, val = i.
