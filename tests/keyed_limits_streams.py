@@ -1,12 +1,15 @@
 """Streams that take one key of the keyed window kernels to M sessions or windows, and an instrumented run of their CPU
 oracles that measures how close each call comes.  TEST INFRASTRUCTURE ONLY.
 
-The kernels K7 (session folds), K8 (``join_window``), K9 (``collect_window``), K10 (session ``join_window``) and K11
-(``max_window`` / ``min_window`` with ``by=``) keep a key's state in a fixed array of M <= 64 records, walked by one
-thread.  What the device counts against M (DESIGN section 10):
+The kernels K7 (session folds), K8 (``join_window``), K9 (``collect_window``), K10 (session ``join_window``), K11
+(``max_window`` / ``min_window`` with ``by=``), K12 (session ``collect_window``), K14 (product ``join_window``) and K16
+(product ``join_window`` over sessions) keep a key's state in a fixed array of M <= 64 records, walked by one thread.
+What the device counts against M (DESIGN section 10):
 
 * sessions: the records a call holds -- live sessions plus the ones merged away in this call, which keep their slot
   until the call's merges are applied -- and the merged ids the live sessions hold;
+* K12 also: the merge intervals the key's sessions hold after the call's merges, before its close (a merge of B into A
+  gives A one interval and B's intervals; a chain C -> B -> A gives A two intervals and one merged id);
 * windows: the open windows, counting the ones this call opened before its close.
 
 ``measure`` runs an oracle with its windowers swapped for subclasses that count these per key and per call, without
@@ -24,15 +27,18 @@ import math
 import random
 from contextlib import contextmanager
 from dataclasses import dataclass
-from typing import List, Optional
+from typing import Dict, List, Optional
 from unittest import mock
 
 from oracle.pyoracle import SlidingWindower
 from tests import arg_window_oracle as aw
 from tests import collect_window_oracle as co
 from tests import join_window_oracle as jo
+from tests import product_join_window_oracle as po
+from tests import session_collect_oracle as sc
 from tests import session_join_oracle as sj
 from tests import session_oracle as so
+from tests import session_product_join_oracle as sp
 
 S, A = so.S, so.A
 WAIT_FOREVER = so.WAIT_FOREVER
@@ -49,9 +55,10 @@ class Call:
     """What one call of one key's logic held at its peak.  Sessions: ``records`` (live plus merged away in this call),
     ``mids`` (merged ids held by live sessions), ``dead`` (largest record index merged away, -1: none), ``merges``,
     ``tie`` (largest record index of the lower of two live sessions with the same open when they were sorted, -1:
-    none).  Windows: ``open``, ``values`` (most values played into one window so far), ``cell`` (largest cell, in K9's
-    lowest-free-cell order), ``reuse`` (largest cell given to a new window after a window on it closed in an earlier
-    call, -1: none)."""
+    none), ``ivs`` (K12's merge intervals held after the merges, before the close).  Windows: ``open``, ``values``
+    (most values played into one window so far), ``wins`` (most windows one value was played into), ``cell`` (largest
+    cell, in K9's lowest-free-cell order), ``reuse`` (largest cell given to a new window after a window on it closed in
+    an earlier call, -1: none)."""
 
     step: int
     records: int = 0
@@ -59,13 +66,25 @@ class Call:
     dead: int = -1
     merges: int = 0
     tie: int = -1
+    ivs: int = 0
     open: int = 0
     values: int = 0
+    wins: int = 0
     cell: int = -1
     reuse: int = -1
 
-    def peak(self) -> int:
-        return max(self.records, self.mids, self.open)
+    def peak(self, fields=None) -> int:
+        """The largest of the numbers a kernel counts against M (``fields``; default: records, merged ids, windows)."""
+        return max(getattr(self, f) for f in fields or COUNTED_DEFAULT)
+
+
+COUNTED_DEFAULT = ("records", "mids", "open")
+COUNTED = {"k12": ("records", "mids", "ivs")}  # only K12 keeps merge intervals
+
+
+def counted(kernel: Optional[str]):
+    """The fields of ``Call`` that ``kernel`` counts against M."""
+    return COUNTED.get(kernel, COUNTED_DEFAULT)
 
 
 class _Tracker:
@@ -104,11 +123,13 @@ class TrackedSessions(so.SessionWindower):
         self.calls: List[Call] = []
         self._cur: Optional[Call] = None
         self._rec: List[int] = []  # record order on the device: live sessions in id order, then the call's new ones
+        self._ivs: Dict[int, int] = {}  # live session id -> its merge intervals (K12)
         _active.logs.append(self.calls)
 
     def _call(self) -> Call:
         if self._cur is None:
-            self._cur = Call(_active.step, records=len(self._rec), mids=sum(len(m[2]) for m in self.sessions.values()))
+            self._cur = Call(_active.step, records=len(self._rec), mids=sum(len(m[2]) for m in self.sessions.values()),
+                             ivs=sum(self._ivs.values()))
         return self._cur
 
     def _find_merges(self) -> None:
@@ -134,8 +155,19 @@ class TrackedSessions(so.SessionWindower):
         c.records = max(c.records, len(self._rec))
         return wid
 
+    def merged(self):
+        """The merge queue, in the order the logic applies it: ``into`` takes one interval and ``orig``'s."""
+        q = super().merged()
+        for orig, into in q:
+            self._ivs[into] = self._ivs.get(into, 0) + 1 + self._ivs.pop(orig, 0)
+        c = self._call()
+        c.ivs = max(c.ivs, sum(self._ivs.values()))
+        return q
+
     def close_for(self, watermark: int):
         closed = super().close_for(watermark)
+        for wid, _ in closed:  # a closing session's intervals go with it
+            self._ivs.pop(wid, None)
         self.calls.append(self._call())
         self._cur = None
         self._rec = list(self.sessions)
@@ -169,6 +201,7 @@ class TrackedWindows(SlidingWindower):
         for wid in ids:
             self._count[wid] = self._count.get(wid, 0) + 1
             c.values = max(c.values, self._count[wid])
+        c.wins = max(c.wins, len(ids))
         c.open = max(c.open, len(self.opened))
         return ids
 
@@ -183,7 +216,8 @@ class TrackedWindows(SlidingWindower):
 
 
 RUNNERS = {"k7": so.run_sessions, "k8": jo.run_join_window, "k9": co.run_collect_window, "k10": sj.run_session_join,
-           "k11": aw.run_arg_window}
+           "k11": aw.run_arg_window, "k12": sc.run_session_collect, "k14": po.run_product_join_window,
+           "k16": sp.run_session_product_join}
 
 
 @contextmanager
@@ -192,8 +226,9 @@ def _instrumented():
     tr = _Tracker()
     _active = tr
     try:
+        # (K12's oracle imports the class by name; K14 and K16 reach theirs through K8's and K10's logic)
         with mock.patch.object(so, "SessionWindower", TrackedSessions), mock.patch.object(sj, "SessionWindower", TrackedSessions), \
-                mock.patch.object(jo, "SlidingWindower", TrackedWindows):
+                mock.patch.object(sc, "SessionWindower", TrackedSessions), mock.patch.object(jo, "SlidingWindower", TrackedWindows):
             yield tr
     finally:
         _active = None
@@ -215,9 +250,11 @@ def peak(logs, field: str) -> int:
     return max((getattr(c, field) for c in calls(logs)), default=-1)
 
 
-def first_overflow(logs, M: int) -> Optional[int]:
-    """The first step (``len(steps)``: EOF) in which a key needs more than M records, merged ids or open windows."""
-    return min((c.step for c in calls(logs) if c.peak() > M), default=None)
+def first_overflow(logs, M: int, kernel: Optional[str] = None) -> Optional[int]:
+    """The first step (``len(steps)``: EOF) in which a key needs more than M of what ``kernel`` counts: records, merged
+    ids or open windows, and for K12 merge intervals."""
+    fields = counted(kernel)
+    return min((c.step for c in calls(logs) if c.peak(fields) > M), default=None)
 
 
 # ---------------------------------------------------------------------------
@@ -354,6 +391,9 @@ def session_builders(M: int):
         "fill_over_spread": fill(M, 5, n=M + 1, calls_=3, gap=0),
         "collapse_extra1": collapse(M, 10, "asc", extra=1),
         "collapse_extra2": collapse(M, 11, "asc", extra=2),
+        # a descending chain leaves one merged id but M - 1 intervals: K12's interval limit alone
+        "collapse_desc_extra1": collapse(M, 16, "desc", extra=1),
+        "collapse_desc_extra2": collapse(M, 17, "desc", extra=2),
         "records_not_live": records_not_live(M, 20),
         "records_not_live_below": records_not_live(M, 21, below=True),
         "many_keys": many_keys(M, 30),
@@ -421,6 +461,27 @@ def sliding(M: int, seed: int, k: Optional[int] = None, more: bool = True):
     return dict(length_us=k * O, offset_us=O, align_us=A, wait_us=0), steps
 
 
+def sliding_creep(M: int, seed: int, n_calls: int = 9):
+    """Sliding windows of length M * O, offset O: every item is in M windows.  The first call puts one to three items in
+    one offset bucket, which opens M windows; each later call is a notify whose moving clock takes the watermark to the
+    next bucket's start, closing the lowest window, then one to three items in that bucket, which open one window on
+    the cell the closed one left.  The items of a call share one timestamp, and the system clock runs O ahead of it
+    (so the notify wakes the key, and with wait 0 nothing is late).  So a window's side lists fill over several calls,
+    and windows opened in different calls hold different generations: under ``complete`` a clear frees a value in some
+    of its windows while others still hold it, and the value is released only when the last of them clears or
+    closes."""
+    rnd = random.Random(seed)
+    b, steps = 100, []
+    for i in range(n_calls):
+        x = rnd.randrange(O // 2)
+        if i:
+            b += 1
+            steps.append(["notify", A + b * O + O])  # watermark: the last items' ts + (now - their arrival) = A + b O
+        items = [(A + b * O + x, None)] * rnd.randint(1, 3) + ([(A + b * O, 3)] if i == 0 else [])
+        steps.append(_batch(rnd, A + b * O + x + O, items, "i64"))
+    return dict(length_us=M * O, offset_us=O, align_us=A, wait_us=0), steps
+
+
 def window_builders(M: int):
     return {
         "tumbling_desc": tumbling(M, 40),
@@ -429,6 +490,7 @@ def window_builders(M: int):
         "tumbling_reopen": tumbling(M, 43, reopen=5),
         "sliding_full": sliding(M, 50),
         "sliding_over": sliding(M, 51, k=M + 1),
+        "sliding_creep": sliding_creep(M, 53),
         "many_keys": window_many_keys(M, 52),
     }
 
@@ -460,8 +522,9 @@ WINDOW_BUILDERS = sorted(window_builders(4))
 
 
 def for_kernel(kernel: str, clock: dict, steps, **spec):
-    """``(spec, steps)`` in ``kernel``'s oracle format.  K7 takes the values; K8 - K11 take running handles (K8 / K10:
-    side = handle mod sides; K11: the value is the by-value).  ``spec`` adds the kernel's own fields."""
+    """``(spec, steps)`` in ``kernel``'s oracle format.  K7 takes the values; the others take running handles (K8, K10,
+    K14, K16: side = handle mod sides; K11: the value is the by-value; K12: no side).  ``spec`` adds the kernel's own
+    fields."""
     spec = dict(clock, **spec)
     if kernel == "k7":
         return spec, [list(s) for s in steps]
@@ -473,7 +536,9 @@ def for_kernel(kernel: str, clock: dict, steps, **spec):
         n = len(s[2])
         hs = list(range(nxt, nxt + n))
         nxt += n
-        if kernel == "k11":
+        if kernel == "k12":
+            out.append(["batch", s[1], s[2], s[3], hs])
+        elif kernel == "k11":
             out.append(["batch", s[1], s[2], s[3], [aw.enc(v) for v in s[4]], hs])
         else:
             out.append(["batch", s[1], s[2], s[3], [h % spec.get("sides", 1) for h in hs], hs])

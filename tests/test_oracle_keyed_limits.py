@@ -18,6 +18,25 @@ def _k9(clock, steps):
     return ks.measure("k9", spec, st)
 
 
+def _spec(kernel, clock, steps, emit_mode="final", sides=2):
+    """K12: unordered; K14 / K16: unordered, ``emit_mode`` over ``sides`` sides."""
+    if kernel == "k12":
+        return ks.for_kernel("k12", clock, steps, ordered=False)
+    return ks.for_kernel(kernel, clock, steps, emit_mode=emit_mode, ordered=False, sides=sides)
+
+
+def _k12(clock, steps):
+    return ks.measure("k12", *_spec("k12", clock, steps))
+
+
+def _k14(clock, steps, **kw):
+    return ks.measure("k14", *_spec("k14", clock, steps, **kw))
+
+
+def _k16(clock, steps, **kw):
+    return ks.measure("k16", *_spec("k16", clock, steps, **kw))
+
+
 @pytest.mark.parametrize("M", ks.MS)
 def test_fill_holds_exactly_M(M):
     b = ks.session_builders(M)
@@ -129,9 +148,99 @@ def test_window_many_keys(M):
 
 @pytest.mark.parametrize("M", ks.MS)
 def test_capacity_is_the_peak(M):
-    """``first_overflow`` passes a stream at exactly its peak and fails it one below, at the call that reaches it."""
-    for clock, steps in list(ks.session_builders(M).values()) + list(ks.window_builders(M).values()):
-        logs = _k7(clock, steps) if "gap_us" in clock else _k9(clock, steps)[1]
-        top = max(c.peak() for c in ks.calls(logs))
-        assert ks.first_overflow(logs, top) is None
-        assert ks.first_overflow(logs, top - 1) == min(c.step for c in ks.calls(logs) if c.peak() == top)
+    """``first_overflow`` passes a stream at exactly its peak and fails it one below, at the call that reaches it: for
+    K7 and K9's measurements, and for K12's (which also counts merge intervals), K14's and K16's."""
+    runs = []
+    for clock, steps in ks.session_builders(M).values():
+        runs += [(None, _k7(clock, steps)), ("k12", _k12(clock, steps)[1]), ("k16", _k16(clock, steps)[1])]
+    for clock, steps in ks.window_builders(M).values():
+        runs += [(None, _k9(clock, steps)[1]), ("k14", _k14(clock, steps)[1])]
+    for kernel, logs in runs:
+        fields = ks.counted(kernel)
+        top = max(c.peak(fields) for c in ks.calls(logs))
+        assert ks.first_overflow(logs, top, kernel) is None
+        assert ks.first_overflow(logs, top - 1, kernel) == min(c.step for c in ks.calls(logs) if c.peak(fields) == top)
+
+
+# ---------------------------------------------------------------------------
+# K12 (session collect), K14 (product join over windows), K16 (product join over sessions)
+# ---------------------------------------------------------------------------
+
+
+@pytest.mark.parametrize("M", ks.MS)
+def test_collapse_desc_fills_the_intervals(M):
+    """A descending collapse chains M - 1 merges into session 0: M - 1 intervals on one merged id.  One more merge
+    makes K12's intervals exactly M, two more M + 1 -- while records and merged ids stay within M, so only K12 fails."""
+    b = ks.session_builders(M)
+    logs = _k12(*b["collapse_desc"])[1]
+    assert ks.peak(logs, "ivs") == M - 1 and ks.peak(logs, "mids") == 1
+    for name, ivs, fail in (("collapse_desc_extra1", M, None), ("collapse_desc_extra2", M + 1, 3)):
+        logs = _k12(*b[name])[1]
+        assert ks.peak(logs, "ivs") == ivs and ks.peak(logs, "mids") <= 3 and ks.peak(logs, "records") == M, name
+        assert ks.first_overflow(logs, M, "k12") == fail and ks.first_overflow(logs, M) is None, name
+        for logs in (_k7(*b[name]), _k16(*b[name])[1]):
+            assert ks.first_overflow(logs, M) is None and ks.peak(logs, "mids") < M, name
+    logs = _k12(*b["collapse_extra2"])[1]  # ascending: intervals and merged ids grow together
+    assert ks.peak(logs, "ivs") == ks.peak(logs, "mids") == M + 1 and ks.first_overflow(logs, M, "k12") == 3
+
+
+@pytest.mark.parametrize("M", ks.MS)
+@pytest.mark.parametrize("order", ks.ORDERS)
+def test_collapse_chains_in_k12_and_k16(M, order):
+    """Every collapse order gives K12 and K16 M - 1 merges in one call, with M records held; K12's intervals are the
+    merges (each merge adds one, whatever the chain)."""
+    b = ks.session_builders(M)[f"collapse_{order}"]
+    for kernel, logs in (("k12", _k12(*b)[1]), ("k16", _k16(*b)[1])):
+        hot = max(ks.calls(logs), key=lambda c: c.merges)
+        assert hot.merges == M - 1 and hot.dead == M - 1 and hot.records == M, kernel
+        assert ks.first_overflow(logs, M, kernel) is None, kernel
+    assert ks.peak(_k12(*b)[1], "ivs") == M - 1
+
+
+def _held_after_clear(acts, released):
+    """Values a ``complete`` emission cleared from one window that are released in a later call: another window still
+    held them."""
+    rel_at = {h: i for i, r in enumerate(released) for h in r}
+    return {h for i, a in enumerate(acts) for r in a if r[2] == "E" for h in r[3] if h is not None and rel_at[h] > i}
+
+
+@pytest.mark.parametrize("M", ks.MS)
+def test_sliding_creep(M):
+    """Every value goes into M windows; the key holds M open windows in every call, and each new window takes the cell
+    the closed one left (up to cell M - 1); under ``complete`` with 2 - 4 sides, clears free values in some of their
+    windows while others still hold them."""
+    clock, steps = ks.window_builders(M)["sliding_creep"]
+    for sides in (1, 2, 3, 4):
+        (acts, released), logs = _k14(clock, steps, emit_mode="complete", sides=sides)
+        assert ks.peak(logs, "wins") == M and ks.peak(logs, "open") == M and ks.first_overflow(logs, M) is None
+        assert ks.peak(logs, "cell") == M - 1 and ks.peak(logs, "reuse") >= 7
+        hot = [c for c in max(logs, key=len) if c.step < len(steps)]  # (the light key's logic wakes once, at EOF)
+        assert len(hot) == len(steps) and all(c.open == M for c in hot if steps[c.step][0] == "batch"), [c.open for c in hot]
+        if sides > 1:
+            assert len(_held_after_clear(acts, released)) >= 3, sides
+    closing = [sum(r[2] == "M" and r[0] == 7 for r in a) for a in acts]
+    assert closing[1:-1:2] == [1] * (len(steps) // 2) and not any(closing[:-1:2])  # each notify closes the hot key's lowest window
+
+
+@pytest.mark.parametrize("M", ks.MS)
+def test_k14_window_builders(M):
+    """K14 counts open windows as K9 does: the same builders reach M (and M + 1 on the ``*_over`` ones)."""
+    b = ks.window_builders(M)
+    for name in sorted(b):
+        logs9, logs14 = _k9(*b[name])[1], _k14(*b[name])[1]
+        assert ks.peak(logs14, "open") == ks.peak(logs9, "open") in (M, M + 1), name
+        assert ks.first_overflow(logs14, M) == ks.first_overflow(logs9, M), name
+
+
+@pytest.mark.parametrize("kernel", ["k12", "k14", "k16"])
+def test_instrumentation_changes_nothing(kernel):
+    """The instrumented oracle returns what the plain one does -- rows and released handles -- on every builder at
+    M = 64 and on seeded streams."""
+    streams = list(ks.session_builders(64).values()) if kernel != "k14" else list(ks.window_builders(64).values())
+    for clock, steps in streams:
+        spec, st = _spec(kernel, clock, steps)
+        assert ks.measure(kernel, spec, st)[0] == ks.RUNNERS[kernel](spec, st)
+    mod = {"k12": ks.sc, "k14": ks.po, "k16": ks.sp}[kernel]
+    for seed in list(mod.SEEDED)[:12]:
+        spec, st = mod.seeded_steps(seed)
+        assert ks.measure(kernel, spec, st)[0] == ks.RUNNERS[kernel](spec, st), seed
