@@ -225,6 +225,31 @@ __global__ void k_join_apply(JoinSlot* slots, u64 cap, u32* err, const u64* ksor
   }
 }
 
+// K6 on world > 1.  A source's rows go to their owners through the partition kernels (bw_exchange.cuh), the side
+// riding in the 8-byte ts column.  Before that, this kernel widens the side into that column and publishes the source's
+// epoch beside its row count at every owner (pub.at[d]: rank d's slot for this source), so that every owner can check
+// that all ranks play the same activation.
+struct XJoinEpochs {
+  u64* at[BW_MAX_WORLD];
+};
+__global__ void k_xjoin_side(const unsigned char* side, i64* side64, u64 n, XJoinEpochs pub, int world, u64 epoch) {
+  if (blockIdx.x == 0 && threadIdx.x < (unsigned)world) *pub.at[threadIdx.x] = epoch;
+  for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (u64)gridDim.x * blockDim.x) side64[i] = side[i] ? 1 : 0;
+}
+
+// At the owner: the received segments (bv.h_counts rows from each source) into contiguous columns in (source rank,
+// source order), the arrival order the world-1 join sees when it is fed the rank-major concatenation; side back to u8.
+__global__ void k_xjoin_gather(BatchView bv, u64 n, u64* keys, u64* vals, unsigned char* side) {
+  for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (u64)gridDim.x * blockDim.x) {
+    int r = 0;
+    u64 o = i;
+    while (o >= bv.h_counts[r]) o -= bv.h_counts[r++];
+    keys[i] = bv.keys[r][o];
+    vals[i] = ((const u64*)bv.vals[r])[o];
+    side[i] = bv.ts[r][o] ? 1 : 0;
+  }
+}
+
 __global__ void k_join_eof(JoinSlot* slots, u64 cap, u32* err, int emit_mode, JoinEmit e, u64 epoch) {
   for (u64 s = (u64)blockIdx.x * blockDim.x + threadIdx.x; s <= cap; s += (u64)gridDim.x * blockDim.x) {
     const u64 fl = slots[s].flags;

@@ -2519,14 +2519,63 @@ struct bw_join {
   u32 batch_no = 0;
   u64 min_epoch = 0, last_epoch = 0;
   bool pending = false;
+  // world > 1: this rank's receive region (JoinRegion), shared with every rank, and the source side of the exchange
+  void* xr_base = nullptr;
+  void* xr_peer[BW_MAX_WORLD] = {nullptr};  // every rank's region as seen from here
+  u64 *d_src_keys = nullptr, *d_src_vals = nullptr;
+  unsigned char* d_src_side = nullptr;
+  i64* d_src_side64 = nullptr;
+  u32* d_tile_counts = nullptr;
+  Counters* d_ctr = nullptr;  // k_part_scan's error word: never raised, a source sends at most region_cap rows
+  u32* d_word = nullptr;      // coll_barrier's word
+  u64* h_head = nullptr;      // pinned: the region's counts and epochs as received
 };
+
+// One rank's receive region for the multi-rank join: head[0][r] = rows from source r, head[1][r] = the epoch source r
+// played, then source r's keys, payloads and sides (8 bytes each, the partition's column widths) at [r * max_batch_rows].
+struct JoinRegion {
+  size_t keys_off, vals_off, side_off, total;
+};
+static JoinRegion join_region(u64 max_batch_rows, int world) {
+  const size_t col = (size_t)max_batch_rows * world * 8;
+  JoinRegion L;
+  L.keys_off = 256;  // head: 2 x BW_MAX_WORLD u64
+  L.vals_off = L.keys_off + col;
+  L.side_off = L.vals_off + col;
+  L.total = L.side_off + col;
+  return L;
+}
+
+// Receive region, source buffers and the region sharing of a join on world > 1 (collective).
+static bw_status join_ranks_setup(bw_join* j) {
+  bw_ctx* ctx = j->ctx;
+  Owner& own = j->own;
+  const u64 B = j->spec.max_batch_rows;
+  const JoinRegion L = join_region(B, ctx->world);
+  CU(ctx, own.dev(&j->xr_base, L.total));
+  CU(ctx, own.dev(&j->d_src_keys, B));
+  CU(ctx, own.dev(&j->d_src_vals, B));
+  CU(ctx, own.dev(&j->d_src_side, B));
+  CU(ctx, own.dev(&j->d_src_side64, B));
+  CU(ctx, own.dev(&j->d_tile_counts, ((B + BW_PART_TILE - 1) / BW_PART_TILE + 1) * BW_MAX_WORLD));
+  CU(ctx, own.dev(&j->d_ctr, 1));
+  CU(ctx, own.dev(&j->d_word, 1));
+  CU(ctx, own.host(&j->h_head, 2 * BW_MAX_WORLD));
+  CU(ctx, cudaMemsetAsync(j->d_ctr, 0, sizeof(Counters), j->s));
+  CU(ctx, cudaMemsetAsync(j->d_word, 0, 4, j->s));
+  CU(ctx, cudaFuncSetAttribute(k_part_scatter, cudaFuncAttributeMaxDynamicSharedMemorySize, BW_PART_TILE * 24));
+  CU(ctx, cudaStreamSynchronize(j->s));
+  return coll_share_base(ctx, j->xr_base, j->xr_peer, j->s);
+}
 
 bw_status bw_join_create(bw_ctx* ctx, const bw_join_spec* spec, bw_join** out) {
   if (!ctx || !spec || !out) CTX_FAIL(ctx, BW_ERR_SPEC, "bw_join_create: NULL argument");
   if (spec->struct_size != sizeof(bw_join_spec)) CTX_FAIL(ctx, BW_ERR_SPEC, "bw_join_spec.struct_size mismatch");
   if (spec->insert_mode < 0 || spec->insert_mode > 1) CTX_FAIL(ctx, BW_ERR_SPEC, "insert_mode must be first or last (product: host path)");
   if (spec->emit_mode < 0 || spec->emit_mode > 2) CTX_FAIL(ctx, BW_ERR_SPEC, "bad emit_mode");
-  if (spec->max_batch_rows == 0 || spec->max_batch_rows >= (1ULL << 31)) CTX_FAIL(ctx, BW_ERR_SPEC, "bad max_batch_rows");
+  // an owner groups up to max_batch_rows from every rank with 32-bit sort indices and sequence numbers
+  if (spec->max_batch_rows == 0 || spec->max_batch_rows > ((1ULL << 31) - 1) / (u64)ctx->world)
+    CTX_FAIL(ctx, BW_ERR_SPEC, "bad max_batch_rows: max_batch_rows * world must be in [1, 2^31)");
   CU(ctx, cudaSetDevice(ctx->device));
   std::unique_ptr<bw_join, void (*)(bw_join*)> jp(new bw_join(), bw_join_destroy);  // torn down on every failure
   bw_join* j = jp.get();
@@ -2542,7 +2591,8 @@ bw_status bw_join_create(bw_ctx* ctx, const bw_join_spec* spec, bw_join** out) {
   CU(ctx, cudaMemsetAsync(j->d_nrows, 0, 8, j->s));
   CU(ctx, own.host(&j->h_err, 64 / sizeof(u32)));
   CU(ctx, own.host(&j->h_nrows, 64 / sizeof(unsigned long long)));
-  const u64 n = spec->max_batch_rows, m = std::max<u64>(spec->max_emit_rows, 1024);
+  // rows one activation brings to this rank: its own on one GPU, up to max_batch_rows from every rank on world > 1
+  const u64 n = spec->max_batch_rows * (u64)ctx->world, m = std::max<u64>(spec->max_emit_rows, 1024);
   bw_status st = keyed_alloc(ctx, own, j->k, n, j->s);
   if (st != BW_OK) return st;
   CU(ctx, own.dev(&j->d_side, n));
@@ -2555,6 +2605,10 @@ bw_status bw_join_create(bw_ctx* ctx, const bw_join_spec* spec, bw_join** out) {
   k_join_init<<<ctx->sm_count * 4, 256, 0, j->s>>>(j->slots, j->cap);
   CU(ctx, cudaGetLastError());
   CU(ctx, cudaStreamSynchronize(j->s));
+  if (ctx->world > 1) {
+    st = join_ranks_setup(j);
+    if (st != BW_OK) return st;
+  }
   *out = jp.release();
   return BW_OK;
 }
@@ -2563,13 +2617,104 @@ void bw_join_destroy(bw_join* j) {
   if (!j) return;
   cudaSetDevice(j->ctx->device);
   if (j->s) cudaStreamSynchronize(j->s);
+  for (int r = 0; r < j->ctx->world; ++r)
+    if (r != j->ctx->rank && !j->ctx->loop && j->xr_peer[r]) cudaIpcCloseMemHandle(j->xr_peer[r]);
   delete j;  // j->own releases every buffer and the stream
+}
+
+// bw_join_apply on world > 1 (include/bwgpu.h): every row to its key's owner, then K6 there over what arrived.
+static bw_status join_apply_ranks(bw_join* j, const u64* keys, const uint8_t* side, const u64* vals, u64 rows, u64 epoch) {
+  bw_ctx* ctx = j->ctx;
+  const int W = ctx->world, R = ctx->rank;
+  const u64 cap = j->spec.max_batch_rows;
+  cudaStream_t s = j->s;
+  CU(ctx, cudaSetDevice(ctx->device));
+  if (rows) {
+    CU(ctx, cudaMemcpyAsync(j->d_src_keys, keys, rows * 8, cudaMemcpyHostToDevice, s));
+    CU(ctx, cudaMemcpyAsync(j->d_src_side, side, rows, cudaMemcpyHostToDevice, s));
+    CU(ctx, cudaMemcpyAsync(j->d_src_vals, vals, rows * 8, cudaMemcpyHostToDevice, s));
+  }
+  // partition + exchange straight into the owners' regions (peer stores), this source's segment at [R * cap]
+  const JoinRegion L = join_region(cap, W);
+  PartIn in;
+  in.keys = j->d_src_keys;
+  in.vals = j->d_src_vals;
+  in.ts = j->d_src_side64;
+  in.n = rows;
+  in.val_bytes = 8;
+  in.world = W;
+  PartOut po;
+  memset(&po, 0, sizeof po);
+  po.region_cap = cap;
+  XJoinEpochs pub;
+  for (int d = 0; d < W; ++d) {
+    char* base = (char*)j->xr_peer[d];
+    po.counts[d] = (u64*)base + R;
+    pub.at[d] = (u64*)base + BW_MAX_WORLD + R;
+    po.keys[d] = (u64*)(base + L.keys_off) + (size_t)R * cap;
+    po.vals[d] = (u64*)(base + L.vals_off) + (size_t)R * cap;
+    po.ts[d] = (i64*)(base + L.side_off) + (size_t)R * cap;
+  }
+  const u64 ntiles = (rows + BW_PART_TILE - 1) / BW_PART_TILE;
+  const int grid = (int)std::min<u64>(std::max<u64>(ntiles, 1), (u64)ctx->sm_count * 8);
+  k_xjoin_side<<<grid, BW_PART_THREADS, 0, s>>>(j->d_src_side, j->d_src_side64, rows, pub, W, epoch);
+  k_part_hist<<<grid, BW_PART_THREADS, 0, s>>>(in, j->d_tile_counts);
+  k_part_scan<<<W, 1024, 0, s>>>(rows, W, j->d_tile_counts, po, j->d_ctr);
+  k_part_scatter<<<grid, BW_PART_THREADS, (size_t)BW_PART_TILE * 24, s>>>(in, j->d_tile_counts, po);
+  CU(ctx, cudaGetLastError());
+  // every rank's stores are complete once it enters the barrier (stream order)
+  bw_status st = coll_barrier(ctx, j->d_word, s);
+  if (st != BW_OK) return st;
+  CU(ctx, cudaMemcpyAsync(j->h_head, j->xr_base, sizeof(u64) * 2 * BW_MAX_WORLD, cudaMemcpyDeviceToHost, s));
+  CU(ctx, cudaStreamSynchronize(s));
+  // every rank reads the same epochs: all of them raise here, or none does
+  const u64* got_epoch = j->h_head + BW_MAX_WORLD;
+  for (int r = 0; r < W; ++r)
+    if (got_epoch[r] != got_epoch[0])
+      CTX_FAIL(ctx, BW_ERR_STATE, "join: rank 0 played epoch %llu and rank %d epoch %llu; every rank must pass the same epoch to one call",
+               (unsigned long long)got_epoch[0], r, (unsigned long long)got_epoch[r]);
+  if (j->pending && epoch < j->last_epoch) CTX_FAIL(ctx, BW_ERR_STATE, "join: epochs must not decrease");
+  if (!j->pending) {
+    j->min_epoch = epoch;
+    j->pending = true;
+  }
+  j->last_epoch = epoch;
+  const u32 batch_no = j->batch_no++;
+  BatchView bv;
+  memset(&bv, 0, sizeof bv);
+  u64 n = 0;
+  for (int r = 0; r < W; ++r) {
+    const char* base = (const char*)j->xr_base;
+    bv.keys[r] = (const u64*)(base + L.keys_off) + (size_t)r * cap;
+    bv.vals[r] = (const u64*)(base + L.vals_off) + (size_t)r * cap;
+    bv.ts[r] = (const i64*)(base + L.side_off) + (size_t)r * cap;
+    bv.h_counts[r] = j->h_head[r];
+    n += j->h_head[r];
+  }
+  bv.nseg = W;
+  if (n) k_xjoin_gather<<<ctx->sm_count * 4, 256, 0, s>>>(bv, n, j->k.d_keys, j->d_vals, j->d_side);
+  CU(ctx, cudaGetLastError());
+  // Past this barrier every owner has gathered, so no source of the next call overwrites rows its owner still reads.
+  // A second barrier rather than double-buffered regions: apply already waits on the host for the received counts, so
+  // a second region set would leave nothing to overlap, and would double the 24 B x world x max_batch_rows per rank.
+  st = coll_barrier(ctx, j->d_word, s);
+  if (st != BW_OK) return st;
+  if (n) {
+    st = keyed_group(ctx, j->k, j->k.d_keys, n, s);
+    if (st != BW_OK) return st;
+    k_join_apply<<<ctx->sm_count * 8, 256, 0, s>>>(j->slots, j->cap, j->d_err, j->k.d_ksorted, j->k.d_isorted, j->k.d_head, j->d_side,
+                                                    j->d_vals, n, j->spec.insert_mode, j->spec.emit_mode, j->e, batch_no, epoch);
+    CU(ctx, cudaGetLastError());
+  }
+  CU(ctx, cudaStreamSynchronize(s));
+  return BW_OK;
 }
 
 bw_status bw_join_apply(bw_join* j, const uint64_t* keys, const uint8_t* side, const uint64_t* vals, uint64_t rows, uint64_t epoch) {
   if (!j) return BW_ERR_SPEC;
   bw_ctx* ctx = j->ctx;
   if (rows > j->spec.max_batch_rows) CTX_FAIL(ctx, BW_ERR_SPEC, "join: rows > max_batch_rows");
+  if (ctx->world > 1) return join_apply_ranks(j, keys, side, vals, rows, epoch);
   if (j->pending && epoch < j->last_epoch) CTX_FAIL(ctx, BW_ERR_STATE, "join: epochs must not decrease");
   if (!j->pending) {
     j->min_epoch = epoch;

@@ -368,7 +368,13 @@ class ZScoreMap:
 
 
 class KeyedJoin:
-    """Two-sided keyed join (``bw_join``; operators/__init__.py:2157-2190)."""
+    """Two-sided keyed join (``bw_join``; operators/__init__.py:2157-2190).
+
+    On a multi-rank context (``world > 1``) the join is sharded by key and collective: every rank creates it with the
+    same arguments and calls ``apply`` once per activation, with its own rows (possibly none) and the same epoch.  Each
+    row goes to rank ``bw_route(key, world)``, which joins what arrived in (source rank, source order); ``vals`` is an
+    opaque u64 payload that travels with its row.  A rank's ``advance`` / ``eof`` return the rows of the keys it owns.
+    Close it only once no rank calls it any more."""
 
     INSERT = {"first": 0, "last": 1}
     EMIT = {"complete": 0, "final": 1, "running": 2}

@@ -370,6 +370,19 @@ typedef struct bw_join_rows {
   const uint64_t* mask;
   const uint64_t* epoch;
 } bw_join_rows;
+/* On a context with world W > 1 the join is sharded by key:
+ *  - bw_join_create is collective (every rank calls it with the same spec).  Each rank holds a receive region of
+ *    W x max_batch_rows rows of key, payload and side, shared with every peer over peer memory (CUDA IPC mappings
+ *    under NCCL, plain pointers on a loopback world); bw_join_destroy closes the mappings, once no rank calls any more.
+ *    max_batch_rows x W must be below 2^31 (BW_ERR_SPEC).
+ *  - bw_join_apply is collective: every rank calls it once per activation with its own rows (possibly none) and the
+ *    same epoch.  Each row goes to rank bw_route(key, W), the owner the window fold uses.  The owner joins what it
+ *    received in (source rank, source order).  Ranks that pass different epochs to one call all get BW_ERR_STATE.
+ *  - vals is an opaque 64-bit payload that travels with its row.
+ *  - Rank r's bw_join_advance / bw_join_eof return the rows of the keys r owns, in the order below.  Merging every
+ *    rank's rows of one activation and stably sorting them by (epoch, key string) gives exactly the rows a world-1 join
+ *    returns when fed the rank-major concatenation of every rank's columns.
+ * A full key table or emit buffer raises on the owning rank's advance, as on one GPU. */
 bw_status bw_join_create(bw_ctx* ctx, const bw_join_spec* spec, bw_join** out);
 void bw_join_destroy(bw_join* j);
 /* One activation: items of both sides in arrival order, side[i] in {0 = left, 1 = right}; host columns. */
