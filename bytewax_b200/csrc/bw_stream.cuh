@@ -40,6 +40,8 @@
 #define BW_SC_THREADS 1024
 #define BW_SC_WARPS (BW_SC_THREADS / 32)
 #define BW_SC_TILE 2048                    // rows per scatter tile == rows per TMA stage: one 64-row chunk per warp
+#define BW_SC_CARRY 2                      // a scatter write-out ends a lane on a multiple of this many records: a 32-byte
+                                           // sector (C1 on an H100 SXM, 700 W: 0.233 ms; whole 128-byte lines, 8: 0.241)
 
 #define BW_SF_THREADS 512
 #define BW_SF_UNROLL 4
@@ -168,6 +170,7 @@ struct ScatterArgs {
   u32 world, nb_local;  // multi-GPU: bucket = owning rank * nb_local + segment of the key in the owner's table
   u32 stg_cap;       // records per bucket assembled in shared memory before they are written out (0: every record straight out)
   u32 stg_every;     // ... every this many tiles
+  u32 ovf_cap;       // rows past their bucket's staging rows held in shared memory until the write-out (beyond: straight out)
   // second run over an activation that has late rows (bw_late.cuh): rows whose bit is set are left out
   const u32* late_bits;
   u32 ts0_set;       // take ts0 from here instead of row 0 (which may be one of the late rows, far in the past)
@@ -196,9 +199,10 @@ __host__ __device__ __forceinline__ u32 bw_scatter_stage_bytes(int tsm, int vb_i
   return (u32)BW_SC_TILE * (8u + (u32)vb_in + (tsm == 0 ? 8u : 0u));
 }
 // barriers + stage-done counters | stages | per bucket: rows this block has put there (u32), rows of those already
-// written out (u32), and stg_cap records being assembled
-__host__ __device__ __forceinline__ size_t bw_scatter_smem(int tsm, int vb_in, u32 nstage, u32 nb, u32 stg_cap) {
-  return 128 + (size_t)nstage * bw_scatter_stage_bytes(tsm, vb_in) + (((size_t)nb * 8 + 15) & ~(size_t)15) + (size_t)nb * stg_cap * 16;
+// written out (u32), and stg_cap records being assembled | ovf_cap overflow rows: record, (bucket, position)
+__host__ __device__ __forceinline__ size_t bw_scatter_smem(int tsm, int vb_in, u32 nstage, u32 nb, u32 stg_cap, u32 ovf_cap) {
+  return 128 + (size_t)nstage * bw_scatter_stage_bytes(tsm, vb_in) + (((size_t)nb * 8 + 15) & ~(size_t)15) + (size_t)nb * stg_cap * 16 +
+         (size_t)ovf_cap * 24;
 }
 
 // TSM: 0 = ts column, 1 = ts from the (integer) value, 2 = none (the *_final folds).
@@ -217,7 +221,13 @@ __host__ __device__ __forceinline__ size_t bw_scatter_smem(int tsm, int vb_in, u
 // cuts every 128-byte line of the output into pieces (C1 on an H100 SXM, 700 W: 0.63 ms against 0.309 ms with 16
 // staging records per bucket).  So the records of a bucket are first assembled in shared memory,
 // stg_cap per bucket, and every stg_every tiles the block writes what it has assembled: eight lanes per bucket,
-// one 128-byte line per wavefront.  A bucket that outruns its staging rows writes those straight out.
+// one 128-byte line per wavefront.
+//
+// A write-out leaves no 32-byte sector of a lane half written: when a bucket has assembled an odd number of rows, the
+// last one stays behind as the first staging row of the next write-out (a half-written sector that L2 evicts before
+// the next write-out completes it costs HBM a read-modify-write).  Only the block's last write-out writes everything.
+// Rows that outrun their bucket's staging rows wait in a block-wide overflow area in shared memory and go out right
+// after the staged ones, in the same write-out; only when that area is full too is a row stored straight to its lane.
 template <int TSM, int VB_IN, int VB_OUT>
 __global__ void __launch_bounds__(BW_SC_THREADS, 1) k_scatter(ScatterArgs A, FoldParams p) {
   extern __shared__ __align__(128) unsigned char sc_raw[];
@@ -227,11 +237,14 @@ __global__ void __launch_bounds__(BW_SC_THREADS, 1) k_scatter(ScatterArgs A, Fol
   // lateness triples of the tiles in flight: [2 * nstage tiles][one per warp], combined by the tile's last warp
   __shared__ i64 c_min[8][BW_SC_WARPS], c_max[8][BW_SC_WARPS];
   __shared__ u32 c_bad[8][BW_SC_WARPS], c_done[8];
+  __shared__ u32 ovf_n;  // rows that went past their staging since the last write-out (more than ovf_cap: some went straight out)
   const u32 sbase = bw_smem_addr(sc_raw);
   const u32 bars = sbase, done = sbase + 64, stage0 = sbase + 128;
   const u32 lcur = stage0 + A.nstage * STAGE;  // u32[nb]: rows this block has put in each bucket
   const u32 fbase = lcur + A.nb * 4;           // u32[nb]: ... of which already written to the lane
   const u32 stg = fbase + (((A.nb * 8 + 15) & ~15u) - A.nb * 4);  // uint4[nb][stg_cap]
+  const u32 ovf_rec = stg + A.nb * A.stg_cap * 16;                // uint4[ovf_cap]
+  const u32 ovf_at = ovf_rec + A.ovf_cap * 16;                    // uint2[ovf_cap]: bucket, position in the lane
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const u64 ntiles = (A.n + T - 1) / T;
   // base of the relative timestamps: event time of row 0
@@ -260,6 +273,7 @@ __global__ void __launch_bounds__(BW_SC_THREADS, 1) k_scatter(ScatterArgs A, Fol
       bw_sts_u32(done + 4 * s, 0u);
     }
     for (int s = 0; s < 8; ++s) c_done[s] = 0u;
+    ovf_n = 0u;
     bw_mbar_fence_init();
   }
   for (u32 d = threadIdx.x; d < A.nb; d += BW_SC_THREADS) {
@@ -408,10 +422,17 @@ __global__ void __launch_bounds__(BW_SC_THREADS, 1) k_scatter(ScatterArgs A, Fol
                        : "memory");
           stored = true;
         } else if (pos < A.lane_cap) {
-          const size_t at = (size_t)(b * bucket_stride + my_lane_off + pos);
-          A.out.rec[at] = rec4;
-          if (VB_OUT == 8) ((u64*)A.out.val)[at] = x;
-          else if (VB_OUT == 4) ((u32*)A.out.val)[at] = (u32)x;
+          const u32 o = (VB_OUT == 0 && A.ovf_cap) ? atomicAdd(&ovf_n, 1u) : A.ovf_cap;
+          if (o < A.ovf_cap) {
+            asm volatile("st.shared.v4.u32 [%0], {%1,%2,%3,%4};" ::"r"(ovf_rec + 16 * o), "r"(rec4.x), "r"(rec4.y), "r"(rec4.z), "r"(rec4.w)
+                         : "memory");
+            asm volatile("st.shared.v2.u32 [%0], {%1,%2};" ::"r"(ovf_at + 8 * o), "r"(b), "r"(pos) : "memory");
+          } else {
+            const size_t at = (size_t)(b * bucket_stride + my_lane_off + pos);
+            A.out.rec[at] = rec4;
+            if (VB_OUT == 8) ((u64*)A.out.val)[at] = x;
+            else if (VB_OUT == 4) ((u32*)A.out.val)[at] = (u32)x;
+          }
           stored = true;
         }
       }
@@ -430,22 +451,56 @@ __global__ void __launch_bounds__(BW_SC_THREADS, 1) k_scatter(ScatterArgs A, Fol
     if (++ring == 2u * A.nstage) ring = 0;
     if (VB_OUT == 0 && A.stg_cap && (++since_flush == A.stg_every || it + 1 == my_tiles)) {
       since_flush = 0;
+      const bool final_out = it + 1 == my_tiles;
       __syncthreads();
+      const u32 on = ovf_n;
+      const bool ovf_all = A.ovf_cap && on <= A.ovf_cap;  // every row past its staging is in the overflow area: any can stay behind
       for (u32 bb = (u32)warp * 4; bb < A.nb; bb += BW_SC_WARPS * 4) {  // uniform trip count per warp: four buckets at a time
         const u32 b = bb + ((u32)lane >> 3);
-        u32 c = 0;
+        const u32 j = (u32)lane & 7u;
+        u32 stop = 0, keep = 0, kept = 0;  // rows [fb, stop) go out; staging rows [keep, kept) move to the front
         if (b < A.nb) {
           const u32 fb = bw_lds_u32(fbase + 4 * b);
-          c = bw_lds_u32(lcur + 4 * b);
-          const u32 nrec = min(c - fb, A.stg_cap);
-          for (u32 r = (u32)lane & 7u; r < nrec && fb + r < A.lane_cap; r += 8) {
+          const u32 c = bw_lds_u32(lcur + 4 * b);
+          stop = min(c, A.lane_cap);
+          const u32 cut = max(fb, stop & ~(BW_SC_CARRY - 1u));
+          if (!final_out && stop == c && cut < stop && stop - cut <= A.stg_cap && (stop - fb <= A.stg_cap || ovf_all)) {
+            keep = cut - fb;
+            kept = min(stop - fb, A.stg_cap);
+            stop = cut;
+          }
+          const u32 nrec = min(stop - fb, A.stg_cap);
+          for (u32 r = j; r < nrec; r += 8) {
             uint4 v;
             asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(stg + 16 * (b * A.stg_cap + r)) : "memory");
             A.out.rec[(size_t)(b * bucket_stride + my_lane_off + fb + r)] = v;
           }
         }
         __syncwarp();
-        if (b < A.nb && ((u32)lane & 7u) == 0) bw_sts_u32(fbase + 4 * b, c);
+        const bool mv = keep != 0 && keep + j < kept;  // (fewer than BW_SC_CARRY <= 8 rows stay: one per lane)
+        uint4 v;
+        if (mv)
+          asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(stg + 16 * (b * A.stg_cap + keep + j)) : "memory");
+        __syncwarp();
+        if (mv)
+          asm volatile("st.shared.v4.u32 [%0], {%1,%2,%3,%4};" ::"r"(stg + 16 * (b * A.stg_cap + j)), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
+        if (b < A.nb && j == 0) bw_sts_u32(fbase + 4 * b, stop);
+      }
+      if (on) {  // the overflow rows go out after the staged rows of the same buckets; those that stay behind move to staging
+        __syncthreads();
+        for (u32 i = threadIdx.x; i < min(on, A.ovf_cap); i += BW_SC_THREADS) {
+          uint4 v;
+          u32 b, pos;
+          asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(ovf_rec + 16 * i) : "memory");
+          asm volatile("ld.shared.v2.u32 {%0,%1}, [%2];" : "=r"(b), "=r"(pos) : "r"(ovf_at + 8 * i) : "memory");
+          const u32 fb = bw_lds_u32(fbase + 4 * b);
+          if (pos < fb)
+            A.out.rec[(size_t)(b * bucket_stride + my_lane_off + pos)] = v;
+          else
+            asm volatile("st.shared.v4.u32 [%0], {%1,%2,%3,%4};" ::"r"(stg + 16 * (b * A.stg_cap + pos - fb)), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w)
+                         : "memory");
+        }
+        if (threadIdx.x == 0) ovf_n = 0u;
       }
       __syncthreads();
     }

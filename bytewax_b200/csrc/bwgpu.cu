@@ -404,7 +404,7 @@ struct bw_fold {
   segfold_kernel_t segfold_kernel = nullptr;
   size_t segfold_smem = 0, scatter_smem = 0;
   int scatter_nstage = 3;
-  u32 last_scatter_grid = 0, scatter_stg_cap = 0, scatter_stg_every = 1;
+  u32 last_scatter_grid = 0, scatter_stg_cap = 0, scatter_stg_every = 1, scatter_ovf_cap = 0;
   // env BW_SC_STG / BW_SC_EVERY / BW_SC_STAGES: the three above, in place of what stream_alloc picks for the shape (-1: not set)
   int force_stg_cap = -1, force_stg_every = -1, force_nstage = -1;
   // multi-GPU streaming path: combine at the source, partials over NVLink, merge at the owner
@@ -745,26 +745,37 @@ static bw_status stream_alloc(bw_fold* f) {
   CU(ctx, own.dev(&sb.chunk_max, 2 * (size_t)sb.tiles_cap * BW_SC_WARPS));
   // Shared memory of the scatter: up to 16 records per bucket assembled before they are written out (counts only: the
   // value column is not staged), then as many TMA stages of the input tile (2..4) as still fit.  Deeper staging beats
-  // more stages: on C1 (489 buckets; H100 SXM, 700 W) 16 records with 2 stages take 0.309 ms, 8 records with 4 stages
-  // 0.352 ms -- fewer, longer runs of a lane's 128-byte lines written per write-out, and a third as many write-outs.
+  // more stages: on C1 (489 buckets; H100 SXM, 700 W) 16 records with 2 stages take 0.233 ms, 8 records with 4 stages
+  // 0.318 ms -- fewer, longer runs of a lane's 128-byte lines written per write-out, and a third as many write-outs.
   const size_t smem_budget = 208 * 1024;
   f->scatter_stg_cap = 0;
   if (sb.val_bytes == 0)
     for (u32 c : {16u, 8u, 6u, 4u})
-      if (bw_scatter_smem(tsm, vb_in, 2, sb.nb, c) <= smem_budget) {
+      if (bw_scatter_smem(tsm, vb_in, 2, sb.nb, c, 0) <= smem_budget) {
         f->scatter_stg_cap = c;
         break;
       }
   if (f->force_stg_cap >= 0) f->scatter_stg_cap = (u32)f->force_stg_cap;
-  // write out when an average bucket has assembled ~7/8 of its staging rows (C1 on an H100 SXM, 700 W, 16 records:
-  // every tile 0.349 ms, every 2 tiles 0.310, every 3 -- this rule's choice -- 0.309)
-  f->scatter_stg_every = (u32)std::max<double>(1.0, std::floor(0.875 * f->scatter_stg_cap * (double)sb.nb / BW_SC_TILE));
+  // write out when an average bucket has assembled ~7/8 of its staging rows, half a row of which on average is the odd
+  // row the last write-out left behind (C1 on an H100 SXM, 700 W, 16 records: every tile 0.295 ms, every 2 tiles 0.244,
+  // every 3 -- this rule's choice -- 0.233)
+  const double fill_tiles = 0.875 * std::max(0.0, f->scatter_stg_cap - 0.5) * (double)sb.nb / BW_SC_TILE;
+  f->scatter_stg_every = (u32)std::max<double>(1.0, std::floor(fill_tiles));
   if (f->force_stg_every >= 0) f->scatter_stg_every = (u32)f->force_stg_every;
   f->scatter_nstage = 4;
-  while (f->scatter_nstage > 2 && bw_scatter_smem(tsm, vb_in, f->scatter_nstage, sb.nb, f->scatter_stg_cap) > smem_budget) --f->scatter_nstage;
+  while (f->scatter_nstage > 2 && bw_scatter_smem(tsm, vb_in, f->scatter_nstage, sb.nb, f->scatter_stg_cap, 0) > smem_budget) --f->scatter_nstage;
   if (f->force_nstage >= 0) f->scatter_nstage = f->force_nstage;
-  if (bw_scatter_smem(tsm, vb_in, f->scatter_nstage, sb.nb, f->scatter_stg_cap) > 216 * 1024) return BW_OK;  // too many segments
-  f->scatter_smem = bw_scatter_smem(tsm, vb_in, f->scatter_nstage, sb.nb, f->scatter_stg_cap);
+  if (bw_scatter_smem(tsm, vb_in, f->scatter_nstage, sb.nb, f->scatter_stg_cap, 0) > 216 * 1024) return BW_OK;  // too many segments
+  // rows that outrun their bucket's staging rows wait in what the budget leaves, up to 1024 of them (C1: ~170 per
+  // write-out on average, from a Poisson count of mean 12.6 against 16 staging rows).  Not when a tile alone outruns an
+  // average bucket's staging: most rows would then pass through the area, all on one shared-memory counter (10^5 keys,
+  // 49 buckets: 0.307 ms with the area against 0.292 without, same card)
+  f->scatter_ovf_cap = 0;
+  if (f->scatter_stg_cap && fill_tiles >= 1.0) {
+    const size_t used = bw_scatter_smem(tsm, vb_in, f->scatter_nstage, sb.nb, f->scatter_stg_cap, 0);
+    if (used < smem_budget) f->scatter_ovf_cap = (u32)std::min<size_t>(1024, (smem_budget - used) / 24) & ~31u;
+  }
+  f->scatter_smem = bw_scatter_smem(tsm, vb_in, f->scatter_nstage, sb.nb, f->scatter_stg_cap, f->scatter_ovf_cap);
   // the attribute belongs to the kernel, not to this fold: folds with other table sizes share it
   CU(ctx, cudaFuncSetAttribute((const void*)f->scatter_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 216 * 1024));
   int occ = 0;
@@ -1338,6 +1349,7 @@ static bw_status stream_front(bw_fold* f, const u64* d_keys, const void* d_vals,
   A.rec_idx = f->p.seq_by_id ? 0u : 1u;
   A.stg_cap = f->scatter_stg_cap;
   A.stg_every = f->scatter_stg_every;
+  A.ovf_cap = f->scatter_ovf_cap;
   A.batch_no = batch_no;
   A.world = (u32)ctx->world;
   A.nb_local = f->nb_local;
