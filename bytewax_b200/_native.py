@@ -94,7 +94,7 @@ class BwJoinRows(C.Structure):
 class BwSessionSpec(C.Structure):
     _fields_ = [("struct_size", C.c_uint32), ("reduction", C.c_int32), ("val_dtype", C.c_int32), ("max_sessions_per_key", C.c_int32),
                 ("gap_us", C.c_int64), ("wait_us", C.c_int64), ("capacity_hint", C.c_uint64), ("max_batch_rows", C.c_uint64),
-                ("max_emit_rows", C.c_uint64), ("max_late_rows", C.c_uint64)]
+                ("max_emit_rows", C.c_uint64), ("max_late_rows", C.c_uint64), ("shard_by_key", C.c_int32), ("reserved", C.c_int32)]
 
 
 class BwSessionRows(C.Structure):
@@ -103,7 +103,8 @@ class BwSessionRows(C.Structure):
                 ("closed_close_us", C.POINTER(C.c_int64)), ("closed_epoch", C.POINTER(C.c_uint64)),
                 ("merged_off", C.POINTER(C.c_uint64)), ("merged_ids", C.POINTER(C.c_int64)),
                 ("n_late", C.c_uint64), ("late_key", C.POINTER(C.c_uint64)), ("late_epoch", C.POINTER(C.c_uint64)),
-                ("late_activation", C.POINTER(C.c_uint64)), ("late_row", C.POINTER(C.c_uint64))]
+                ("late_activation", C.POINTER(C.c_uint64)), ("late_row", C.POINTER(C.c_uint64)),
+                ("late_rank", C.POINTER(C.c_uint64))]
 
 
 class BwJwinSpec(C.Structure):

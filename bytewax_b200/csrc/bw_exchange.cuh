@@ -37,6 +37,7 @@ struct PartOut {
   i64* ts[BW_MAX_WORLD];
   u64* counts[BW_MAX_WORLD];  // where to publish "rows from this rank" at destination d
   u64 region_cap;
+  u32* rows[BW_MAX_WORLD];    // k_part_scatter<true>: each row's index in this rank's columns
 };
 
 __device__ __forceinline__ u32 bw_dest_of(u64 key, int world) { return bw_route_hash(bw_mix64(key), (u32)world); }
@@ -113,6 +114,9 @@ __global__ void __launch_bounds__(1024) k_part_scan(u64 n, int world, u32* tile_
 // whole block with consecutive lanes on consecutive addresses.  Peer (NVLink) stores
 // therefore arrive as long contiguous runs (2-8 KB per destination per tile) instead of
 // warp-sized fragments -- the fragmented version reached ~200 GB/s over NVLink.
+// SRC_ROW adds a fourth column, each row's index i in the source columns (u32), for an owner that must name the rows it
+// received (K7 on N ranks); the dynamic shared memory then grows from BW_PART_TILE x 24 to BW_PART_TILE x 28 bytes.
+template <bool SRC_ROW>
 __global__ void __launch_bounds__(BW_PART_THREADS)
 k_part_scatter(PartIn in, const u32* tile_off, PartOut out) {
   // [iteration][warp][dest] counts, scanned in (iteration, warp) order per dest
@@ -122,6 +126,7 @@ k_part_scatter(PartIn in, const u32* tile_off, PartOut out) {
   u64* s_keys = (u64*)stage_raw;
   unsigned char* s_vals = stage_raw + (size_t)BW_PART_TILE * 8;
   i64* s_ts = (i64*)(s_vals + (size_t)BW_PART_TILE * (in.val_bytes ? in.val_bytes : 0));
+  u32* s_row = (u32*)(s_ts + (in.ts ? BW_PART_TILE : 0));
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const u32 lt = (1u << lane) - 1u;
   const u64 ntiles = (in.n + BW_PART_TILE - 1) / BW_PART_TILE;
@@ -185,6 +190,7 @@ k_part_scatter(PartIn in, const u32* tile_off, PartOut out) {
           ((u32*)s_vals)[lp] = bw_ld_stream_u32((const u32*)in.vals + i);
         }
         if (in.ts) s_ts[lp] = (i64)bw_ld_stream_u64((const u64*)in.ts + i);
+        if (SRC_ROW) s_row[lp] = (u32)i;
       }
     }
     __syncthreads();
@@ -205,7 +211,31 @@ k_part_scatter(PartIn in, const u32* tile_off, PartOut out) {
         i64* gt = out.ts[d] + g0;
         for (u32 e = threadIdx.x; e < n_d; e += BW_PART_THREADS) gt[e] = s_ts[s0 + e];
       }
+      if (SRC_ROW) {
+        u32* gr = out.rows[d] + g0;
+        for (u32 e = threadIdx.x; e < n_d; e += BW_PART_THREADS) gr[e] = s_row[s0 + e];
+      }
     }
     __syncthreads();
+  }
+}
+// Instantiated here, before any kernel that declares its dynamic shared memory with a stricter alignment (bw_stream.cuh
+// asks for 128 bytes): instantiated at the end of the translation unit, the staging would start at that alignment too.
+template __global__ void k_part_scatter<false>(PartIn, const u32*, PartOut);
+template __global__ void k_part_scatter<true>(PartIn, const u32*, PartOut);
+
+// Keyed kernels on N ranks (K6, K7; RankXchg in bwgpu.cu): what a source publishes beside its row count in every owner's
+// region head, so that every owner can check that all ranks play the same call.  at[d] is this source's column in rank
+// d's head; rows 1-3 of the head take the epoch, the system time and the refusal flag (row 0, the count, is
+// k_part_scan's).
+struct XchgHead {
+  u64* at[BW_MAX_WORLD];
+};
+__global__ void k_xchg_head(XchgHead pub, int world, u64 epoch, i64 now, u64 refused) {
+  if (threadIdx.x < (unsigned)world) {
+    u64* h = pub.at[threadIdx.x];
+    h[BW_MAX_WORLD] = epoch;
+    h[2 * BW_MAX_WORLD] = (u64)now;
+    h[3 * BW_MAX_WORLD] = refused;
   }
 }

@@ -226,14 +226,8 @@ __global__ void k_join_apply(JoinSlot* slots, u64 cap, u32* err, const u64* ksor
 }
 
 // K6 on world > 1.  A source's rows go to their owners through the partition kernels (bw_exchange.cuh), the side
-// riding in the 8-byte ts column.  Before that, this kernel widens the side into that column and publishes the source's
-// epoch beside its row count at every owner (pub.at[d]: rank d's slot for this source), so that every owner can check
-// that all ranks play the same activation.
-struct XJoinEpochs {
-  u64* at[BW_MAX_WORLD];
-};
-__global__ void k_xjoin_side(const unsigned char* side, i64* side64, u64 n, XJoinEpochs pub, int world, u64 epoch) {
-  if (blockIdx.x == 0 && threadIdx.x < (unsigned)world) *pub.at[threadIdx.x] = epoch;
+// riding in the 8-byte ts column: this kernel widens it into that column first.
+__global__ void k_xjoin_side(const unsigned char* side, i64* side64, u64 n) {
   for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (u64)gridDim.x * blockDim.x) side64[i] = side[i] ? 1 : 0;
 }
 

@@ -448,6 +448,30 @@ __global__ void k_session_apply(SessTable t, SessEmit e, SessParams p, const u64
   }
 }
 
+// K7 on world > 1, at the owner: the received segments (bv.h_counts rows from each source) into K7's columns in (source
+// rank, source order), the arrival order a world-1 fold sees when it is fed the rank-major concatenation.  name[i] =
+// source rank << 32 | the row's index in that source's columns (src_row: the region's row column, `cap` rows per source).
+// vals is NULL for count, which sends none.
+__global__ void k_xsess_gather(BatchView bv, const u32* src_row, u64 cap, u64 n, u64* keys, u64* vals, i64* ts, u64* name) {
+  for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (u64)gridDim.x * blockDim.x) {
+    int r = 0;
+    u64 o = i;
+    while (o >= bv.h_counts[r]) o -= bv.h_counts[r++];
+    keys[i] = bv.keys[r][o];
+    if (vals) vals[i] = ((const u64*)bv.vals[r])[o];
+    ts[i] = bv.ts[r][o];
+    name[i] = (u64)r << 32 | src_row[(u64)r * cap + o];
+  }
+}
+
+// After k_session_apply on world > 1: the late rows this call added, [*before, min(*n_late, max_late)), hold positions in
+// the gathered columns; give them their rows' names instead.  Names grow with the position, so arrival order holds.
+__global__ void k_xsess_name_late(const unsigned long long* before, const unsigned long long* n_late, u64 max_late, u64* l_row,
+                                  const u64* name) {
+  const u64 hi = *n_late < max_late ? *n_late : max_late;
+  for (u64 i = *before + (u64)blockIdx.x * blockDim.x + threadIdx.x; i < hi; i += (u64)gridDim.x * blockDim.x) l_row[i] = name[l_row[i]];
+}
+
 // notify phase (src/operators.rs:808-858): a key is due when min(close) + gap <= now (`notify_at`, windowing.py:790-796,
 // identity `to_system_utc`); it closes what its watermark at `now` allows (`on_notify`, :1135-1142, :289-298).
 // eof (src/operators.rs:862-894, windowing.py:1144-1151): every key, watermark UTC_MAX.

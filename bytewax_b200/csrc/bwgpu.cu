@@ -958,7 +958,7 @@ static bw_status xchg_setup(bw_fold* f) {
   Owner& own = f->own;
   CU(ctx, own.dev(&f->xchg_base, L.total));
   CU(ctx, cudaMemset(f->xchg_base, 0, L.total));
-  CU(ctx, cudaFuncSetAttribute(k_part_scatter, cudaFuncAttributeMaxDynamicSharedMemorySize, BW_PART_TILE * 24));
+  CU(ctx, cudaFuncSetAttribute(k_part_scatter<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, BW_PART_TILE * 24));
   u64 ntiles = (f->spec.max_batch_rows + BW_PART_TILE - 1) / BW_PART_TILE + 1;
   CU(ctx, own.dev(&f->d_tile_counts, ntiles * BW_MAX_WORLD));
   if (f->spec.exchange == BW_XCHG_P2P) {
@@ -1207,7 +1207,7 @@ static bw_status exchange(bw_fold* f, const u64* d_keys, const void* d_vals, con
   k_part_hist<<<grid, BW_PART_THREADS, 0, s>>>(in, f->d_tile_counts);
   k_part_scan<<<W, 1024, 0, s>>>(rows, W, f->d_tile_counts, po, f->d_ctr);
   const size_t stage_bytes = (size_t)BW_PART_TILE * (8 + (size_t)in.val_bytes + (in.ts ? 8 : 0));
-  k_part_scatter<<<grid, BW_PART_THREADS, stage_bytes, s>>>(in, f->d_tile_counts, po);
+  k_part_scatter<false><<<grid, BW_PART_THREADS, stage_bytes, s>>>(in, f->d_tile_counts, po);
   CU(ctx, cudaGetLastError());
   f->st.kernel_launches += 3;
   char* mine = (char*)f->xchg_base;
@@ -2513,6 +2513,105 @@ bw_status bw_smap_apply(bw_smap* m, const uint64_t* keys, const void* vals, uint
   return bw_smap_sync(m);
 }
 
+// ---- keyed kernels on N ranks (K6, K7): every row to its key's owner ----
+// One rank's receive region: a 256-byte head of four rows of BW_MAX_WORLD u64 -- per source rank r: the rows r sent
+// here, the epoch, the system time and the refusal flag r published (k_xchg_head) -- then source r's keys, values and ts
+// (8 bytes each, the partition's column widths) and, with source rows, its rows' indices (4 bytes) at [r * cap].
+// Setup is collective: the region is shared with every rank (coll_share_base).  A call is collective too: send()
+// publishes the head, partitions the source's columns straight into the owners' regions (peer stores), enters a barrier
+// and reads the head; the caller checks it and gathers what arrived, then done() enters a second barrier, past which no
+// source of the next call overwrites rows an owner still reads.  A second barrier rather than double-buffered regions:
+// a call already waits on the host for the received counts, so a second region set would leave nothing to overlap and
+// would double the region.
+struct RankXchg {
+  u64 cap = 0;       // rows per source: max_batch_rows
+  bool src_rows = false;
+  size_t keys_off = 0, vals_off = 0, ts_off = 0, rows_off = 0, total = 0;
+  void* base = nullptr;
+  void* peer[BW_MAX_WORLD] = {nullptr};  // every rank's region as seen from here
+  u32* d_tile_counts = nullptr;
+  Counters* d_ctr = nullptr;  // k_part_scan's error word: never raised, a source sends at most `cap` rows
+  u32* d_word = nullptr;      // coll_barrier's word
+  u64* h_head = nullptr;      // pinned: the head as received
+
+  bw_status setup(bw_ctx* ctx, Owner& own, u64 max_batch_rows, bool with_src_rows, cudaStream_t s) {
+    cap = max_batch_rows;
+    src_rows = with_src_rows;
+    const size_t col = (size_t)cap * ctx->world;
+    keys_off = 4 * BW_MAX_WORLD * sizeof(u64);
+    vals_off = keys_off + col * 8;
+    ts_off = vals_off + col * 8;
+    rows_off = ts_off + col * 8;
+    total = rows_off + (src_rows ? col * 4 : 0);
+    CU(ctx, own.dev(&base, total));
+    CU(ctx, own.dev(&d_tile_counts, ((cap + BW_PART_TILE - 1) / BW_PART_TILE + 1) * BW_MAX_WORLD));
+    CU(ctx, own.dev(&d_ctr, 1));
+    CU(ctx, own.dev(&d_word, 1));
+    CU(ctx, own.host(&h_head, 4 * BW_MAX_WORLD));
+    CU(ctx, cudaMemsetAsync(d_ctr, 0, sizeof(Counters), s));
+    CU(ctx, cudaMemsetAsync(d_word, 0, 4, s));
+    CU(ctx, cudaFuncSetAttribute(src_rows ? k_part_scatter<true> : k_part_scatter<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 BW_PART_TILE * (src_rows ? 28 : 24)));
+    CU(ctx, cudaStreamSynchronize(s));
+    return coll_share_base(ctx, base, peer, s);
+  }
+  // closes the IPC mappings; the caller's Owner frees the rest
+  void close(bw_ctx* ctx) {
+    for (int r = 0; r < ctx->world; ++r)
+      if (r != ctx->rank && !ctx->loop && peer[r]) cudaIpcCloseMemHandle(peer[r]);
+  }
+  // head row `row` (0 rows, 1 epoch, 2 system time, 3 refusal flag), one entry per source rank
+  const u64* head(int row) const { return h_head + row * BW_MAX_WORLD; }
+  bw_status send(bw_ctx* ctx, cudaStream_t s, const PartIn& in, u64 epoch, i64 now, bool refused) {
+    const int W = ctx->world, R = ctx->rank;
+    PartOut po;
+    memset(&po, 0, sizeof po);
+    po.region_cap = cap;
+    XchgHead pub;
+    for (int d = 0; d < W; ++d) {
+      char* b = (char*)peer[d];
+      po.counts[d] = (u64*)b + R;
+      pub.at[d] = (u64*)b + R;
+      po.keys[d] = (u64*)(b + keys_off) + (size_t)R * cap;
+      po.vals[d] = (u64*)(b + vals_off) + (size_t)R * cap;
+      po.ts[d] = (i64*)(b + ts_off) + (size_t)R * cap;
+      if (src_rows) po.rows[d] = (u32*)(b + rows_off) + (size_t)R * cap;
+    }
+    const u64 ntiles = (in.n + BW_PART_TILE - 1) / BW_PART_TILE;
+    const int grid = (int)std::min<u64>(std::max<u64>(ntiles, 1), (u64)ctx->sm_count * 8);
+    const size_t stage = (size_t)BW_PART_TILE * (8 + in.val_bytes + (in.ts ? 8 : 0) + (src_rows ? 4 : 0));
+    k_xchg_head<<<1, 32, 0, s>>>(pub, W, epoch, now, refused ? 1 : 0);
+    k_part_hist<<<grid, BW_PART_THREADS, 0, s>>>(in, d_tile_counts);
+    k_part_scan<<<W, 1024, 0, s>>>(in.n, W, d_tile_counts, po, d_ctr);
+    if (src_rows) k_part_scatter<true><<<grid, BW_PART_THREADS, stage, s>>>(in, d_tile_counts, po);
+    else k_part_scatter<false><<<grid, BW_PART_THREADS, stage, s>>>(in, d_tile_counts, po);
+    CU(ctx, cudaGetLastError());
+    // every rank's stores are complete once it enters the barrier (stream order)
+    bw_status st = coll_barrier(ctx, d_word, s);
+    if (st != BW_OK) return st;
+    CU(ctx, cudaMemcpyAsync(h_head, base, sizeof(u64) * 4 * BW_MAX_WORLD, cudaMemcpyDeviceToHost, s));
+    CU(ctx, cudaStreamSynchronize(s));
+    return BW_OK;
+  }
+  // the received segments, in source rank order; returns the rows in all of them
+  u64 received(bw_ctx* ctx, BatchView& bv) const {
+    memset(&bv, 0, sizeof bv);
+    u64 n = 0;
+    for (int r = 0; r < ctx->world; ++r) {
+      const char* b = (const char*)base;
+      bv.keys[r] = (const u64*)(b + keys_off) + (size_t)r * cap;
+      bv.vals[r] = (const u64*)(b + vals_off) + (size_t)r * cap;
+      bv.ts[r] = (const i64*)(b + ts_off) + (size_t)r * cap;
+      bv.h_counts[r] = h_head[r];
+      n += h_head[r];
+    }
+    bv.nseg = ctx->world;
+    return n;
+  }
+  const u32* rows() const { return (const u32*)((const char*)base + rows_off); }
+  bw_status done(bw_ctx* ctx, cudaStream_t s) { return coll_barrier(ctx, d_word, s); }
+};
+
 struct bw_join {
   Owner own;  // every buffer and the stream below
   bw_ctx* ctx = nullptr;
@@ -2531,53 +2630,23 @@ struct bw_join {
   u32 batch_no = 0;
   u64 min_epoch = 0, last_epoch = 0;
   bool pending = false;
-  // world > 1: this rank's receive region (JoinRegion), shared with every rank, and the source side of the exchange
-  void* xr_base = nullptr;
-  void* xr_peer[BW_MAX_WORLD] = {nullptr};  // every rank's region as seen from here
+  // world > 1: the exchange, and the source columns it sends
+  RankXchg x;
   u64 *d_src_keys = nullptr, *d_src_vals = nullptr;
   unsigned char* d_src_side = nullptr;
   i64* d_src_side64 = nullptr;
-  u32* d_tile_counts = nullptr;
-  Counters* d_ctr = nullptr;  // k_part_scan's error word: never raised, a source sends at most region_cap rows
-  u32* d_word = nullptr;      // coll_barrier's word
-  u64* h_head = nullptr;      // pinned: the region's counts and epochs as received
 };
 
-// One rank's receive region for the multi-rank join: head[0][r] = rows from source r, head[1][r] = the epoch source r
-// played, then source r's keys, payloads and sides (8 bytes each, the partition's column widths) at [r * max_batch_rows].
-struct JoinRegion {
-  size_t keys_off, vals_off, side_off, total;
-};
-static JoinRegion join_region(u64 max_batch_rows, int world) {
-  const size_t col = (size_t)max_batch_rows * world * 8;
-  JoinRegion L;
-  L.keys_off = 256;  // head: 2 x BW_MAX_WORLD u64
-  L.vals_off = L.keys_off + col;
-  L.side_off = L.vals_off + col;
-  L.total = L.side_off + col;
-  return L;
-}
-
-// Receive region, source buffers and the region sharing of a join on world > 1 (collective).
+// Source buffers and the exchange of a join on world > 1 (collective): the side rides in the 8-byte ts column.
 static bw_status join_ranks_setup(bw_join* j) {
   bw_ctx* ctx = j->ctx;
   Owner& own = j->own;
   const u64 B = j->spec.max_batch_rows;
-  const JoinRegion L = join_region(B, ctx->world);
-  CU(ctx, own.dev(&j->xr_base, L.total));
   CU(ctx, own.dev(&j->d_src_keys, B));
   CU(ctx, own.dev(&j->d_src_vals, B));
   CU(ctx, own.dev(&j->d_src_side, B));
   CU(ctx, own.dev(&j->d_src_side64, B));
-  CU(ctx, own.dev(&j->d_tile_counts, ((B + BW_PART_TILE - 1) / BW_PART_TILE + 1) * BW_MAX_WORLD));
-  CU(ctx, own.dev(&j->d_ctr, 1));
-  CU(ctx, own.dev(&j->d_word, 1));
-  CU(ctx, own.host(&j->h_head, 2 * BW_MAX_WORLD));
-  CU(ctx, cudaMemsetAsync(j->d_ctr, 0, sizeof(Counters), j->s));
-  CU(ctx, cudaMemsetAsync(j->d_word, 0, 4, j->s));
-  CU(ctx, cudaFuncSetAttribute(k_part_scatter, cudaFuncAttributeMaxDynamicSharedMemorySize, BW_PART_TILE * 24));
-  CU(ctx, cudaStreamSynchronize(j->s));
-  return coll_share_base(ctx, j->xr_base, j->xr_peer, j->s);
+  return j->x.setup(ctx, own, B, false, j->s);
 }
 
 bw_status bw_join_create(bw_ctx* ctx, const bw_join_spec* spec, bw_join** out) {
@@ -2629,16 +2698,14 @@ void bw_join_destroy(bw_join* j) {
   if (!j) return;
   cudaSetDevice(j->ctx->device);
   if (j->s) cudaStreamSynchronize(j->s);
-  for (int r = 0; r < j->ctx->world; ++r)
-    if (r != j->ctx->rank && !j->ctx->loop && j->xr_peer[r]) cudaIpcCloseMemHandle(j->xr_peer[r]);
+  j->x.close(j->ctx);
   delete j;  // j->own releases every buffer and the stream
 }
 
 // bw_join_apply on world > 1 (include/bwgpu.h): every row to its key's owner, then K6 there over what arrived.
 static bw_status join_apply_ranks(bw_join* j, const u64* keys, const uint8_t* side, const u64* vals, u64 rows, u64 epoch) {
   bw_ctx* ctx = j->ctx;
-  const int W = ctx->world, R = ctx->rank;
-  const u64 cap = j->spec.max_batch_rows;
+  const int W = ctx->world;
   cudaStream_t s = j->s;
   CU(ctx, cudaSetDevice(ctx->device));
   if (rows) {
@@ -2646,8 +2713,6 @@ static bw_status join_apply_ranks(bw_join* j, const u64* keys, const uint8_t* si
     CU(ctx, cudaMemcpyAsync(j->d_src_side, side, rows, cudaMemcpyHostToDevice, s));
     CU(ctx, cudaMemcpyAsync(j->d_src_vals, vals, rows * 8, cudaMemcpyHostToDevice, s));
   }
-  // partition + exchange straight into the owners' regions (peer stores), this source's segment at [R * cap]
-  const JoinRegion L = join_region(cap, W);
   PartIn in;
   in.keys = j->d_src_keys;
   in.vals = j->d_src_vals;
@@ -2655,32 +2720,12 @@ static bw_status join_apply_ranks(bw_join* j, const u64* keys, const uint8_t* si
   in.n = rows;
   in.val_bytes = 8;
   in.world = W;
-  PartOut po;
-  memset(&po, 0, sizeof po);
-  po.region_cap = cap;
-  XJoinEpochs pub;
-  for (int d = 0; d < W; ++d) {
-    char* base = (char*)j->xr_peer[d];
-    po.counts[d] = (u64*)base + R;
-    pub.at[d] = (u64*)base + BW_MAX_WORLD + R;
-    po.keys[d] = (u64*)(base + L.keys_off) + (size_t)R * cap;
-    po.vals[d] = (u64*)(base + L.vals_off) + (size_t)R * cap;
-    po.ts[d] = (i64*)(base + L.side_off) + (size_t)R * cap;
-  }
-  const u64 ntiles = (rows + BW_PART_TILE - 1) / BW_PART_TILE;
-  const int grid = (int)std::min<u64>(std::max<u64>(ntiles, 1), (u64)ctx->sm_count * 8);
-  k_xjoin_side<<<grid, BW_PART_THREADS, 0, s>>>(j->d_src_side, j->d_src_side64, rows, pub, W, epoch);
-  k_part_hist<<<grid, BW_PART_THREADS, 0, s>>>(in, j->d_tile_counts);
-  k_part_scan<<<W, 1024, 0, s>>>(rows, W, j->d_tile_counts, po, j->d_ctr);
-  k_part_scatter<<<grid, BW_PART_THREADS, (size_t)BW_PART_TILE * 24, s>>>(in, j->d_tile_counts, po);
-  CU(ctx, cudaGetLastError());
-  // every rank's stores are complete once it enters the barrier (stream order)
-  bw_status st = coll_barrier(ctx, j->d_word, s);
+  const int grid = (int)std::min<u64>(std::max<u64>((rows + BW_PART_TILE - 1) / BW_PART_TILE, 1), (u64)ctx->sm_count * 8);
+  k_xjoin_side<<<grid, BW_PART_THREADS, 0, s>>>(j->d_src_side, j->d_src_side64, rows);
+  bw_status st = j->x.send(ctx, s, in, epoch, 0, false);
   if (st != BW_OK) return st;
-  CU(ctx, cudaMemcpyAsync(j->h_head, j->xr_base, sizeof(u64) * 2 * BW_MAX_WORLD, cudaMemcpyDeviceToHost, s));
-  CU(ctx, cudaStreamSynchronize(s));
   // every rank reads the same epochs: all of them raise here, or none does
-  const u64* got_epoch = j->h_head + BW_MAX_WORLD;
+  const u64* got_epoch = j->x.head(1);
   for (int r = 0; r < W; ++r)
     if (got_epoch[r] != got_epoch[0])
       CTX_FAIL(ctx, BW_ERR_STATE, "join: rank 0 played epoch %llu and rank %d epoch %llu; every rank must pass the same epoch to one call",
@@ -2693,23 +2738,10 @@ static bw_status join_apply_ranks(bw_join* j, const u64* keys, const uint8_t* si
   j->last_epoch = epoch;
   const u32 batch_no = j->batch_no++;
   BatchView bv;
-  memset(&bv, 0, sizeof bv);
-  u64 n = 0;
-  for (int r = 0; r < W; ++r) {
-    const char* base = (const char*)j->xr_base;
-    bv.keys[r] = (const u64*)(base + L.keys_off) + (size_t)r * cap;
-    bv.vals[r] = (const u64*)(base + L.vals_off) + (size_t)r * cap;
-    bv.ts[r] = (const i64*)(base + L.side_off) + (size_t)r * cap;
-    bv.h_counts[r] = j->h_head[r];
-    n += j->h_head[r];
-  }
-  bv.nseg = W;
+  const u64 n = j->x.received(ctx, bv);
   if (n) k_xjoin_gather<<<ctx->sm_count * 4, 256, 0, s>>>(bv, n, j->k.d_keys, j->d_vals, j->d_side);
   CU(ctx, cudaGetLastError());
-  // Past this barrier every owner has gathered, so no source of the next call overwrites rows its owner still reads.
-  // A second barrier rather than double-buffered regions: apply already waits on the host for the received counts, so
-  // a second region set would leave nothing to overlap, and would double the 24 B x world x max_batch_rows per rank.
-  st = coll_barrier(ctx, j->d_word, s);
+  st = j->x.done(ctx, s);
   if (st != BW_OK) return st;
   if (n) {
     st = keyed_group(ctx, j->k, j->k.d_keys, n, s);
@@ -2818,7 +2850,7 @@ struct bw_session {
   SessEmit e{};
   SortScratch srt;  // ordering scratch
   HostCols hc[2];   // closed: key, window id, acc, open, close | epoch, merged count, merged offset
-  HostCols hl;      // late: key, epoch, activation, row
+  HostCols hl;      // late: key, epoch, activation, row, source rank
   i64* h_mids = nullptr;
   std::vector<u64> merged_off;
   std::vector<i64> merged_ids;
@@ -2827,19 +2859,32 @@ struct bw_session {
   u64 last_epoch = 0;
   i64 now = INT64_MIN;
   bool failed = false;
+  // world > 1: the exchange (with source rows), each gathered row's name (source rank << 32 | source row), and the late
+  // row count before a fold
+  RankXchg x;
+  u64* d_name = nullptr;
+  unsigned long long* d_late0 = nullptr;
 };
 
-bw_status bw_session_create(bw_ctx* ctx, const bw_session_spec* spec, bw_session** out) {
-  if (!ctx || !spec || !out) CTX_FAIL(ctx, BW_ERR_SPEC, "bw_session_create: NULL argument");
-  if (spec->struct_size != sizeof(bw_session_spec)) CTX_FAIL(ctx, BW_ERR_SPEC, "bw_session_spec.struct_size mismatch");
-  if (ctx->world != 1) CTX_FAIL(ctx, BW_ERR_SPEC, "session folds run on one GPU (world == 1)");
+bw_status bw_session_create(bw_ctx* ctx, const bw_session_spec* user, bw_session** out) {
+  if (!ctx || !user || !out) CTX_FAIL(ctx, BW_ERR_SPEC, "bw_session_create: NULL argument");
+  // a spec built against the header before shard_by_key existed ends just before it, and leaves it 0
+  if (user->struct_size != sizeof(bw_session_spec) && user->struct_size != offsetof(bw_session_spec, shard_by_key))
+    CTX_FAIL(ctx, BW_ERR_SPEC, "bw_session_spec.struct_size mismatch");
+  bw_session_spec copy{};
+  memcpy(&copy, user, user->struct_size);
+  const bw_session_spec* spec = &copy;
+  if (ctx->world != 1 && !spec->shard_by_key)
+    CTX_FAIL(ctx, BW_ERR_SPEC, "session folds run on one GPU (world == 1) unless the spec sets shard_by_key");
   if (spec->reduction < BW_RED_COUNT || spec->reduction > BW_RED_MAX) CTX_FAIL(ctx, BW_ERR_SPEC, "reduction must be count, sum, min or max");
   if (spec->val_dtype != BW_VAL_I64 && spec->val_dtype != BW_VAL_F64) CTX_FAIL(ctx, BW_ERR_SPEC, "val_dtype must be I64 or F64");
   if (spec->gap_us < 0 || spec->gap_us > BW_UTC_MAX_US - BW_UTC_MIN_US) CTX_FAIL(ctx, BW_ERR_SPEC, "gap_us must be in 0..UTC_MAX - UTC_MIN");
   if (spec->wait_us < 0) CTX_FAIL(ctx, BW_ERR_SPEC, "wait_us must not be negative");
   if (spec->max_sessions_per_key < 1 || spec->max_sessions_per_key > BW_SESS_MAXM)
     CTX_FAIL(ctx, BW_ERR_SPEC, "max_sessions_per_key must be in 1..%d", BW_SESS_MAXM);
-  if (spec->max_batch_rows == 0 || spec->max_batch_rows >= (1ULL << 31)) CTX_FAIL(ctx, BW_ERR_SPEC, "bad max_batch_rows");
+  // an owner groups up to max_batch_rows from every rank with 32-bit sort indices
+  if (spec->max_batch_rows == 0 || spec->max_batch_rows > ((1ULL << 31) - 1) / (u64)ctx->world)
+    CTX_FAIL(ctx, BW_ERR_SPEC, "bad max_batch_rows: max_batch_rows * world must be in [1, 2^31)");
   CU(ctx, cudaSetDevice(ctx->device));
   std::unique_ptr<bw_session, void (*)(bw_session*)> sp(new bw_session(), bw_session_destroy);  // torn down on every failure
   bw_session* f = sp.get();
@@ -2863,7 +2908,8 @@ bw_status bw_session_create(bw_ctx* ctx, const bw_session_spec* spec, bw_session
   CU(ctx, cudaMemsetAsync(f->d_cnt, 0, 24, f->s));
   CU(ctx, own.host(&f->h_err, 64 / sizeof(u32)));
   CU(ctx, own.host(&f->h_cnt, 64 / sizeof(unsigned long long)));
-  const u64 n = spec->max_batch_rows, m = std::max<u64>(spec->max_emit_rows, 1), l = std::max<u64>(spec->max_late_rows, 1);
+  // rows one activation brings to this rank: its own on one GPU, up to max_batch_rows from every rank on world > 1
+  const u64 n = spec->max_batch_rows * (u64)ctx->world, m = std::max<u64>(spec->max_emit_rows, 1), l = std::max<u64>(spec->max_late_rows, 1);
   bw_status st = keyed_alloc(ctx, own, f->k, n, f->s);
   if (st != BW_OK) return st;
   CU(ctx, own.dev(&f->d_vals, n));
@@ -2885,6 +2931,12 @@ bw_status bw_session_create(bw_ctx* ctx, const bw_session_spec* spec, bw_session
   k_session_init<<<ctx->sm_count * 4, 256, 0, f->s>>>(t);
   CU(ctx, cudaGetLastError());
   CU(ctx, cudaStreamSynchronize(f->s));
+  if (ctx->world > 1) {
+    CU(ctx, own.dev(&f->d_name, n));
+    CU(ctx, own.dev(&f->d_late0, 1));
+    st = f->x.setup(ctx, own, spec->max_batch_rows, true, f->s);
+    if (st != BW_OK) return st;
+  }
   *out = sp.release();
   return BW_OK;
 }
@@ -2893,6 +2945,7 @@ void bw_session_destroy(bw_session* f) {
   if (!f) return;
   cudaSetDevice(f->ctx->device);
   if (f->s) cudaStreamSynchronize(f->s);
+  f->x.close(f->ctx);
   delete f;  // f->own releases every buffer and the stream
 }
 
@@ -2930,10 +2983,102 @@ static bw_status session_check(bw_session* f) {
   return BW_OK;
 }
 
+// bw_session_apply / _apply_device on world > 1 (include/bwgpu.h): every row to its key's owner, then K7 there over what
+// arrived.  `host`: the columns are host memory.
+static bw_status session_apply_ranks(bw_session* f, const u64* keys, const void* vals, const i64* ts_us, u64 rows, u64 epoch,
+                                     i64 system_now_us, bool host) {
+  bw_ctx* ctx = f->ctx;
+  const int W = ctx->world;
+  const bool count = f->spec.reduction == BW_RED_COUNT;
+  cudaStream_t s = f->s;
+  CU(ctx, cudaSetDevice(ctx->device));
+  // A call that cannot go ahead still takes part in the exchange and both barriers, so that no peer waits for it in a
+  // barrier: it sends no rows and raises its refusal flag, and every rank then fails the call.
+  bw_status refuse = BW_OK;
+  std::string why;
+  if (f->failed) {
+    refuse = BW_ERR_STATE;
+    why = "session fold: an earlier call ran out of capacity; the fold is unusable";
+  } else if (rows > f->spec.max_batch_rows) {
+    refuse = BW_ERR_SPEC;
+    why = "session: rows > max_batch_rows";
+  } else if (rows && (!keys || !ts_us || (!vals && !count))) {
+    refuse = BW_ERR_SPEC;
+    why = "session: NULL column";
+  } else if (f->batch_no && epoch < f->last_epoch) {
+    refuse = BW_ERR_STATE;
+    why = "session: epochs must not decrease";
+  } else if ((refuse = session_check(f)) != BW_OK) {  // a full table or session list met by an earlier apply_device
+    why = ctx->err;
+  }
+  if (refuse != BW_OK) rows = 0;
+  PartIn in;
+  in.keys = keys;
+  in.vals = count ? nullptr : vals;
+  in.ts = ts_us;
+  in.n = rows;
+  in.val_bytes = count ? 0 : 8;
+  in.world = W;
+  if (host && rows) {  // staged in K7's own columns: the gather overwrites them only after the scatter has read them
+    CU(ctx, cudaMemcpyAsync(f->k.d_keys, keys, rows * 8, cudaMemcpyHostToDevice, s));
+    CU(ctx, cudaMemcpyAsync(f->d_ts, ts_us, rows * 8, cudaMemcpyHostToDevice, s));
+    if (!count) CU(ctx, cudaMemcpyAsync(f->d_vals, vals, rows * 8, cudaMemcpyHostToDevice, s));
+    in.keys = f->k.d_keys;
+    in.vals = count ? nullptr : f->d_vals;
+    in.ts = f->d_ts;
+  }
+  bw_status st = f->x.send(ctx, s, in, epoch, system_now_us, refuse != BW_OK);
+  if (st != BW_OK) return st;
+  // every rank reads the same head: all of them fail here, or none does
+  const u64 *got_epoch = f->x.head(1), *got_now = f->x.head(2), *got_refused = f->x.head(3);
+  int refused = -1, epoch_differs = -1, now_differs = -1;
+  for (int r = W - 1; r >= 0; --r) {
+    if (got_refused[r]) refused = r;
+    if (got_epoch[r] != got_epoch[0]) epoch_differs = r;
+    if (got_now[r] != got_now[0]) now_differs = r;
+  }
+  const bool go = refused < 0 && epoch_differs < 0 && now_differs < 0;
+  u64 n = 0;
+  if (go) {
+    BatchView bv;
+    n = f->x.received(ctx, bv);
+    if (n)
+      k_xsess_gather<<<ctx->sm_count * 4, 256, 0, s>>>(bv, f->x.rows(), f->spec.max_batch_rows, n, f->k.d_keys, count ? nullptr : f->d_vals,
+                                                       f->d_ts, f->d_name);
+    CU(ctx, cudaGetLastError());
+  }
+  st = f->x.done(ctx, s);
+  if (st != BW_OK) return st;
+  if (refuse != BW_OK) CTX_FAIL(ctx, refuse, "%s", why.c_str());
+  if (refused >= 0) CTX_FAIL(ctx, BW_ERR_STATE, "session: rank %d refused this call (its own error says why); no rank folded it", refused);
+  if (epoch_differs >= 0)
+    CTX_FAIL(ctx, BW_ERR_STATE, "session: rank 0 played epoch %llu and rank %d epoch %llu; every rank must pass the same epoch to one call",
+             (unsigned long long)got_epoch[0], epoch_differs, (unsigned long long)got_epoch[epoch_differs]);
+  if (now_differs >= 0)
+    CTX_FAIL(ctx, BW_ERR_STATE,
+             "session: rank 0 passed system_now_us %lld and rank %d %lld; every rank must pass the same system time to one call",
+             (long long)got_now[0], now_differs, (long long)got_now[now_differs]);
+  f->last_epoch = epoch;
+  session_now(f, system_now_us);
+  const SessParams p = session_params(f, epoch);
+  f->batch_no++;
+  if (n) {
+    st = keyed_group(ctx, f->k, f->k.d_keys, n, s);
+    if (st != BW_OK) return st;
+    CU(ctx, cudaMemcpyAsync(f->d_late0, f->e.n_late, 8, cudaMemcpyDeviceToDevice, s));
+    k_session_apply<<<ctx->sm_count * 8, 256, 0, s>>>(f->t, f->e, p, f->k.d_ksorted, f->k.d_isorted, f->k.d_head,
+                                                      count ? nullptr : f->d_vals, f->d_ts, n);
+    k_xsess_name_late<<<ctx->sm_count * 4, 256, 0, s>>>(f->d_late0, f->e.n_late, f->e.max_late, f->e.l_row, f->d_name);
+    CU(ctx, cudaGetLastError());
+  }
+  return host ? session_check(f) : BW_OK;
+}
+
 bw_status bw_session_apply_device(bw_session* f, const uint64_t* d_keys, const void* d_vals, const int64_t* d_ts_us, uint64_t rows,
                                   uint64_t epoch, int64_t system_now_us) {
   if (!f) return BW_ERR_SPEC;
   bw_ctx* ctx = f->ctx;
+  if (ctx->world > 1) return session_apply_ranks(f, d_keys, d_vals, d_ts_us, rows, epoch, system_now_us, false);
   if (f->failed) CTX_FAIL(ctx, BW_ERR_STATE, "session fold: an earlier call ran out of capacity; the fold is unusable");
   if (rows > f->spec.max_batch_rows) CTX_FAIL(ctx, BW_ERR_SPEC, "session: rows > max_batch_rows");
   if (rows && (!d_keys || !d_ts_us || (!d_vals && f->spec.reduction != BW_RED_COUNT))) CTX_FAIL(ctx, BW_ERR_SPEC, "session: NULL column");
@@ -2956,6 +3101,7 @@ bw_status bw_session_apply(bw_session* f, const uint64_t* keys, const void* vals
                            int64_t system_now_us) {
   if (!f) return BW_ERR_SPEC;
   bw_ctx* ctx = f->ctx;
+  if (ctx->world > 1) return session_apply_ranks(f, keys, vals, ts_us, rows, epoch, system_now_us, true);
   if (rows > f->spec.max_batch_rows) CTX_FAIL(ctx, BW_ERR_SPEC, "session: rows > max_batch_rows");
   CU(ctx, cudaSetDevice(ctx->device));
   const bool has_vals = vals != nullptr;
@@ -2992,7 +3138,7 @@ static bw_status session_collect(bw_session* f, bw_session_rows* out) {
     }
     if (nmid) CU(ctx, cudaMemcpyAsync(f->h_mids, e.mids, nmid * 8, cudaMemcpyDeviceToHost, s));
   }
-  if (nl) {  // per call, key string, then arrival order
+  if (nl) {  // per call, key string, then arrival order (the row column holds names: source rank << 32 | source row)
     st = order_perm(ctx, x, s, nl, e.l_key, e.l_row, e.l_ord, nullptr, n_ord, f->first_call, nullptr);
     if (st != BW_OK) return st;
     const u64* src[] = {e.l_key, e.l_epoch, e.l_act, e.l_row};
@@ -3004,6 +3150,11 @@ static bw_status session_collect(bw_session* f, bw_session_rows* out) {
   CU(ctx, cudaGetLastError());
   CU(ctx, cudaMemsetAsync(f->d_cnt, 0, 24, s));
   CU(ctx, cudaStreamSynchronize(s));
+  u64 *lrow = f->hl.col[3], *lrank = f->hl.col[4];
+  for (u64 i = 0; i < nl; ++i) {
+    lrank[i] = lrow[i] >> 32;
+    lrow[i] &= 0xffffffffULL;
+  }
   // merged ids in row order
   f->merged_off.assign(nc + 1, 0);
   f->merged_ids.resize(nmid);
@@ -3027,6 +3178,7 @@ static bw_status session_collect(bw_session* f, bw_session_rows* out) {
   out->late_epoch = f->hl.col[1];
   out->late_activation = f->hl.col[2];
   out->late_row = f->hl.col[3];
+  out->late_rank = f->hl.col[4];
   return BW_OK;
 }
 

@@ -443,7 +443,8 @@ class SessionRows:
     late_key: np.ndarray
     late_epoch: np.ndarray
     late_activation: np.ndarray
-    late_row: np.ndarray
+    late_row: np.ndarray  # the row's index in the columns its source rank passed
+    late_rank: np.ndarray  # that source rank; all zeros on one rank
 
     def merged(self, i: int) -> List[int]:
         return self.merged_ids[self.merged_off[i] : self.merged_off[i + 1]].tolist()
@@ -462,11 +463,20 @@ class SessionRows:
 
 
 class SessionFold:
-    """Session-window count / sum / min / max by key (``bw_session``, K7; windowing.py:671-810, 1046-1190)."""
+    """Session-window count / sum / min / max by key (``bw_session``, K7; windowing.py:671-810, 1046-1190).
+
+    On a multi-rank context (``world > 1``) the fold needs ``shard_by_key=True`` (without it, create raises, as a fold
+    that cannot see the other ranks' rows would be wrong); it is then sharded by key and collective: every rank creates
+    it with the same arguments and calls ``apply`` or ``apply_device`` once per activation, with its own rows (possibly none), the
+    same epoch and the same ``system_now_us``.  Each row goes to rank ``bw_route(key, world)``, which folds what arrived
+    in (source rank, source order).  A call one rank cannot make (too many rows, a decreasing epoch, a failed fold)
+    fails on every rank, and no rank folds it.  A rank's ``advance`` / ``eof`` return the sessions and late rows of the
+    keys it owns; a late row names its input row by (``late_activation``, ``late_rank``, ``late_row``).  Close it only
+    once no rank calls it any more."""
 
     def __init__(self, ctx: Context, reduction: str = "count", gap_us: int = 10_000_000, wait_us: Optional[int] = 0,
                  val_dtype: str = "i64", capacity_hint: int = 1 << 16, max_batch_rows: int = 1 << 20, max_emit_rows: int = 1 << 20,
-                 max_late_rows: int = 1 << 20, max_sessions_per_key: int = 16):
+                 max_late_rows: int = 1 << 20, max_sessions_per_key: int = 16, shard_by_key: bool = False):
         """``wait_us=None``: the watermark never advances on data (``BW_WAIT_FOREVER``)."""
         self.ctx, self.lib = ctx, ctx.lib
         self.reduction, self.val_dtype = reduction, val_dtype
@@ -476,6 +486,7 @@ class SessionFold:
         s.gap_us, s.wait_us = gap_us, N.BW_WAIT_FOREVER if wait_us is None else wait_us
         s.capacity_hint, s.max_batch_rows, s.max_emit_rows, s.max_late_rows = capacity_hint, max_batch_rows, max_emit_rows, max_late_rows
         s.max_sessions_per_key = max_sessions_per_key
+        s.shard_by_key = int(shard_by_key)
         self.spec = s
         h = C.c_void_p()
         N.check(self.lib.bw_session_create(ctx.h, C.byref(s), C.byref(h)), ctx.h)
@@ -516,7 +527,7 @@ class SessionFold:
                            arr(r.closed_open_us, nc, np.int64), arr(r.closed_close_us, nc, np.int64), arr(r.closed_epoch, nc, np.uint64),
                            off, arr(r.merged_ids, int(off[-1]), np.int64),
                            arr(r.late_key, nl, np.uint64), arr(r.late_epoch, nl, np.uint64), arr(r.late_activation, nl, np.uint64),
-                           arr(r.late_row, nl, np.uint64))
+                           arr(r.late_row, nl, np.uint64), arr(r.late_rank, nl, np.uint64))
 
     def advance(self, system_now_us: int = 0) -> SessionRows:
         """Rows since the last call; ``system_now_us`` > 0 first runs the notify phase at that system time."""

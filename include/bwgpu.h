@@ -405,7 +405,32 @@ bw_status bw_join_eof(bw_join* j, bw_join_rows* out);
  * `close_for` (:774-788): sessions with close < watermark - gap (UTC_MIN if that is below it), in id order.
  * Accumulators: count_window :1679-1689; reduce_window(operator.add) :2268-2285 (i64 sums wrap past 2^63);
  * max_window / min_window :2189 / :2236 with `by` = identity (the accumulator is replaced only if the new value is
- * strictly greater / less, so signed zeros and NaN come out exactly as in Python).  One GPU only. */
+ * strictly greater / less, so signed zeros and NaN come out exactly as in Python).
+ *
+ * On a context with world W > 1 the fold runs only when the spec sets shard_by_key (else bw_session_create returns
+ * BW_ERR_SPEC, before any collective); it is then sharded by key (all of its state is per key):
+ *  - bw_session_create is collective (every rank calls it with the same spec).  Each rank holds a receive region of
+ *    W x max_batch_rows rows of key, value, ts and source row (28 B a row), shared with every peer over peer memory
+ *    (CUDA IPC mappings under NCCL, plain pointers on a loopback world); bw_session_destroy closes the mappings, once
+ *    no rank calls any more.  max_batch_rows x W must be below 2^31 (BW_ERR_SPEC): an owner groups with 32-bit sort
+ *    indices.
+ *  - bw_session_apply and bw_session_apply_device are collective: every rank calls one of them once per activation with
+ *    its own rows (possibly none), the same epoch and the same system_now_us.  Each row goes to rank bw_route(key, W),
+ *    the owner the window fold uses, which folds what it received in (source rank, source order).  Ranks that pass
+ *    different epochs or different system_now_us to one call all get BW_ERR_STATE.  apply_device reads its columns in
+ *    the exchange, before it returns.
+ *  - A call that cannot go ahead on one rank (rows > max_batch_rows, a NULL column, a decreasing epoch, a fold already
+ *    failed) still takes part in the exchange, so that no rank is left waiting: that rank returns its own error, every
+ *    other rank BW_ERR_STATE, and no rank folds the call.  A full key table or session list raises BW_ERR_CAPACITY on
+ *    the owning rank (bw_session_apply: in that call; apply_device: in the next call or advance), and from then on
+ *    every rank's apply returns BW_ERR_STATE.
+ *  - bw_session_advance (notify phase included) and bw_session_eof stay local: rank r closes and returns the sessions
+ *    of the keys it owns.  A late row is named by (late_activation, late_rank, late_row): late_row is the row's index in
+ *    the columns that source rank passed.
+ *  - Taking each call's rows from every rank, concatenating them and stably sorting the closed and the late columns
+ *    separately by key string gives exactly what a world-1 fold returns for that call when it is fed the rank-major
+ *    concatenation of every rank's columns; late row (r, i) is world-1 row offset_r + i.  Float sums match bit for bit:
+ *    the fold order is the same. */
 typedef struct bw_session bw_session;
 typedef struct bw_session_spec {
   uint32_t struct_size;
@@ -420,6 +445,9 @@ typedef struct bw_session_spec {
   uint64_t max_batch_rows;
   uint64_t max_emit_rows;       /* closed sessions, and their merged ids, retained between bw_session_advance calls */
   uint64_t max_late_rows;       /* late rows retained between bw_session_advance calls */
+  int32_t shard_by_key;         /* world > 1: 1 shards the fold by key over the ranks (above); ignored on world 1.  A
+                                   spec whose struct_size ends before this field has it 0 */
+  int32_t reserved;
 } bw_session_spec;
 /* Rows handed downstream since the last advance / eof, in the reference's order: per call (activation, notify phase
  * or EOF), ascending key string (src/operators.rs:758-767, :862-894); within a key late rows in arrival order and
@@ -436,12 +464,14 @@ typedef struct bw_session_rows {
   const uint64_t* closed_epoch;   /* the epoch of the activation, or of the last one before a notify / EOF */
   const uint64_t* merged_off;     /* [n_closed + 1]: row i merged ids are merged_ids[merged_off[i] .. merged_off[i+1]) */
   const int64_t* merged_ids;      /* ascending per row */
-  /* `late` stream: one row per late item; (activation, row) name the input row (activations counted from 0) */
+  /* `late` stream: one row per late item; (activation, row) name the input row (activations counted from 0), with
+   * late_rank on world > 1 */
   uint64_t n_late;
   const uint64_t* late_key;
   const uint64_t* late_epoch;
   const uint64_t* late_activation;
   const uint64_t* late_row;
+  const uint64_t* late_rank;      /* the source rank of late_row on world > 1; all zeros on world 1 */
 } bw_session_rows;
 bw_status bw_session_create(bw_ctx* ctx, const bw_session_spec* spec, bw_session** out);
 void bw_session_destroy(bw_session* s);
