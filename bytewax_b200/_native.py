@@ -78,7 +78,8 @@ class BwSnapshot(C.Structure):
 
 class BwSmapSpec(C.Structure):
     _fields_ = [("struct_size", C.c_uint32), ("window", C.c_int32), ("val_dtype", C.c_int32), ("reserved", C.c_int32),
-                ("threshold", C.c_double), ("capacity_hint", C.c_uint64), ("max_batch_rows", C.c_uint64)]
+                ("threshold", C.c_double), ("capacity_hint", C.c_uint64), ("max_batch_rows", C.c_uint64), ("shard_by_key", C.c_int32),
+                ("reserved2", C.c_int32)]
 
 
 class BwJoinSpec(C.Structure):

@@ -239,3 +239,16 @@ __global__ void k_xchg_head(XchgHead pub, int world, u64 epoch, i64 now, u64 ref
     h[3 * BW_MAX_WORLD] = refused;
   }
 }
+
+// A keyed map on N ranks (K5) returns each row's results to the rank that passed the row: the return section of one
+// rank's region (RankXchg in bwgpu.cu), `cap` rows of mu, sigma and flag at the source's row index, and one error word
+// per owner rank.
+struct XchgRet {
+  double* mu;
+  double* sigma;
+  unsigned char* flag;
+  u32* err;  // [BW_MAX_WORLD]: owner rank d's table error (its t.err) after the call
+};
+struct XchgRetPeers {
+  XchgRet at[BW_MAX_WORLD];  // every rank's return section as seen from this rank
+};

@@ -244,6 +244,38 @@ __global__ void k_xjoin_gather(BatchView bv, u64 n, u64* keys, u64* vals, unsign
   }
 }
 
+// K5 on world > 1, at the owner: the received segments into K5's columns in (source rank, source order), the order a
+// world-1 map sees when it is fed the rank-major concatenation.  Values are 4 (f32) or 8 (f64) bytes, packed at the
+// start of each source's segment.  name[i] = source rank << 32 | the row's index in that source's columns (src_row: the
+// region's row column, `cap` rows per source).
+__global__ void k_xsmap_gather(BatchView bv, const u32* src_row, u64 cap, u64 n, int is_f32, u64* keys, void* vals, u64* name) {
+  for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (u64)gridDim.x * blockDim.x) {
+    int r = 0;
+    u64 o = i;
+    while (o >= bv.h_counts[r]) o -= bv.h_counts[r++];
+    keys[i] = bv.keys[r][o];
+    if (is_f32) ((u32*)vals)[i] = ((const u32*)bv.vals[r])[o];
+    else ((u64*)vals)[i] = ((const u64*)bv.vals[r])[o];
+    name[i] = (u64)r << 32 | src_row[(u64)r * cap + o];
+  }
+}
+
+// The return leg: gathered row i's results into its source rank's return section at its source row, over peer memory;
+// then this owner's table error into every rank's error word for this owner (every owner, every call, rows or not).
+__global__ void k_xsmap_return(XchgRetPeers to, const u64* name, const double* mu, const double* sigma, const unsigned char* flag,
+                               u64 n, const u32* err, int me, int world) {
+  for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (u64)gridDim.x * blockDim.x) {
+    const u64 nm = name[i];
+    const XchgRet& d = to.at[nm >> 32];
+    const u32 row = (u32)nm;
+    d.mu[row] = mu[i];
+    d.sigma[row] = sigma[i];
+    d.flag[row] = flag[i];
+  }
+  if (blockIdx.x == 0 && threadIdx.x < (unsigned)world) to.at[threadIdx.x].err[me] = *err;
+  __threadfence_system();
+}
+
 __global__ void k_join_eof(JoinSlot* slots, u64 cap, u32* err, int emit_mode, JoinEmit e, u64 epoch) {
   for (u64 s = (u64)blockIdx.x * blockDim.x + threadIdx.x; s <= cap; s += (u64)gridDim.x * blockDim.x) {
     const u64 fl = slots[s].flags;

@@ -2411,122 +2411,25 @@ static bw_status keyed_group(bw_ctx* ctx, KeyedScratch& k, const u64* d_keys, u6
   return BW_OK;
 }
 
-struct bw_smap {
-  Owner own;  // every buffer and the stream below
-  bw_ctx* ctx = nullptr;
-  bw_smap_spec spec{};
-  SmapTable t{};
-  KeyedScratch k;
-  cudaStream_t s = nullptr;
-  u32* h_err = nullptr;
-  void* d_vals = nullptr;
-  double *d_mu = nullptr, *d_sigma = nullptr;
-  unsigned char* d_flag = nullptr;
-};
-
-bw_status bw_smap_create(bw_ctx* ctx, const bw_smap_spec* spec, bw_smap** out) {
-  if (!ctx || !spec || !out) CTX_FAIL(ctx, BW_ERR_SPEC, "bw_smap_create: NULL argument");
-  if (spec->struct_size != sizeof(bw_smap_spec)) CTX_FAIL(ctx, BW_ERR_SPEC, "bw_smap_spec.struct_size mismatch");
-  if (spec->window < 1 || spec->window > BW_SMAP_MAXW) CTX_FAIL(ctx, BW_ERR_SPEC, "window must be in 1..%d", BW_SMAP_MAXW);
-  if (spec->val_dtype != BW_VAL_F32 && spec->val_dtype != BW_VAL_F64) CTX_FAIL(ctx, BW_ERR_SPEC, "val_dtype must be F32 or F64");
-  if (spec->max_batch_rows == 0 || spec->max_batch_rows >= (1ULL << 31)) CTX_FAIL(ctx, BW_ERR_SPEC, "bad max_batch_rows");
-  CU(ctx, cudaSetDevice(ctx->device));
-  std::unique_ptr<bw_smap, void (*)(bw_smap*)> mp(new bw_smap(), bw_smap_destroy);  // torn down on every failure
-  bw_smap* m = mp.get();
-  Owner& own = m->own;
-  m->ctx = ctx;
-  m->spec = *spec;
-  u64 cap = std::max<u64>(1024, 2 * std::max<u64>(spec->capacity_hint, 1));
-  m->t.cap = cap;
-  m->t.window = spec->window;
-  CU(ctx, own.stream(&m->s));
-  CU(ctx, own.dev(&m->t.keys, cap + 1));
-  CU(ctx, own.dev(&m->t.cnt, cap + 1));
-  CU(ctx, own.dev(&m->t.ring, (cap + 1) * (u64)spec->window));
-  CU(ctx, own.dev(&m->t.err, 1));
-  CU(ctx, cudaMemsetAsync(m->t.err, 0, 4, m->s));
-  CU(ctx, own.host(&m->h_err, 64 / sizeof(u32)));
-  const u64 n = spec->max_batch_rows;
-  bw_status st = keyed_alloc(ctx, own, m->k, n, m->s);
-  if (st != BW_OK) return st;
-  CU(ctx, own.dev(&m->d_vals, n * 8));
-  CU(ctx, own.dev(&m->d_mu, n));
-  CU(ctx, own.dev(&m->d_sigma, n));
-  CU(ctx, own.dev(&m->d_flag, n));
-  k_smap_init<<<ctx->sm_count * 4, 256, 0, m->s>>>(m->t);
-  CU(ctx, cudaGetLastError());
-  CU(ctx, cudaStreamSynchronize(m->s));
-  *out = mp.release();
-  return BW_OK;
-}
-
-void bw_smap_destroy(bw_smap* m) {
-  if (!m) return;
-  cudaSetDevice(m->ctx->device);
-  if (m->s) cudaStreamSynchronize(m->s);
-  delete m;  // m->own releases every buffer and the stream
-}
-
-bw_status bw_smap_apply_device(bw_smap* m, const uint64_t* d_keys, const void* d_vals, uint64_t rows, double* d_mu,
-                               double* d_sigma, uint8_t* d_flag) {
-  if (!m) return BW_ERR_SPEC;
-  bw_ctx* ctx = m->ctx;
-  if (rows > m->spec.max_batch_rows) CTX_FAIL(ctx, BW_ERR_SPEC, "smap: rows > max_batch_rows");
-  if (rows == 0) return BW_OK;
-  CU(ctx, cudaSetDevice(ctx->device));
-  bw_status st = keyed_group(ctx, m->k, d_keys, rows, m->s);
-  if (st != BW_OK) return st;
-  const int grid = ctx->sm_count * 8;
-  const int is_f32 = m->spec.val_dtype == BW_VAL_F32;
-  k_smap_slots<<<grid, 256, 0, m->s>>>(m->t, m->k.d_ksorted, m->k.d_head, m->k.d_slot, rows);
-  k_smap_eval<<<grid, 256, 0, m->s>>>(m->t, m->k.d_isorted, m->k.d_head, m->k.d_slot, d_vals, is_f32, m->spec.threshold, d_mu, d_sigma,
-                                       d_flag, rows);
-  k_smap_update<<<grid, 256, 0, m->s>>>(m->t, m->k.d_ksorted, m->k.d_isorted, m->k.d_head, m->k.d_slot, d_vals, is_f32, rows);
-  CU(ctx, cudaGetLastError());
-  return BW_OK;
-}
-
-bw_status bw_smap_sync(bw_smap* m) {
-  if (!m) return BW_ERR_SPEC;
-  bw_ctx* ctx = m->ctx;
-  CU(ctx, cudaMemcpyAsync(m->h_err, m->t.err, 4, cudaMemcpyDeviceToHost, m->s));
-  CU(ctx, cudaStreamSynchronize(m->s));
-  if (*m->h_err) CTX_FAIL(ctx, (bw_status)*m->h_err, "smap kernel raised status %u: key table full (raise capacity_hint)", *m->h_err);
-  return BW_OK;
-}
-
-bw_status bw_smap_apply(bw_smap* m, const uint64_t* keys, const void* vals, uint64_t rows, double* out_mu, double* out_sigma,
-                        uint8_t* out_flag) {
-  if (!m) return BW_ERR_SPEC;
-  bw_ctx* ctx = m->ctx;
-  if (rows > m->spec.max_batch_rows) CTX_FAIL(ctx, BW_ERR_SPEC, "smap: rows > max_batch_rows");
-  if (rows == 0) return BW_OK;
-  CU(ctx, cudaSetDevice(ctx->device));
-  const size_t vb = m->spec.val_dtype == BW_VAL_F32 ? 4 : 8;
-  CU(ctx, cudaMemcpyAsync(m->k.d_keys, keys, rows * 8, cudaMemcpyHostToDevice, m->s));
-  CU(ctx, cudaMemcpyAsync(m->d_vals, vals, rows * vb, cudaMemcpyHostToDevice, m->s));
-  bw_status st = bw_smap_apply_device(m, m->k.d_keys, m->d_vals, rows, m->d_mu, m->d_sigma, m->d_flag);
-  if (st != BW_OK) return st;
-  CU(ctx, cudaMemcpyAsync(out_mu, m->d_mu, rows * 8, cudaMemcpyDeviceToHost, m->s));
-  CU(ctx, cudaMemcpyAsync(out_sigma, m->d_sigma, rows * 8, cudaMemcpyDeviceToHost, m->s));
-  CU(ctx, cudaMemcpyAsync(out_flag, m->d_flag, rows, cudaMemcpyDeviceToHost, m->s));
-  return bw_smap_sync(m);
-}
-
-// ---- keyed kernels on N ranks (K6, K7): every row to its key's owner ----
+// ---- keyed kernels on N ranks (K5, K6, K7): every row to its key's owner ----
 // One rank's receive region: a 256-byte head of four rows of BW_MAX_WORLD u64 -- per source rank r: the rows r sent
 // here, the epoch, the system time and the refusal flag r published (k_xchg_head) -- then source r's keys, values and ts
-// (8 bytes each, the partition's column widths) and, with source rows, its rows' indices (4 bytes) at [r * cap].
+// (8 bytes each, the partition's column widths) and, with source rows, its rows' indices (4 bytes) at [r * cap].  With a
+// return section (a keyed map, K5), 256-byte aligned at the end: this rank's own `cap` rows of mu (f64), sigma (f64),
+// the W owners' error words (u32, BW_MAX_WORLD of them) and flag (u8), which owners store into at the row's index.
 // Setup is collective: the region is shared with every rank (coll_share_base).  A call is collective too: send()
 // publishes the head, partitions the source's columns straight into the owners' regions (peer stores), enters a barrier
-// and reads the head; the caller checks it and gathers what arrived, then done() enters a second barrier, past which no
-// source of the next call overwrites rows an owner still reads.  A second barrier rather than double-buffered regions:
-// a call already waits on the host for the received counts, so a second region set would leave nothing to overlap and
+// and reads the head; the caller checks it, gathers what arrived (and, with a return section, maps it and stores the
+// results back), then done() enters a second barrier, past which no source of the next call overwrites rows an owner
+// still reads, and every source may read its return section.  A second barrier rather than double-buffered regions: a
+// call already waits on the host for the received counts, so a second region set would leave nothing to overlap and
 // would double the region.
+#define BW_XRET_ROW_BYTES 17  // mu, sigma, flag
 struct RankXchg {
   u64 cap = 0;       // rows per source: max_batch_rows
   bool src_rows = false;
-  size_t keys_off = 0, vals_off = 0, ts_off = 0, rows_off = 0, total = 0;
+  size_t keys_off = 0, vals_off = 0, ts_off = 0, rows_off = 0, ret_off = 0, total = 0;
+  int ret_row = 0;   // bytes of a return row: 0 (none) or BW_XRET_ROW_BYTES
   void* base = nullptr;
   void* peer[BW_MAX_WORLD] = {nullptr};  // every rank's region as seen from here
   u32* d_tile_counts = nullptr;
@@ -2534,16 +2437,23 @@ struct RankXchg {
   u32* d_word = nullptr;      // coll_barrier's word
   u64* h_head = nullptr;      // pinned: the head as received
 
-  bw_status setup(bw_ctx* ctx, Owner& own, u64 max_batch_rows, bool with_src_rows, cudaStream_t s) {
+  bw_status setup(bw_ctx* ctx, Owner& own, u64 max_batch_rows, bool with_src_rows, int ret_row_bytes, cudaStream_t s) {
+    if (ret_row_bytes != 0 && ret_row_bytes != BW_XRET_ROW_BYTES) CTX_FAIL(ctx, BW_ERR_SPEC, "RankXchg: bad return row width");
     cap = max_batch_rows;
     src_rows = with_src_rows;
+    ret_row = ret_row_bytes;
     const size_t col = (size_t)cap * ctx->world;
     keys_off = 4 * BW_MAX_WORLD * sizeof(u64);
     vals_off = keys_off + col * 8;
     ts_off = vals_off + col * 8;
     rows_off = ts_off + col * 8;
     total = rows_off + (src_rows ? col * 4 : 0);
+    if (ret_row) {
+      ret_off = (total + 255) & ~(size_t)255;
+      total = ret_off + (size_t)cap * ret_row + BW_MAX_WORLD * sizeof(u32);
+    }
     CU(ctx, own.dev(&base, total));
+    if (ret_row) CU(ctx, cudaMemsetAsync(ret_at(base).err, 0, BW_MAX_WORLD * sizeof(u32), s));
     CU(ctx, own.dev(&d_tile_counts, ((cap + BW_PART_TILE - 1) / BW_PART_TILE + 1) * BW_MAX_WORLD));
     CU(ctx, own.dev(&d_ctr, 1));
     CU(ctx, own.dev(&d_word, 1));
@@ -2610,7 +2520,248 @@ struct RankXchg {
   }
   const u32* rows() const { return (const u32*)((const char*)base + rows_off); }
   bw_status done(bw_ctx* ctx, cudaStream_t s) { return coll_barrier(ctx, d_word, s); }
+  // the return section of the region at `b` (setup with a return row width)
+  XchgRet ret_at(void* b) const {
+    char* p = (char*)b + ret_off;
+    XchgRet c;
+    c.mu = (double*)p;
+    c.sigma = (double*)(p + cap * 8);
+    c.err = (u32*)(p + cap * 16);
+    c.flag = (unsigned char*)(c.err + BW_MAX_WORLD);
+    return c;
+  }
+  XchgRet ret_mine() const { return ret_at(base); }
+  XchgRetPeers ret_peers(bw_ctx* ctx) const {
+    XchgRetPeers p;
+    memset(&p, 0, sizeof p);
+    for (int r = 0; r < ctx->world; ++r) p.at[r] = ret_at(peer[r]);
+    return p;
+  }
 };
+
+struct bw_smap {
+  Owner own;  // every buffer and the stream below
+  bw_ctx* ctx = nullptr;
+  bw_smap_spec spec{};
+  SmapTable t{};
+  KeyedScratch k;
+  cudaStream_t s = nullptr;
+  u32* h_err = nullptr;
+  void* d_vals = nullptr;
+  double *d_mu = nullptr, *d_sigma = nullptr;
+  unsigned char* d_flag = nullptr;
+  // sharded by key (shard_by_key on world > 1): the exchange (with source rows and a return section), each gathered
+  // row's name (source rank << 32 | source row), the owners' error words as read back, and whether a call has failed
+  bool shard = false;
+  RankXchg x;
+  u64* d_name = nullptr;
+  u32* h_ret_err = nullptr;
+  bool failed = false;
+};
+
+bw_status bw_smap_create(bw_ctx* ctx, const bw_smap_spec* user, bw_smap** out) {
+  if (!ctx || !user || !out) CTX_FAIL(ctx, BW_ERR_SPEC, "bw_smap_create: NULL argument");
+  // a spec built against the header before shard_by_key existed ends just before it, and leaves it 0
+  if (user->struct_size != sizeof(bw_smap_spec) && user->struct_size != offsetof(bw_smap_spec, shard_by_key))
+    CTX_FAIL(ctx, BW_ERR_SPEC, "bw_smap_spec.struct_size mismatch");
+  bw_smap_spec copy{};
+  memcpy(&copy, user, user->struct_size);
+  const bw_smap_spec* spec = &copy;
+  if (spec->window < 1 || spec->window > BW_SMAP_MAXW) CTX_FAIL(ctx, BW_ERR_SPEC, "window must be in 1..%d", BW_SMAP_MAXW);
+  if (spec->val_dtype != BW_VAL_F32 && spec->val_dtype != BW_VAL_F64) CTX_FAIL(ctx, BW_ERR_SPEC, "val_dtype must be F32 or F64");
+  if (spec->max_batch_rows == 0 || spec->max_batch_rows >= (1ULL << 31)) CTX_FAIL(ctx, BW_ERR_SPEC, "bad max_batch_rows");
+  const bool shard = spec->shard_by_key && ctx->world > 1;
+  // an owner groups up to max_batch_rows from every rank with 32-bit sort indices, and names rows rank << 32 | row
+  if (shard && spec->max_batch_rows > ((1ULL << 31) - 1) / (u64)ctx->world)
+    CTX_FAIL(ctx, BW_ERR_SPEC, "bad max_batch_rows: max_batch_rows * world must be in [1, 2^31)");
+  CU(ctx, cudaSetDevice(ctx->device));
+  std::unique_ptr<bw_smap, void (*)(bw_smap*)> mp(new bw_smap(), bw_smap_destroy);  // torn down on every failure
+  bw_smap* m = mp.get();
+  Owner& own = m->own;
+  m->ctx = ctx;
+  m->spec = *spec;
+  m->shard = shard;
+  u64 cap = std::max<u64>(1024, 2 * std::max<u64>(spec->capacity_hint, 1));
+  m->t.cap = cap;
+  m->t.window = spec->window;
+  CU(ctx, own.stream(&m->s));
+  CU(ctx, own.dev(&m->t.keys, cap + 1));
+  CU(ctx, own.dev(&m->t.cnt, cap + 1));
+  CU(ctx, own.dev(&m->t.ring, (cap + 1) * (u64)spec->window));
+  CU(ctx, own.dev(&m->t.err, 1));
+  CU(ctx, cudaMemsetAsync(m->t.err, 0, 4, m->s));
+  CU(ctx, own.host(&m->h_err, 64 / sizeof(u32)));
+  // rows one activation brings to this rank: its own, or up to max_batch_rows from every rank when sharded
+  const u64 n = spec->max_batch_rows * (shard ? (u64)ctx->world : 1);
+  bw_status st = keyed_alloc(ctx, own, m->k, n, m->s);
+  if (st != BW_OK) return st;
+  CU(ctx, own.dev(&m->d_vals, n * 8));
+  CU(ctx, own.dev(&m->d_mu, n));
+  CU(ctx, own.dev(&m->d_sigma, n));
+  CU(ctx, own.dev(&m->d_flag, n));
+  k_smap_init<<<ctx->sm_count * 4, 256, 0, m->s>>>(m->t);
+  CU(ctx, cudaGetLastError());
+  CU(ctx, cudaStreamSynchronize(m->s));
+  if (shard) {
+    CU(ctx, own.dev(&m->d_name, n));
+    CU(ctx, own.host(&m->h_ret_err, BW_MAX_WORLD));
+    st = m->x.setup(ctx, own, spec->max_batch_rows, true, BW_XRET_ROW_BYTES, m->s);
+    if (st != BW_OK) return st;
+  }
+  *out = mp.release();
+  return BW_OK;
+}
+
+void bw_smap_destroy(bw_smap* m) {
+  if (!m) return;
+  cudaSetDevice(m->ctx->device);
+  if (m->s) cudaStreamSynchronize(m->s);
+  m->x.close(m->ctx);
+  delete m;  // m->own releases every buffer and the stream
+}
+
+// K5 over n device rows: group by key, then the ring kernels; outputs aligned with the rows
+static bw_status smap_map(bw_smap* m, const u64* d_keys, const void* d_vals, u64 n, double* d_mu, double* d_sigma, uint8_t* d_flag) {
+  bw_ctx* ctx = m->ctx;
+  bw_status st = keyed_group(ctx, m->k, d_keys, n, m->s);
+  if (st != BW_OK) return st;
+  const int grid = ctx->sm_count * 8;
+  const int is_f32 = m->spec.val_dtype == BW_VAL_F32;
+  k_smap_slots<<<grid, 256, 0, m->s>>>(m->t, m->k.d_ksorted, m->k.d_head, m->k.d_slot, n);
+  k_smap_eval<<<grid, 256, 0, m->s>>>(m->t, m->k.d_isorted, m->k.d_head, m->k.d_slot, d_vals, is_f32, m->spec.threshold, d_mu, d_sigma,
+                                       d_flag, n);
+  k_smap_update<<<grid, 256, 0, m->s>>>(m->t, m->k.d_ksorted, m->k.d_isorted, m->k.d_head, m->k.d_slot, d_vals, is_f32, n);
+  CU(ctx, cudaGetLastError());
+  return BW_OK;
+}
+
+// bw_smap_apply / _apply_device when sharded by key (include/bwgpu.h): every row to its key's owner, K5 there over
+// what arrived, and each row's mu, sigma and flag back to its source rank at its row.  `host`: the columns are host
+// memory.  Blocks until the call is complete.
+static bw_status smap_apply_ranks(bw_smap* m, const u64* keys, const void* vals, u64 rows, double* mu, double* sigma, uint8_t* flag,
+                                  bool host) {
+  bw_ctx* ctx = m->ctx;
+  const int W = ctx->world;
+  const int is_f32 = m->spec.val_dtype == BW_VAL_F32;
+  cudaStream_t s = m->s;
+  CU(ctx, cudaSetDevice(ctx->device));
+  // A call that cannot go ahead still takes part in the exchange and both barriers, so that no peer waits for it in a
+  // barrier: it sends no rows and raises its refusal flag, and every rank then fails the call.
+  bw_status refuse = BW_OK;
+  const char* why = "";
+  if (m->failed) {
+    refuse = BW_ERR_STATE;
+    why = "smap: an earlier call failed; the map is unusable";
+  } else if (rows > m->spec.max_batch_rows) {
+    refuse = BW_ERR_SPEC;
+    why = "smap: rows > max_batch_rows";
+  } else if (rows && (!keys || !vals || !mu || !sigma || !flag)) {
+    refuse = BW_ERR_SPEC;
+    why = "smap: NULL column";
+  }
+  if (refuse != BW_OK) rows = 0;
+  PartIn in;
+  in.keys = keys;
+  in.vals = vals;
+  in.ts = nullptr;
+  in.n = rows;
+  in.val_bytes = is_f32 ? 4 : 8;
+  in.world = W;
+  if (host && rows) {  // staged in K5's own columns: the gather overwrites them only after the scatter has read them
+    CU(ctx, cudaMemcpyAsync(m->k.d_keys, keys, rows * 8, cudaMemcpyHostToDevice, s));
+    CU(ctx, cudaMemcpyAsync(m->d_vals, vals, rows * in.val_bytes, cudaMemcpyHostToDevice, s));
+    in.keys = m->k.d_keys;
+    in.vals = m->d_vals;
+  }
+  // K5 has no epoch and no clock: the head's epoch and time rows carry 0
+  bw_status st = m->x.send(ctx, s, in, 0, 0, refuse != BW_OK);
+  if (st != BW_OK) return st;
+  // every rank reads the same head: all of them fail here, or none does
+  const u64* got_refused = m->x.head(3);
+  int refused = -1;
+  for (int r = W - 1; r >= 0; --r)
+    if (got_refused[r]) refused = r;
+  if (refused < 0) {
+    BatchView bv;
+    const u64 n = m->x.received(ctx, bv);
+    if (n) {
+      k_xsmap_gather<<<ctx->sm_count * 4, 256, 0, s>>>(bv, m->x.rows(), m->spec.max_batch_rows, n, is_f32, m->k.d_keys, m->d_vals, m->d_name);
+      CU(ctx, cudaGetLastError());
+      st = smap_map(m, m->k.d_keys, m->d_vals, n, m->d_mu, m->d_sigma, m->d_flag);
+      if (st != BW_OK) return st;
+    }
+    k_xsmap_return<<<ctx->sm_count * 4, 256, 0, s>>>(m->x.ret_peers(ctx), m->d_name, m->d_mu, m->d_sigma, m->d_flag, n, m->t.err, ctx->rank, W);
+    CU(ctx, cudaGetLastError());
+  }
+  // Ordering of the return sections.  Owners store into rank r's return section only between barrier 1 (in send) and
+  // barrier 2 (below) of a call; rank r reads it after barrier 2, and enqueues that read before its own barrier 1 of the
+  // next call.  coll_barrier is stream-ordered (an NCCL all-reduce on the stream, or a stream synchronise and then the
+  // host barrier on a loopback world), so no owner's next stores can overtake the read: no second region set and no
+  // third barrier are needed.
+  st = m->x.done(ctx, s);
+  if (st != BW_OK) return st;
+  if (refuse != BW_OK) CTX_FAIL(ctx, refuse, "%s", why);
+  if (refused >= 0) CTX_FAIL(ctx, BW_ERR_STATE, "smap: rank %d refused this call (its own error says why); no rank mapped it", refused);
+  const XchgRet ret = m->x.ret_mine();
+  if (rows) {
+    const cudaMemcpyKind kind = host ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice;
+    CU(ctx, cudaMemcpyAsync(mu, ret.mu, rows * 8, kind, s));
+    CU(ctx, cudaMemcpyAsync(sigma, ret.sigma, rows * 8, kind, s));
+    CU(ctx, cudaMemcpyAsync(flag, ret.flag, rows, kind, s));
+  }
+  CU(ctx, cudaMemcpyAsync(m->h_ret_err, ret.err, W * sizeof(u32), cudaMemcpyDeviceToHost, s));
+  CU(ctx, cudaStreamSynchronize(s));
+  int full = -1;
+  for (int r = W - 1; r >= 0; --r)
+    if (m->h_ret_err[r]) full = r;
+  if (full >= 0) {
+    m->failed = true;
+    const u32 e = m->h_ret_err[ctx->rank];
+    if (e) CTX_FAIL(ctx, (bw_status)e, "smap kernel raised status %u: key table full (raise capacity_hint)", e);
+    CTX_FAIL(ctx, BW_ERR_STATE, "smap: rank %d's key table is full; this call's results are invalid and the map is unusable", full);
+  }
+  return BW_OK;
+}
+
+bw_status bw_smap_apply_device(bw_smap* m, const uint64_t* d_keys, const void* d_vals, uint64_t rows, double* d_mu,
+                               double* d_sigma, uint8_t* d_flag) {
+  if (!m) return BW_ERR_SPEC;
+  bw_ctx* ctx = m->ctx;
+  if (m->shard) return smap_apply_ranks(m, d_keys, d_vals, rows, d_mu, d_sigma, d_flag, false);
+  if (rows > m->spec.max_batch_rows) CTX_FAIL(ctx, BW_ERR_SPEC, "smap: rows > max_batch_rows");
+  if (rows == 0) return BW_OK;
+  CU(ctx, cudaSetDevice(ctx->device));
+  return smap_map(m, d_keys, d_vals, rows, d_mu, d_sigma, d_flag);
+}
+
+bw_status bw_smap_sync(bw_smap* m) {
+  if (!m) return BW_ERR_SPEC;
+  bw_ctx* ctx = m->ctx;
+  CU(ctx, cudaMemcpyAsync(m->h_err, m->t.err, 4, cudaMemcpyDeviceToHost, m->s));
+  CU(ctx, cudaStreamSynchronize(m->s));
+  if (*m->h_err) CTX_FAIL(ctx, (bw_status)*m->h_err, "smap kernel raised status %u: key table full (raise capacity_hint)", *m->h_err);
+  if (m->failed) CTX_FAIL(ctx, BW_ERR_STATE, "smap: an earlier call failed; the map is unusable");
+  return BW_OK;
+}
+
+bw_status bw_smap_apply(bw_smap* m, const uint64_t* keys, const void* vals, uint64_t rows, double* out_mu, double* out_sigma,
+                        uint8_t* out_flag) {
+  if (!m) return BW_ERR_SPEC;
+  bw_ctx* ctx = m->ctx;
+  if (m->shard) return smap_apply_ranks(m, keys, vals, rows, out_mu, out_sigma, out_flag, true);
+  if (rows > m->spec.max_batch_rows) CTX_FAIL(ctx, BW_ERR_SPEC, "smap: rows > max_batch_rows");
+  if (rows == 0) return BW_OK;
+  CU(ctx, cudaSetDevice(ctx->device));
+  const size_t vb = m->spec.val_dtype == BW_VAL_F32 ? 4 : 8;
+  CU(ctx, cudaMemcpyAsync(m->k.d_keys, keys, rows * 8, cudaMemcpyHostToDevice, m->s));
+  CU(ctx, cudaMemcpyAsync(m->d_vals, vals, rows * vb, cudaMemcpyHostToDevice, m->s));
+  bw_status st = bw_smap_apply_device(m, m->k.d_keys, m->d_vals, rows, m->d_mu, m->d_sigma, m->d_flag);
+  if (st != BW_OK) return st;
+  CU(ctx, cudaMemcpyAsync(out_mu, m->d_mu, rows * 8, cudaMemcpyDeviceToHost, m->s));
+  CU(ctx, cudaMemcpyAsync(out_sigma, m->d_sigma, rows * 8, cudaMemcpyDeviceToHost, m->s));
+  CU(ctx, cudaMemcpyAsync(out_flag, m->d_flag, rows, cudaMemcpyDeviceToHost, m->s));
+  return bw_smap_sync(m);
+}
 
 struct bw_join {
   Owner own;  // every buffer and the stream below
@@ -2646,7 +2797,7 @@ static bw_status join_ranks_setup(bw_join* j) {
   CU(ctx, own.dev(&j->d_src_vals, B));
   CU(ctx, own.dev(&j->d_src_side, B));
   CU(ctx, own.dev(&j->d_src_side64, B));
-  return j->x.setup(ctx, own, B, false, j->s);
+  return j->x.setup(ctx, own, B, false, 0, j->s);
 }
 
 bw_status bw_join_create(bw_ctx* ctx, const bw_join_spec* spec, bw_join** out) {
@@ -2934,7 +3085,7 @@ bw_status bw_session_create(bw_ctx* ctx, const bw_session_spec* user, bw_session
   if (ctx->world > 1) {
     CU(ctx, own.dev(&f->d_name, n));
     CU(ctx, own.dev(&f->d_late0, 1));
-    st = f->x.setup(ctx, own, spec->max_batch_rows, true, f->s);
+    st = f->x.setup(ctx, own, spec->max_batch_rows, true, 0, f->s);
     if (st != BW_OK) return st;
   }
   *out = sp.release();

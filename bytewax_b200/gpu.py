@@ -338,15 +338,26 @@ class WindowFold:
 
 
 class ZScoreMap:
-    """``stateful_map`` with the rolling z-score detector (``bw_smap``; examples/anomaly_detector.py:16-48)."""
+    """``stateful_map`` with the rolling z-score detector (``bw_smap``; examples/anomaly_detector.py:16-48).
+
+    On a multi-rank context (``world > 1``) the map is rank-local unless ``shard_by_key=True``: each rank keeps its own
+    ring for every key it sees, so the caller must send every row of a key to one rank.  With ``shard_by_key=True`` it is
+    sharded by key and collective: every rank creates it with the same arguments and calls ``apply`` or ``apply_device``
+    once per activation, with its own rows (possibly none).  Each row goes to rank ``bw_route(key, world)``, which maps
+    what arrived in (source rank, source order) and sends each row's results back, so a rank's outputs stay aligned with
+    its own input rows; every rank's outputs concatenated rank-major equal a world-1 map over the rank-major
+    concatenation of every rank's rows.  A call one rank cannot make (too many rows, a NULL column, a failed map) fails
+    on every rank, and no rank maps it; a full key table on an owner fails the call on every rank and the map refuses
+    every later call.  Close it only once no rank calls it any more."""
 
     def __init__(self, ctx: Context, window: int = 10, threshold: float = 2.0, val_dtype: str = "f32", capacity_hint: int = 1 << 16,
-                 max_batch_rows: int = 1 << 20):
+                 max_batch_rows: int = 1 << 20, shard_by_key: bool = False):
         self.ctx, self.lib, self.val_dtype = ctx, ctx.lib, val_dtype
         s = N.BwSmapSpec()
         s.struct_size = C.sizeof(N.BwSmapSpec)
         s.window, s.val_dtype, s.threshold = window, N.VAL[val_dtype], threshold
         s.capacity_hint, s.max_batch_rows = capacity_hint, max_batch_rows
+        s.shard_by_key = int(shard_by_key)
         h = C.c_void_p()
         N.check(self.lib.bw_smap_create(ctx.h, C.byref(s), C.byref(h)), ctx.h)
         self.h = h
@@ -360,6 +371,16 @@ class ZScoreMap:
         vp = lambda a: a.ctypes.data_as(C.c_void_p)  # noqa: E731
         N.check(self.lib.bw_smap_apply(self.h, vp(keys), vp(vals), n, vp(mu), vp(sigma), vp(flag)), self.ctx.h)
         return mu, sigma, flag.astype(bool)
+
+    def apply_device(self, d_keys: int, d_vals: int, rows: int, d_mu: int, d_sigma: int, d_flag: int):
+        """One activation from device columns (u64 keys, f32 / f64 values) into device columns (f64 mu, f64 sigma, u8
+        flag), aligned with the input rows.  On one rank it returns once the work is enqueued (``sync`` waits); sharded
+        by key it returns once the call is complete."""
+        N.check(self.lib.bw_smap_apply_device(self.h, C.c_void_p(d_keys), C.c_void_p(d_vals), rows, C.c_void_p(d_mu),
+                                              C.c_void_p(d_sigma), C.c_void_p(d_flag)), self.ctx.h)
+
+    def sync(self):
+        N.check(self.lib.bw_smap_sync(self.h), self.ctx.h)
 
     def close(self):
         if self.h:

@@ -325,7 +325,27 @@ bw_status bw_gen_c1(bw_fold* fold, uint64_t* d_keys, uint64_t* d_vals, uint64_t 
  * (pysrc/bytewax/operators/__init__.py:1024-1042, 2860-2890) behind src/operators.rs:755-806:
  * per key, in arrival order: flag = |v - mu| / sigma > threshold on the statistics BEFORE the
  * push (false while mu or sigma is None or 0.0), then push v into the last-`window` ring and
- * recompute mu = sum/len, sigma = sqrt(sum((x - mu)^2)/len), both newest -> oldest. */
+ * recompute mu = sum/len, sigma = sqrt(sum((x - mu)^2)/len), both newest -> oldest.
+ *
+ * On a context with world W > 1 the map is rank-local unless the spec sets shard_by_key: each rank keeps its own ring
+ * for every key it sees, so the caller routes keys (every row of a key to one rank).  With shard_by_key it is sharded
+ * by key (all of its state is per key):
+ *  - bw_smap_create is collective (every rank calls it with the same spec).  Each rank holds a receive region of
+ *    W x max_batch_rows rows of key, value and source row, plus a return section of max_batch_rows rows of mu, sigma
+ *    and flag, shared with every peer over peer memory (CUDA IPC mappings under NCCL, plain pointers on a loopback
+ *    world); bw_smap_destroy closes the mappings, once no rank calls any more.  max_batch_rows x W must be below 2^31
+ *    (BW_ERR_SPEC, before any collective): an owner groups with 32-bit sort indices.
+ *  - bw_smap_apply and bw_smap_apply_device are collective: every rank calls one of them once per activation with its
+ *    own rows (possibly none).  Each row goes to rank bw_route(key, W), the owner the window fold uses, which maps what
+ *    it received in (source rank, source order) and stores each row's mu, sigma and flag back into its source rank's
+ *    return section at the row's index.  Both calls block until the call is complete on this rank (apply_device too:
+ *    bw_smap_sync then only re-reports).
+ *  - A call that cannot go ahead on one rank (rows > max_batch_rows, a NULL column, a map already failed) still takes
+ *    part in the exchange, so that no rank is left waiting: that rank returns its own error, every other rank
+ *    BW_ERR_STATE, and no rank maps the call.  A full key table on an owner fails the call on every rank: the owner
+ *    returns BW_ERR_CAPACITY, every other rank BW_ERR_STATE, and from then on every call returns BW_ERR_STATE.
+ *  - Concatenating every rank's outputs rank-major gives, bit for bit, what a world-1 map returns when fed the
+ *    rank-major concatenation of every rank's columns: row (r, i) is world-1 row offset_r + i. */
 typedef struct bw_smap bw_smap;
 typedef struct bw_smap_spec {
   uint32_t struct_size;
@@ -335,6 +355,9 @@ typedef struct bw_smap_spec {
   double threshold;    /* the example uses 2.0 */
   uint64_t capacity_hint;
   uint64_t max_batch_rows;
+  int32_t shard_by_key; /* world > 1: 1 shards the map by key over the ranks (above), 0 keeps it rank-local; ignored on
+                           world 1.  A spec whose struct_size ends before this field has it 0 */
+  int32_t reserved2;
 } bw_smap_spec;
 bw_status bw_smap_create(bw_ctx* ctx, const bw_smap_spec* spec, bw_smap** out);
 void bw_smap_destroy(bw_smap* m);
