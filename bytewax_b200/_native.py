@@ -112,7 +112,8 @@ class BwJwinSpec(C.Structure):
     _fields_ = [("struct_size", C.c_uint32), ("insert_mode", C.c_int32), ("emit_mode", C.c_int32), ("ordered", C.c_int32),
                 ("sides", C.c_int32), ("max_windows_per_key", C.c_int32), ("length_us", C.c_int64), ("offset_us", C.c_int64),
                 ("align_us", C.c_int64), ("wait_us", C.c_int64), ("capacity_hint", C.c_uint64), ("max_queued_rows", C.c_uint64),
-                ("max_batch_rows", C.c_uint64), ("max_emit_rows", C.c_uint64), ("max_late_rows", C.c_uint64)]
+                ("max_batch_rows", C.c_uint64), ("max_emit_rows", C.c_uint64), ("max_late_rows", C.c_uint64), ("shard_by_key", C.c_int32),
+                ("reserved", C.c_int32)]
 
 
 class BwJwinRows(C.Structure):
@@ -122,7 +123,7 @@ class BwJwinRows(C.Structure):
                 ("meta_epoch", C.POINTER(C.c_uint64)),
                 ("n_late", C.c_uint64), ("late_key", C.POINTER(C.c_uint64)), ("late_window_id", C.POINTER(C.c_int64)),
                 ("late_epoch", C.POINTER(C.c_uint64)), ("late_activation", C.POINTER(C.c_uint64)), ("late_row", C.POINTER(C.c_uint64)),
-                ("n_released", C.c_uint64), ("released", C.POINTER(C.c_uint64))]
+                ("n_released", C.c_uint64), ("released", C.POINTER(C.c_uint64)), ("late_rank", C.POINTER(C.c_uint64))]
 
 
 class BwPjwinSpec(C.Structure):

@@ -39,6 +39,11 @@ struct PartOut {
   u64 region_cap;
   u32* rows[BW_MAX_WORLD];    // k_part_scatter<true>: each row's index in this rank's columns
 };
+// k_part_scatter<true, true>: a one-byte column that travels with the rows (the side of a windowed join row, K8)
+struct PartSide {
+  const unsigned char* src;         // this rank's column
+  unsigned char* dst[BW_MAX_WORLD];  // destination d's region for this source rank
+};
 
 __device__ __forceinline__ u32 bw_dest_of(u64 key, int world) { return bw_route_hash(bw_mix64(key), (u32)world); }
 
@@ -116,9 +121,12 @@ __global__ void __launch_bounds__(1024) k_part_scan(u64 n, int world, u32* tile_
 // warp-sized fragments -- the fragmented version reached ~200 GB/s over NVLink.
 // SRC_ROW adds a fourth column, each row's index i in the source columns (u32), for an owner that must name the rows it
 // received (K7 on N ranks); the dynamic shared memory then grows from BW_PART_TILE x 24 to BW_PART_TILE x 28 bytes.
-template <bool SRC_ROW>
+// SIDE (with SRC_ROW) adds a fifth column, one byte per row from `side` (K8 on N ranks), and BW_PART_TILE more bytes of
+// dynamic shared memory; without it `side` is not read.
+template <bool SRC_ROW, bool SIDE = false>
 __global__ void __launch_bounds__(BW_PART_THREADS)
-k_part_scatter(PartIn in, const u32* tile_off, PartOut out) {
+k_part_scatter(PartIn in, const u32* tile_off, PartOut out, PartSide side) {
+  static_assert(SRC_ROW || !SIDE, "the side column follows the source rows");
   // [iteration][warp][dest] counts, scanned in (iteration, warp) order per dest
   __shared__ u32 cnt[BW_PART_PER_THREAD][BW_PART_THREADS / 32][BW_MAX_WORLD];
   __shared__ u32 tot[BW_MAX_WORLD], dstart[BW_MAX_WORLD + 1];
@@ -127,6 +135,7 @@ k_part_scatter(PartIn in, const u32* tile_off, PartOut out) {
   unsigned char* s_vals = stage_raw + (size_t)BW_PART_TILE * 8;
   i64* s_ts = (i64*)(s_vals + (size_t)BW_PART_TILE * (in.val_bytes ? in.val_bytes : 0));
   u32* s_row = (u32*)(s_ts + (in.ts ? BW_PART_TILE : 0));
+  unsigned char* s_side = (unsigned char*)(s_row + BW_PART_TILE);
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const u32 lt = (1u << lane) - 1u;
   const u64 ntiles = (in.n + BW_PART_TILE - 1) / BW_PART_TILE;
@@ -191,6 +200,7 @@ k_part_scatter(PartIn in, const u32* tile_off, PartOut out) {
         }
         if (in.ts) s_ts[lp] = (i64)bw_ld_stream_u64((const u64*)in.ts + i);
         if (SRC_ROW) s_row[lp] = (u32)i;
+        if (SIDE) s_side[lp] = side.src[i];
       }
     }
     __syncthreads();
@@ -215,16 +225,21 @@ k_part_scatter(PartIn in, const u32* tile_off, PartOut out) {
         u32* gr = out.rows[d] + g0;
         for (u32 e = threadIdx.x; e < n_d; e += BW_PART_THREADS) gr[e] = s_row[s0 + e];
       }
+      if (SIDE) {
+        unsigned char* gs = side.dst[d] + g0;
+        for (u32 e = threadIdx.x; e < n_d; e += BW_PART_THREADS) gs[e] = s_side[s0 + e];
+      }
     }
     __syncthreads();
   }
 }
 // Instantiated here, before any kernel that declares its dynamic shared memory with a stricter alignment (bw_stream.cuh
 // asks for 128 bytes): instantiated at the end of the translation unit, the staging would start at that alignment too.
-template __global__ void k_part_scatter<false>(PartIn, const u32*, PartOut);
-template __global__ void k_part_scatter<true>(PartIn, const u32*, PartOut);
+template __global__ void k_part_scatter<false>(PartIn, const u32*, PartOut, PartSide);
+template __global__ void k_part_scatter<true>(PartIn, const u32*, PartOut, PartSide);
+template __global__ void k_part_scatter<true, true>(PartIn, const u32*, PartOut, PartSide);
 
-// Keyed kernels on N ranks (K6, K7; RankXchg in bwgpu.cu): what a source publishes beside its row count in every owner's
+// Keyed kernels on N ranks (K6, K7, K8; RankXchg in bwgpu.cu): what a source publishes beside its row count in every owner's
 // region head, so that every owner can check that all ranks play the same call.  at[d] is this source's column in rank
 // d's head; rows 1-3 of the head take the epoch, the system time and the refusal flag (row 0, the count, is
 // k_part_scan's).

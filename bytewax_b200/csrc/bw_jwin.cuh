@@ -378,6 +378,38 @@ __global__ void k_jwin_apply(JwTable t, JwEmit e, JwParams p, JwPool pool, u64 b
   }
 }
 
+// K8 on world > 1, at the owner: the received segments (bv.h_counts rows from each source) into K8's columns in (source
+// rank, source order), the arrival order a world-1 join sees when it is fed the rank-major concatenation.  The handle
+// travels in the value column, the side in the region's side column; name[i] = source rank << 32 | the row's index in
+// that source's columns (src_row, src_side: the region's row and side columns, `cap` rows per source).
+__global__ void k_xjwin_gather(BatchView bv, const u32* src_row, const unsigned char* src_side, u64 cap, u64 n, u64* keys, u64* handles,
+                               unsigned char* side, i64* ts, u64* name) {
+  for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (u64)gridDim.x * blockDim.x) {
+    int r = 0;
+    u64 o = i;
+    while (o >= bv.h_counts[r]) o -= bv.h_counts[r++];
+    keys[i] = bv.keys[r][o];
+    handles[i] = ((const u64*)bv.vals[r])[o];
+    side[i] = src_side[(u64)r * cap + o];
+    ts[i] = bv.ts[r][o];
+    name[i] = (u64)r << 32 | src_row[(u64)r * cap + o];
+  }
+}
+
+// After k_jwin_apply on world > 1: the late rows this call added, [*before, *n_late), hold positions in the gathered
+// columns (below n); give them their rows' names instead.  Names grow with the position, so arrival order holds.  A
+// late item reserves one row per window id, all or none (bw_jw_late_rows): when a reservation crossed max_late, the
+// slots it left unwritten still hold an earlier call's names, so nothing is renamed -- the call has failed
+// (BW_JW_FULL_LATE) and its late rows are never handed out.
+__global__ void k_xjwin_name_late(const unsigned long long* before, const unsigned long long* n_late, u64 max_late, u64* l_row,
+                                  const u64* name, u64 n) {
+  if (*n_late > max_late) return;
+  for (u64 i = *before + (u64)blockIdx.x * blockDim.x + threadIdx.x; i < *n_late; i += (u64)gridDim.x * blockDim.x) {
+    const u64 p = l_row[i];
+    if (p < n) l_row[i] = name[p];  // (always, when no reservation failed)
+  }
+}
+
 // notify_at of the sliding windower's keys (the default of k_jwin_mark)
 struct JwNotifyAt {
   template <class W>

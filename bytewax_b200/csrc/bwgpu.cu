@@ -1207,7 +1207,7 @@ static bw_status exchange(bw_fold* f, const u64* d_keys, const void* d_vals, con
   k_part_hist<<<grid, BW_PART_THREADS, 0, s>>>(in, f->d_tile_counts);
   k_part_scan<<<W, 1024, 0, s>>>(rows, W, f->d_tile_counts, po, f->d_ctr);
   const size_t stage_bytes = (size_t)BW_PART_TILE * (8 + (size_t)in.val_bytes + (in.ts ? 8 : 0));
-  k_part_scatter<false><<<grid, BW_PART_THREADS, stage_bytes, s>>>(in, f->d_tile_counts, po);
+  k_part_scatter<false><<<grid, BW_PART_THREADS, stage_bytes, s>>>(in, f->d_tile_counts, po, PartSide{});
   CU(ctx, cudaGetLastError());
   f->st.kernel_launches += 3;
   char* mine = (char*)f->xchg_base;
@@ -2411,11 +2411,11 @@ static bw_status keyed_group(bw_ctx* ctx, KeyedScratch& k, const u64* d_keys, u6
   return BW_OK;
 }
 
-// ---- keyed kernels on N ranks (K5, K6, K7): every row to its key's owner ----
+// ---- keyed kernels on N ranks (K5, K6, K7, K8): every row to its key's owner ----
 // One rank's receive region: a 256-byte head of four rows of BW_MAX_WORLD u64 -- per source rank r: the rows r sent
 // here, the epoch, the system time and the refusal flag r published (k_xchg_head) -- then source r's keys, values and ts
-// (8 bytes each, the partition's column widths) and, with source rows, its rows' indices (4 bytes) at [r * cap].  With a
-// return section (a keyed map, K5), 256-byte aligned at the end: this rank's own `cap` rows of mu (f64), sigma (f64),
+// (8 bytes each, the partition's column widths), with source rows its rows' indices (4 bytes) and, with sides, its
+// rows' sides (1 byte; K8) at [r * cap].  With a return section (a keyed map, K5), 256-byte aligned at the end: this rank's own `cap` rows of mu (f64), sigma (f64),
 // the W owners' error words (u32, BW_MAX_WORLD of them) and flag (u8), which owners store into at the row's index.
 // Setup is collective: the region is shared with every rank (coll_share_base).  A call is collective too: send()
 // publishes the head, partitions the source's columns straight into the owners' regions (peer stores), enters a barrier
@@ -2427,8 +2427,8 @@ static bw_status keyed_group(bw_ctx* ctx, KeyedScratch& k, const u64* d_keys, u6
 #define BW_XRET_ROW_BYTES 17  // mu, sigma, flag
 struct RankXchg {
   u64 cap = 0;       // rows per source: max_batch_rows
-  bool src_rows = false;
-  size_t keys_off = 0, vals_off = 0, ts_off = 0, rows_off = 0, ret_off = 0, total = 0;
+  bool src_rows = false, sides = false;
+  size_t keys_off = 0, vals_off = 0, ts_off = 0, rows_off = 0, side_off = 0, ret_off = 0, total = 0;
   int ret_row = 0;   // bytes of a return row: 0 (none) or BW_XRET_ROW_BYTES
   void* base = nullptr;
   void* peer[BW_MAX_WORLD] = {nullptr};  // every rank's region as seen from here
@@ -2437,17 +2437,21 @@ struct RankXchg {
   u32* d_word = nullptr;      // coll_barrier's word
   u64* h_head = nullptr;      // pinned: the head as received
 
-  bw_status setup(bw_ctx* ctx, Owner& own, u64 max_batch_rows, bool with_src_rows, int ret_row_bytes, cudaStream_t s) {
+  // with_sides needs with_src_rows (k_part_scatter<true, true>)
+  bw_status setup(bw_ctx* ctx, Owner& own, u64 max_batch_rows, bool with_src_rows, bool with_sides, int ret_row_bytes, cudaStream_t s) {
     if (ret_row_bytes != 0 && ret_row_bytes != BW_XRET_ROW_BYTES) CTX_FAIL(ctx, BW_ERR_SPEC, "RankXchg: bad return row width");
+    if (with_sides && !with_src_rows) CTX_FAIL(ctx, BW_ERR_SPEC, "RankXchg: sides travel only with source rows");
     cap = max_batch_rows;
     src_rows = with_src_rows;
+    sides = with_sides;
     ret_row = ret_row_bytes;
     const size_t col = (size_t)cap * ctx->world;
     keys_off = 4 * BW_MAX_WORLD * sizeof(u64);
     vals_off = keys_off + col * 8;
     ts_off = vals_off + col * 8;
     rows_off = ts_off + col * 8;
-    total = rows_off + (src_rows ? col * 4 : 0);
+    side_off = rows_off + (src_rows ? col * 4 : 0);
+    total = side_off + (sides ? col : 0);
     if (ret_row) {
       ret_off = (total + 255) & ~(size_t)255;
       total = ret_off + (size_t)cap * ret_row + BW_MAX_WORLD * sizeof(u32);
@@ -2460,8 +2464,8 @@ struct RankXchg {
     CU(ctx, own.host(&h_head, 4 * BW_MAX_WORLD));
     CU(ctx, cudaMemsetAsync(d_ctr, 0, sizeof(Counters), s));
     CU(ctx, cudaMemsetAsync(d_word, 0, 4, s));
-    CU(ctx, cudaFuncSetAttribute(src_rows ? k_part_scatter<true> : k_part_scatter<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                 BW_PART_TILE * (src_rows ? 28 : 24)));
+    CU(ctx, cudaFuncSetAttribute(sides ? k_part_scatter<true, true> : src_rows ? k_part_scatter<true> : k_part_scatter<false>,
+                                 cudaFuncAttributeMaxDynamicSharedMemorySize, BW_PART_TILE * (sides ? 29 : src_rows ? 28 : 24)));
     CU(ctx, cudaStreamSynchronize(s));
     return coll_share_base(ctx, base, peer, s);
   }
@@ -2472,11 +2476,15 @@ struct RankXchg {
   }
   // head row `row` (0 rows, 1 epoch, 2 system time, 3 refusal flag), one entry per source rank
   const u64* head(int row) const { return h_head + row * BW_MAX_WORLD; }
-  bw_status send(bw_ctx* ctx, cudaStream_t s, const PartIn& in, u64 epoch, i64 now, bool refused) {
+  // `side`: the source's side column, set up with sides (it may be NULL when in.n is 0)
+  bw_status send(bw_ctx* ctx, cudaStream_t s, const PartIn& in, u64 epoch, i64 now, bool refused, const unsigned char* side = nullptr) {
     const int W = ctx->world, R = ctx->rank;
     PartOut po;
     memset(&po, 0, sizeof po);
     po.region_cap = cap;
+    PartSide ps;
+    memset(&ps, 0, sizeof ps);
+    ps.src = side;
     XchgHead pub;
     for (int d = 0; d < W; ++d) {
       char* b = (char*)peer[d];
@@ -2486,15 +2494,17 @@ struct RankXchg {
       po.vals[d] = (u64*)(b + vals_off) + (size_t)R * cap;
       po.ts[d] = (i64*)(b + ts_off) + (size_t)R * cap;
       if (src_rows) po.rows[d] = (u32*)(b + rows_off) + (size_t)R * cap;
+      if (sides) ps.dst[d] = (unsigned char*)(b + side_off) + (size_t)R * cap;
     }
     const u64 ntiles = (in.n + BW_PART_TILE - 1) / BW_PART_TILE;
     const int grid = (int)std::min<u64>(std::max<u64>(ntiles, 1), (u64)ctx->sm_count * 8);
-    const size_t stage = (size_t)BW_PART_TILE * (8 + in.val_bytes + (in.ts ? 8 : 0) + (src_rows ? 4 : 0));
+    const size_t stage = (size_t)BW_PART_TILE * (8 + in.val_bytes + (in.ts ? 8 : 0) + (src_rows ? 4 : 0) + (sides ? 1 : 0));
     k_xchg_head<<<1, 32, 0, s>>>(pub, W, epoch, now, refused ? 1 : 0);
     k_part_hist<<<grid, BW_PART_THREADS, 0, s>>>(in, d_tile_counts);
     k_part_scan<<<W, 1024, 0, s>>>(in.n, W, d_tile_counts, po, d_ctr);
-    if (src_rows) k_part_scatter<true><<<grid, BW_PART_THREADS, stage, s>>>(in, d_tile_counts, po);
-    else k_part_scatter<false><<<grid, BW_PART_THREADS, stage, s>>>(in, d_tile_counts, po);
+    if (sides) k_part_scatter<true, true><<<grid, BW_PART_THREADS, stage, s>>>(in, d_tile_counts, po, ps);
+    else if (src_rows) k_part_scatter<true><<<grid, BW_PART_THREADS, stage, s>>>(in, d_tile_counts, po, ps);
+    else k_part_scatter<false><<<grid, BW_PART_THREADS, stage, s>>>(in, d_tile_counts, po, ps);
     CU(ctx, cudaGetLastError());
     // every rank's stores are complete once it enters the barrier (stream order)
     bw_status st = coll_barrier(ctx, d_word, s);
@@ -2519,6 +2529,7 @@ struct RankXchg {
     return n;
   }
   const u32* rows() const { return (const u32*)((const char*)base + rows_off); }
+  const unsigned char* side() const { return (const unsigned char*)base + side_off; }
   bw_status done(bw_ctx* ctx, cudaStream_t s) { return coll_barrier(ctx, d_word, s); }
   // the return section of the region at `b` (setup with a return row width)
   XchgRet ret_at(void* b) const {
@@ -2605,7 +2616,7 @@ bw_status bw_smap_create(bw_ctx* ctx, const bw_smap_spec* user, bw_smap** out) {
   if (shard) {
     CU(ctx, own.dev(&m->d_name, n));
     CU(ctx, own.host(&m->h_ret_err, BW_MAX_WORLD));
-    st = m->x.setup(ctx, own, spec->max_batch_rows, true, BW_XRET_ROW_BYTES, m->s);
+    st = m->x.setup(ctx, own, spec->max_batch_rows, true, false, BW_XRET_ROW_BYTES, m->s);
     if (st != BW_OK) return st;
   }
   *out = mp.release();
@@ -2797,7 +2808,7 @@ static bw_status join_ranks_setup(bw_join* j) {
   CU(ctx, own.dev(&j->d_src_vals, B));
   CU(ctx, own.dev(&j->d_src_side, B));
   CU(ctx, own.dev(&j->d_src_side64, B));
-  return j->x.setup(ctx, own, B, false, 0, j->s);
+  return j->x.setup(ctx, own, B, false, false, 0, j->s);
 }
 
 bw_status bw_join_create(bw_ctx* ctx, const bw_join_spec* spec, bw_join** out) {
@@ -3085,7 +3096,7 @@ bw_status bw_session_create(bw_ctx* ctx, const bw_session_spec* user, bw_session
   if (ctx->world > 1) {
     CU(ctx, own.dev(&f->d_name, n));
     CU(ctx, own.dev(&f->d_late0, 1));
-    st = f->x.setup(ctx, own, spec->max_batch_rows, true, 0, f->s);
+    st = f->x.setup(ctx, own, spec->max_batch_rows, true, false, 0, f->s);
     if (st != BW_OK) return st;
   }
   *out = sp.release();
@@ -3379,6 +3390,7 @@ struct bw_jwin {
   SortScratch srt;       // pool sort and ordering scratch
   HostCols hd[2];        // down: key, window id, h0, h1, h2 | h3, mask, epoch
   HostCols hm, hl;       // meta: key, window id, epoch; late: key, window id, epoch, activation, row
+  std::vector<u64> late_rank;     // the late rows' source ranks, split off their row column
   std::vector<u64> released;      // since the last advance / eof
   std::vector<u64> released_out;  // what the last advance / eof handed out
   bool undrained = false;     // a call whose released handles and queue count are not read back yet
@@ -3388,6 +3400,11 @@ struct bw_jwin {
   u64 last_epoch = 0;
   i64 now = INT64_MIN;
   bool failed = false;
+  // world > 1: the exchange (with source rows and sides), each gathered row's name (source rank << 32 | source row),
+  // and the late row count before a call
+  RankXchg x;
+  u64* d_name = nullptr;
+  unsigned long long* d_late0 = nullptr;
 };
 
 static bw_status jwin_pool_alloc(bw_ctx* ctx, Owner& own, JwPool& p, u64 n) {
@@ -3398,10 +3415,16 @@ static bw_status jwin_pool_alloc(bw_ctx* ctx, Owner& own, JwPool& p, u64 n) {
   return BW_OK;
 }
 
-bw_status bw_jwin_create(bw_ctx* ctx, const bw_jwin_spec* spec, bw_jwin** out) {
-  if (!ctx || !spec || !out) CTX_FAIL(ctx, BW_ERR_SPEC, "bw_jwin_create: NULL argument");
-  if (spec->struct_size != sizeof(bw_jwin_spec)) CTX_FAIL(ctx, BW_ERR_SPEC, "bw_jwin_spec.struct_size mismatch");
-  if (ctx->world != 1) CTX_FAIL(ctx, BW_ERR_SPEC, "windowed joins run on one GPU (world == 1)");
+bw_status bw_jwin_create(bw_ctx* ctx, const bw_jwin_spec* user, bw_jwin** out) {
+  if (!ctx || !user || !out) CTX_FAIL(ctx, BW_ERR_SPEC, "bw_jwin_create: NULL argument");
+  // a spec built against the header before shard_by_key existed ends just before it, and leaves it 0
+  if (user->struct_size != sizeof(bw_jwin_spec) && user->struct_size != offsetof(bw_jwin_spec, shard_by_key))
+    CTX_FAIL(ctx, BW_ERR_SPEC, "bw_jwin_spec.struct_size mismatch");
+  bw_jwin_spec copy{};
+  memcpy(&copy, user, user->struct_size);
+  const bw_jwin_spec* spec = &copy;
+  if (ctx->world != 1 && !spec->shard_by_key)
+    CTX_FAIL(ctx, BW_ERR_SPEC, "windowed joins run on one GPU (world == 1) unless the spec sets shard_by_key");
   if (spec->insert_mode != BW_JOIN_INSERT_FIRST && spec->insert_mode != BW_JOIN_INSERT_LAST)
     CTX_FAIL(ctx, BW_ERR_SPEC, "insert_mode must be first or last (product: host engine)");
   if (spec->emit_mode < BW_JOIN_EMIT_COMPLETE || spec->emit_mode > BW_JOIN_EMIT_RUNNING) CTX_FAIL(ctx, BW_ERR_SPEC, "bad emit_mode");
@@ -3413,8 +3436,11 @@ bw_status bw_jwin_create(bw_ctx* ctx, const bw_jwin_spec* spec, bw_jwin** out) {
   if (spec->offset_us <= 0 || spec->offset_us > spec->length_us) CTX_FAIL(ctx, BW_ERR_SPEC, "offset_us must be in 1..length_us");
   if (spec->align_us < BW_UTC_MIN_US || spec->align_us > BW_UTC_MAX_US) CTX_FAIL(ctx, BW_ERR_SPEC, "align_us out of range");
   if (spec->wait_us < 0) CTX_FAIL(ctx, BW_ERR_SPEC, "wait_us must not be negative");
-  if (spec->max_batch_rows == 0 || spec->max_batch_rows >= (1ULL << 31)) CTX_FAIL(ctx, BW_ERR_SPEC, "bad max_batch_rows");
-  if (spec->max_queued_rows >= (1ULL << 31) - spec->max_batch_rows) CTX_FAIL(ctx, BW_ERR_SPEC, "max_queued_rows + max_batch_rows must stay below 2^31");
+  // an owner groups and sorts up to max_batch_rows from every rank, and its pool, with 32-bit indices
+  if (spec->max_batch_rows == 0 || spec->max_batch_rows > ((1ULL << 31) - 1) / (u64)ctx->world)
+    CTX_FAIL(ctx, BW_ERR_SPEC, "bad max_batch_rows: max_batch_rows * world must be in [1, 2^31)");
+  if (spec->max_queued_rows >= (1ULL << 31) - spec->max_batch_rows * (u64)ctx->world)
+    CTX_FAIL(ctx, BW_ERR_SPEC, "max_queued_rows + max_batch_rows * world must stay below 2^31");
   if (spec->capacity_hint >= (1ULL << 30)) CTX_FAIL(ctx, BW_ERR_SPEC, "capacity_hint must be below 2^30");
   CU(ctx, cudaSetDevice(ctx->device));
   std::unique_ptr<bw_jwin, void (*)(bw_jwin*)> jp(new bw_jwin(), bw_jwin_destroy);  // torn down on every failure
@@ -3440,7 +3466,8 @@ bw_status bw_jwin_create(bw_ctx* ctx, const bw_jwin_spec* spec, bw_jwin** out) {
   CU(ctx, cudaMemsetAsync(j->d_cnt, 0, 40, j->s));
   CU(ctx, own.host(&j->h_err, 64 / sizeof(u32)));
   CU(ctx, own.host(&j->h_cnt, 64 / sizeof(unsigned long long)));
-  const u64 n = spec->max_batch_rows, m = std::max<u64>(spec->max_emit_rows, 1), l = std::max<u64>(spec->max_late_rows, 1);
+  // rows one activation brings to this rank: its own on one GPU, up to max_batch_rows from every rank on world > 1
+  const u64 n = spec->max_batch_rows * (u64)ctx->world, m = std::max<u64>(spec->max_emit_rows, 1), l = std::max<u64>(spec->max_late_rows, 1);
   const u64 q = spec->ordered ? spec->max_queued_rows : 0;
   bw_status st = keyed_alloc(ctx, own, j->k, n, j->s);
   if (st != BW_OK) return st;
@@ -3476,6 +3503,12 @@ bw_status bw_jwin_create(bw_ctx* ctx, const bw_jwin_spec* spec, bw_jwin** out) {
   k_jwin_init<<<ctx->sm_count * 4, 256, 0, j->s>>>(t);
   CU(ctx, cudaGetLastError());
   CU(ctx, cudaStreamSynchronize(j->s));
+  if (ctx->world > 1) {
+    CU(ctx, own.dev(&j->d_name, n));
+    CU(ctx, own.dev(&j->d_late0, 1));
+    st = j->x.setup(ctx, own, spec->max_batch_rows, true, true, 0, j->s);
+    if (st != BW_OK) return st;
+  }
   *out = jp.release();
   return BW_OK;
 }
@@ -3484,6 +3517,7 @@ void bw_jwin_destroy(bw_jwin* j) {
   if (!j) return;
   cudaSetDevice(j->ctx->device);
   if (j->s) cudaStreamSynchronize(j->s);
+  j->x.close(j->ctx);
   delete j;  // j->own releases every buffer and the stream
 }
 
@@ -3608,10 +3642,116 @@ static bw_status jwin_flush_pool(bw_jwin* j, const JwParams& p, u64 n) {
   });
 }
 
+// bw_jwin_apply / _apply_device on world > 1 (include/bwgpu.h): every row to its key's owner, then K8 there over what
+// arrived.  `host`: the columns are host memory.
+static bw_status jwin_apply_ranks(bw_jwin* j, const u64* keys, const uint8_t* side, const u64* handles, const i64* ts_us, u64 rows,
+                                  u64 epoch, i64 system_now_us, bool host) {
+  bw_ctx* ctx = j->ctx;
+  const int W = ctx->world;
+  cudaStream_t s = j->s;
+  CU(ctx, cudaSetDevice(ctx->device));
+  // A call that cannot go ahead still takes part in the exchange and both barriers, so that no peer waits for it in a
+  // barrier: it sends no rows and raises its refusal flag, and every rank then fails the call.
+  bw_status refuse = BW_OK;
+  std::string why;
+  if (j->failed) {
+    refuse = BW_ERR_STATE;
+    why = "windowed join: an earlier call failed on the device; the join is unusable";
+  } else if (rows > j->spec.max_batch_rows) {
+    refuse = BW_ERR_SPEC;
+    why = "windowed join: rows > max_batch_rows";
+  } else if (rows && (!keys || !side || !handles || !ts_us)) {
+    refuse = BW_ERR_SPEC;
+    why = "windowed join: NULL column";
+  } else if (j->batch_no && epoch < j->last_epoch) {
+    refuse = BW_ERR_STATE;
+    why = "windowed join: epochs must not decrease";
+  } else if ((refuse = jwin_drain(j)) != BW_OK) {  // a device error met by an earlier apply_device
+    why = ctx->err;
+  }
+  for (u64 i = 0; host && refuse == BW_OK && i < rows; ++i)
+    if (side[i] >= (u32)j->spec.sides) {
+      refuse = BW_ERR_SPEC;
+      why = "windowed join: side " + std::to_string(side[i]) + " of row " + std::to_string(i) + " is not below sides";
+    }
+  if (refuse != BW_OK) rows = 0;
+  PartIn in;
+  in.keys = keys;
+  in.vals = handles;
+  in.ts = ts_us;
+  in.n = rows;
+  in.val_bytes = 8;
+  in.world = W;
+  const unsigned char* in_side = side;
+  if (host && rows) {  // staged in K8's own columns: the gather overwrites them only after the scatter has read them
+    CU(ctx, cudaMemcpyAsync(j->k.d_keys, keys, rows * 8, cudaMemcpyHostToDevice, s));
+    CU(ctx, cudaMemcpyAsync(j->d_side, side, rows, cudaMemcpyHostToDevice, s));
+    CU(ctx, cudaMemcpyAsync(j->d_handles, handles, rows * 8, cudaMemcpyHostToDevice, s));
+    CU(ctx, cudaMemcpyAsync(j->d_ts, ts_us, rows * 8, cudaMemcpyHostToDevice, s));
+    in.keys = j->k.d_keys;
+    in.vals = j->d_handles;
+    in.ts = j->d_ts;
+    in_side = j->d_side;
+  }
+  bw_status st = j->x.send(ctx, s, in, epoch, system_now_us, refuse != BW_OK, in_side);
+  if (st != BW_OK) return st;
+  // every rank reads the same head: all of them fail here, or none does
+  const u64 *got_epoch = j->x.head(1), *got_now = j->x.head(2), *got_refused = j->x.head(3);
+  int refused = -1, epoch_differs = -1, now_differs = -1;
+  for (int r = W - 1; r >= 0; --r) {
+    if (got_refused[r]) refused = r;
+    if (got_epoch[r] != got_epoch[0]) epoch_differs = r;
+    if (got_now[r] != got_now[0]) now_differs = r;
+  }
+  const bool go = refused < 0 && epoch_differs < 0 && now_differs < 0;
+  u64 n = 0;
+  if (go) {
+    BatchView bv;
+    n = j->x.received(ctx, bv);
+    if (n)
+      k_xjwin_gather<<<ctx->sm_count * 4, 256, 0, s>>>(bv, j->x.rows(), j->x.side(), j->spec.max_batch_rows, n, j->k.d_keys, j->d_handles,
+                                                       j->d_side, j->d_ts, j->d_name);
+    CU(ctx, cudaGetLastError());
+  }
+  st = j->x.done(ctx, s);
+  if (st != BW_OK) return st;
+  if (refuse != BW_OK) CTX_FAIL(ctx, refuse, "%s", why.c_str());
+  if (refused >= 0) CTX_FAIL(ctx, BW_ERR_STATE, "windowed join: rank %d refused this call (its own error says why); no rank played it", refused);
+  if (epoch_differs >= 0)
+    CTX_FAIL(ctx, BW_ERR_STATE,
+             "windowed join: rank 0 played epoch %llu and rank %d epoch %llu; every rank must pass the same epoch to one call",
+             (unsigned long long)got_epoch[0], epoch_differs, (unsigned long long)got_epoch[epoch_differs]);
+  if (now_differs >= 0)
+    CTX_FAIL(ctx, BW_ERR_STATE,
+             "windowed join: rank 0 passed system_now_us %lld and rank %d %lld; every rank must pass the same system time to one call",
+             (long long)got_now[0], now_differs, (long long)got_now[now_differs]);
+  j->last_epoch = epoch;
+  if (system_now_us > j->now) j->now = system_now_us;  // `now_getter()` never goes backwards (windowing.py:250-261)
+  const JwParams p = jwin_params(j, epoch);
+  j->batch_no++;
+  if (n) {
+    // the n rows received (not max_batch_rows x W): the release buffer holds what the join holds
+    if ((st = jwin_room(j, n)) != BW_OK) return st;
+    j->outstanding += n;
+    st = keyed_group(ctx, j->k, j->k.d_keys, n, s);
+    if (st != BW_OK) return st;
+    CU(ctx, cudaMemcpyAsync(j->d_late0, j->e.n_late, 8, cudaMemcpyDeviceToDevice, s));
+    k_jwin_apply<<<ctx->sm_count * 8, 256, 0, s>>>(j->t, j->e, p, j->pool, j->nq, j->k.d_ksorted, j->k.d_isorted, j->k.d_head, j->d_handles,
+                                                   j->d_side, j->d_ts, j->d_late, n);
+    k_xjwin_name_late<<<ctx->sm_count * 4, 256, 0, s>>>(j->d_late0, j->e.n_late, j->e.max_late, j->e.l_row, j->d_name, n);
+    CU(ctx, cudaGetLastError());
+    j->undrained = true;
+    if (j->spec.ordered && (st = jwin_flush_pool(j, p, j->nq + n)) != BW_OK) return st;
+  }
+  // the host columns may be reused by the caller once this returns
+  return host ? jwin_drain(j) : BW_OK;
+}
+
 bw_status bw_jwin_apply_device(bw_jwin* j, const uint64_t* d_keys, const uint8_t* d_side, const uint64_t* d_handles, const int64_t* d_ts_us,
                                uint64_t rows, uint64_t epoch, int64_t system_now_us) {
   if (!j) return BW_ERR_SPEC;
   bw_ctx* ctx = j->ctx;
+  if (ctx->world > 1) return jwin_apply_ranks(j, d_keys, d_side, d_handles, d_ts_us, rows, epoch, system_now_us, false);
   JWIN_REFUSE_FAILED(j);
   if (rows > j->spec.max_batch_rows) CTX_FAIL(ctx, BW_ERR_SPEC, "windowed join: rows > max_batch_rows");
   if (rows && (!d_keys || !d_side || !d_handles || !d_ts_us)) CTX_FAIL(ctx, BW_ERR_SPEC, "windowed join: NULL column");
@@ -3665,6 +3805,7 @@ static bw_status jwin_apply_host(J* j, const uint64_t* keys, const uint8_t* side
 
 bw_status bw_jwin_apply(bw_jwin* j, const uint64_t* keys, const uint8_t* side, const uint64_t* handles, const int64_t* ts_us, uint64_t rows,
                         uint64_t epoch, int64_t system_now_us) {
+  if (j && j->ctx->world > 1) return jwin_apply_ranks(j, keys, side, handles, ts_us, rows, epoch, system_now_us, true);
   return jwin_apply_host(j, keys, side, handles, ts_us, rows, epoch, system_now_us, bw_jwin_apply_device);
 }
 
@@ -3700,6 +3841,13 @@ static bw_status jwin_collect(bw_jwin* j, bw_jwin_rows* out) {
   CU(ctx, cudaGetLastError());
   CU(ctx, cudaMemsetAsync(j->d_cnt, 0, 24, j->s));
   CU(ctx, cudaStreamSynchronize(j->s));
+  // the row column holds names, source rank << 32 | source row (on world 1 the rank is 0)
+  u64* lrow = j->hl.col[4];
+  j->late_rank.resize(nl);
+  for (u64 i = 0; i < nl; ++i) {
+    j->late_rank[i] = lrow[i] >> 32;
+    lrow[i] &= 0xffffffffULL;
+  }
   j->first_call = j->calls;
   out->n_down = nd;
   out->down_key = j->hd[0].col[0];
@@ -3720,6 +3868,7 @@ static bw_status jwin_collect(bw_jwin* j, bw_jwin_rows* out) {
   out->late_epoch = j->hl.col[2];
   out->late_activation = j->hl.col[3];
   out->late_row = j->hl.col[4];
+  out->late_rank = j->late_rank.data();
   // handed out until the next advance / eof, then cleared
   j->released.swap(j->released_out);
   j->released.clear();
@@ -5472,6 +5621,7 @@ struct bw_pjwin {
   u64 rows_cap = 0;
   HostCols hd[2];                      // down: key, window id, h0, h1, h2 | h3, mask, epoch
   HostCols hm, hl;                     // meta: key, window id, epoch; late: key, window id, epoch, activation, row
+  std::vector<u64> late_rank;          // the late rows' source ranks: all zeros (one GPU)
   std::vector<u64> released;           // since the last advance / eof
   std::vector<u64> released_out;       // what the last advance / eof handed out
   bool undrained = false;     // a call whose counts are not read back yet
@@ -5857,6 +6007,8 @@ static bw_status pjwin_collect(bw_pjwin* j, bw_jwin_rows* out) {
   out->late_epoch = j->hl.col[2];
   out->late_activation = j->hl.col[3];
   out->late_row = j->hl.col[4];
+  j->late_rank.assign(nl, 0);
+  out->late_rank = j->late_rank.data();
   // handed out until the next advance / eof, then cleared
   j->released.swap(j->released_out);
   j->released.clear();

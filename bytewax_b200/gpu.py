@@ -584,7 +584,8 @@ class JoinWindowRows:
     late_window_id: np.ndarray
     late_epoch: np.ndarray
     late_activation: np.ndarray
-    late_row: np.ndarray
+    late_row: np.ndarray  # the row's index in the columns its source rank passed
+    late_rank: np.ndarray  # that source rank; all zeros on one rank
     released: np.ndarray  # uint64, in no particular order
 
     def tuples(self) -> List[tuple]:
@@ -654,14 +655,24 @@ class _HandleJoin:
 class JoinWindow(_HandleJoin):
     """``join_window`` with insert mode first / last over tumbling or sliding windows (``bw_jwin``, K8;
     windowing.py:1046-1190, 1849-1902).  Values travel as uint64 handles; the caller keeps the objects and may drop
-    each one once it comes back in ``released``."""
+    each one once it comes back in ``released``.
+
+    On a multi-rank context (``world > 1``) the join needs ``shard_by_key=True`` (without it, create raises, as a join
+    that cannot see the other ranks' rows would be wrong); it is then sharded by key and collective: every rank creates
+    it with the same arguments and calls ``apply`` or ``apply_device`` once per activation, with its own rows (possibly
+    none), the same epoch and the same ``system_now_us``.  Each row goes to rank ``bw_route(key, world)``, which joins
+    what arrived in (source rank, source order).  A call one rank cannot make (too many rows, a side out of range, a
+    decreasing epoch, a failed join) fails on every rank, and no rank plays it.  A rank's ``advance`` / ``eof`` return
+    the rows of the keys it owns, and ``released`` lists each handle once, on the owner of its key (handles travel
+    opaquely: put the source rank in the handle if it is needed); a late row names its input row by
+    (``late_activation``, ``late_rank``, ``late_row``).  Close it only once no rank calls it any more."""
 
     _PREFIX, _ROWS = "bw_jwin", N.BwJwinRows
 
     def __init__(self, ctx: Context, insert_mode: str = "last", emit_mode: str = "final", ordered: bool = True, sides: int = 2,
                  length_us: int = 10_000_000, offset_us: Optional[int] = None, align_us: int = 0, wait_us: Optional[int] = 0,
                  capacity_hint: int = 1 << 16, max_windows_per_key: int = 16, max_queued_rows: int = 1 << 20,
-                 max_batch_rows: int = 1 << 20, max_emit_rows: int = 1 << 20, max_late_rows: int = 1 << 20):
+                 max_batch_rows: int = 1 << 20, max_emit_rows: int = 1 << 20, max_late_rows: int = 1 << 20, shard_by_key: bool = False):
         """``offset_us=None``: tumbling.  ``wait_us=None``: the watermark never advances on data (``BW_WAIT_FOREVER``)."""
         s = N.BwJwinSpec()
         s.struct_size = C.sizeof(N.BwJwinSpec)
@@ -671,6 +682,7 @@ class JoinWindow(_HandleJoin):
         s.wait_us = N.BW_WAIT_FOREVER if wait_us is None else wait_us
         s.capacity_hint, s.max_queued_rows, s.max_batch_rows = capacity_hint, max_queued_rows, max_batch_rows
         s.max_emit_rows, s.max_late_rows = max_emit_rows, max_late_rows
+        s.shard_by_key = int(shard_by_key)
         self._create(ctx, s, sides)
 
     def window_bounds(self, window_id: int):
@@ -688,7 +700,7 @@ class JoinWindow(_HandleJoin):
         return JoinWindowRows(arr(r.down_key, nd), arr(r.down_window_id, nd, np.int64), hs, arr(r.down_mask, nd), arr(r.down_epoch, nd),
                               arr(r.meta_key, nm), arr(r.meta_window_id, nm, np.int64), arr(r.meta_epoch, nm),
                               arr(r.late_key, nl), arr(r.late_window_id, nl, np.int64), arr(r.late_epoch, nl),
-                              arr(r.late_activation, nl), arr(r.late_row, nl), arr(r.released, nr))
+                              arr(r.late_activation, nl), arr(r.late_row, nl), arr(r.late_rank, nl), arr(r.released, nr))
 
 
 class ProductJoinWindow(JoinWindow):
@@ -759,12 +771,15 @@ class SessionJoinWindow(_HandleJoin):
 
         hs = np.stack([arr(r.down_handle[s], nd) for s in range(self.sides)], axis=1) if nd else np.zeros((0, self.sides), np.uint64)
         off = arr(r.merged_off, nm + 1).astype(np.int64)
-        return SessionJoinWindowRows(arr(r.down_key, nd), arr(r.down_window_id, nd, np.int64), hs, arr(r.down_mask, nd), arr(r.down_epoch, nd),
-                                     arr(r.meta_key, nm), arr(r.meta_window_id, nm, np.int64), arr(r.meta_epoch, nm),
-                                     arr(r.late_key, nl), np.full(nl, -1, np.int64), arr(r.late_epoch, nl),
-                                     arr(r.late_activation, nl), arr(r.late_row, nl), arr(r.released, nr),
-                                     arr(r.meta_open_us, nm, np.int64), arr(r.meta_close_us, nm, np.int64), off,
-                                     arr(r.merged_ids, int(off[-1]), np.int64))
+        # by keyword: the fields of JoinWindowRows come first (K10 runs on one GPU: its late rows' source rank is 0)
+        return SessionJoinWindowRows(down_key=arr(r.down_key, nd), down_window_id=arr(r.down_window_id, nd, np.int64), down_handles=hs,
+                                     down_mask=arr(r.down_mask, nd), down_epoch=arr(r.down_epoch, nd), meta_key=arr(r.meta_key, nm),
+                                     meta_window_id=arr(r.meta_window_id, nm, np.int64), meta_epoch=arr(r.meta_epoch, nm),
+                                     late_key=arr(r.late_key, nl), late_window_id=np.full(nl, -1, np.int64), late_epoch=arr(r.late_epoch, nl),
+                                     late_activation=arr(r.late_activation, nl), late_row=arr(r.late_row, nl),
+                                     late_rank=np.zeros(nl, np.uint64), released=arr(r.released, nr),
+                                     meta_open_us=arr(r.meta_open_us, nm, np.int64), meta_close_us=arr(r.meta_close_us, nm, np.int64),
+                                     merged_off=off, merged_ids=arr(r.merged_ids, int(off[-1]), np.int64))
 
 
 class SessionProductJoinWindow(SessionJoinWindow):

@@ -525,7 +525,39 @@ bw_status bw_session_eof(bw_session* s, bw_session_rows* out);
  * the tuple and clears the state once every side is set, "running" emits the tuple after every value; then
  * `_handle_closed` (:1087-1093): windows with close <= watermark in first-opened order, each giving the `final` tuple
  * (emit mode final) and then its metadata row.  A key with no open window and an empty queue is discarded, clock state
- * included (:1110-1113, src/operators.rs:796-799).  One GPU only. */
+ * included (:1110-1113, src/operators.rs:796-799).
+ *
+ * On a context with world W > 1 the join runs only when the spec sets shard_by_key (else bw_jwin_create returns
+ * BW_ERR_SPEC, before any collective); it is then sharded by key (the clock, the watermark, the windows, the queue and
+ * the discard of an empty key are all per key):
+ *  - bw_jwin_create is collective (every rank calls it with the same spec).  Each rank holds a receive region of
+ *    W x max_batch_rows rows of key, handle, ts, source row and side (29 B a row), shared with every peer over peer
+ *    memory (CUDA IPC mappings under NCCL, plain pointers on a loopback world); bw_jwin_destroy closes the mappings,
+ *    once no rank calls any more.  Every per-activation buffer of a rank is sized for the W x max_batch_rows rows it
+ *    may receive.  max_batch_rows x W must be below 2^31, and so must max_queued_rows + W x max_batch_rows
+ *    (BW_ERR_SPEC, before any collective).
+ *  - bw_jwin_apply and bw_jwin_apply_device are collective: every rank calls one of them once per activation with its
+ *    own rows (possibly none), the same epoch and the same system_now_us.  Each row goes to rank bw_route(key, W), the
+ *    owner the window fold uses, which joins what it received in (source rank, source order).  Ranks that pass
+ *    different epochs or different system_now_us to one call all get BW_ERR_STATE.  apply_device reads its columns in
+ *    the exchange, before it returns.
+ *  - A call that cannot go ahead on one rank (rows > max_batch_rows, a NULL column, a host side >= sides, a decreasing
+ *    epoch, a join already failed) still takes part in the exchange, so that no rank is left waiting: that rank
+ *    returns its own error, every other rank BW_ERR_STATE, and no rank plays the call.  A full key table, window list,
+ *    queue, emit or late buffer on an owner, or a device side >= sides it received, fails that owner as on one GPU
+ *    (bw_jwin_apply: in that call; apply_device: in the next call or advance), and from then on every rank's apply
+ *    returns BW_ERR_STATE.
+ *  - Handles stay opaque and travel with their rows: an owner's down_handle columns hold handles other ranks passed,
+ *    and each handle is listed in `released` exactly once, on the rank that owns its key, in the call that let go of
+ *    it.  A caller that needs a handle's source rank puts that rank in the handle.
+ *  - bw_jwin_advance (notify phase included) and bw_jwin_eof stay local: rank r flushes and returns the keys it owns.
+ *    As apply is collective, the activation count, the epochs and the system time agree on every rank, so
+ *    late_activation and down_epoch mean the same everywhere.  A late row is named by (late_activation, late_rank,
+ *    late_row): late_row is the row's index in the columns that source rank passed.
+ *  - Taking each call's rows from every rank, concatenating them and stably sorting the down, meta and late columns
+ *    separately by key string gives exactly what a world-1 join returns for that call when it is fed the rank-major
+ *    concatenation of every rank's columns; late row (r, i) is world-1 row offset_r + i, and the union of the ranks'
+ *    `released` is world 1's. */
 typedef struct bw_jwin bw_jwin;
 typedef struct bw_jwin_spec {
   uint32_t struct_size;
@@ -543,6 +575,9 @@ typedef struct bw_jwin_spec {
   uint64_t max_batch_rows;
   uint64_t max_emit_rows;       /* down rows, and meta rows, retained between bw_jwin_advance calls */
   uint64_t max_late_rows;       /* late rows retained between bw_jwin_advance calls */
+  int32_t shard_by_key;         /* world > 1: 1 shards the join by key over the ranks (above); ignored on world 1.  A
+                                   spec whose struct_size ends before this field has it 0 */
+  int32_t reserved;
 } bw_jwin_spec;
 /* Rows handed downstream since the last advance / eof, in the reference's order: per call (activation, notify phase
  * or EOF), ascending key string (src/operators.rs:758-767, :862-894); within a key `down` rows in play order with the
@@ -563,12 +598,15 @@ typedef struct bw_jwin_rows {
   const uint64_t* late_key;
   const int64_t* late_window_id;
   const uint64_t* late_epoch;
-  const uint64_t* late_activation; /* (activation, row) name the input row (activations counted from 0) */
+  const uint64_t* late_activation; /* (activation, row) name the input row (activations counted from 0), with late_rank
+                                      on world > 1 */
   const uint64_t* late_row;
   /* handles no window and no queue entry holds any more; each handle passed to apply is listed exactly once, in the
    * rows of the call that let go of it (late items and values never stored: the call that received them) */
   uint64_t n_released;           /* (the device buffer behind it grows with the handles held, never with the table size) */
   const uint64_t* released;
+  const uint64_t* late_rank;     /* [n_late]: the source rank of late_row on world > 1; all zeros on world 1 (and for
+                                    bw_pjwin_*, which runs on one GPU) */
 } bw_jwin_rows;
 bw_status bw_jwin_create(bw_ctx* ctx, const bw_jwin_spec* spec, bw_jwin** out);
 void bw_jwin_destroy(bw_jwin* j);
