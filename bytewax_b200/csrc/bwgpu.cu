@@ -2870,6 +2870,21 @@ static bw_status join_apply_ranks(bw_join* j, const u64* keys, const uint8_t* si
   const int W = ctx->world;
   cudaStream_t s = j->s;
   CU(ctx, cudaSetDevice(ctx->device));
+  // A call that cannot go ahead still takes part in the exchange and both barriers, so that no peer waits for it in a
+  // barrier: it sends no rows and raises its refusal flag, and every rank then fails the call.
+  bw_status refuse = BW_OK;
+  const char* why = "";
+  if (rows > j->spec.max_batch_rows) {
+    refuse = BW_ERR_SPEC;
+    why = "join: rows > max_batch_rows";
+  } else if (rows && (!keys || !side || !vals)) {
+    refuse = BW_ERR_SPEC;
+    why = "join: NULL column";
+  } else if (j->pending && epoch < j->last_epoch) {
+    refuse = BW_ERR_STATE;
+    why = "join: epochs must not decrease";
+  }
+  if (refuse != BW_OK) rows = 0;
   if (rows) {
     CU(ctx, cudaMemcpyAsync(j->d_src_keys, keys, rows * 8, cudaMemcpyHostToDevice, s));
     CU(ctx, cudaMemcpyAsync(j->d_src_side, side, rows, cudaMemcpyHostToDevice, s));
@@ -2884,27 +2899,39 @@ static bw_status join_apply_ranks(bw_join* j, const u64* keys, const uint8_t* si
   in.world = W;
   const int grid = (int)std::min<u64>(std::max<u64>((rows + BW_PART_TILE - 1) / BW_PART_TILE, 1), (u64)ctx->sm_count * 8);
   k_xjoin_side<<<grid, BW_PART_THREADS, 0, s>>>(j->d_src_side, j->d_src_side64, rows);
-  bw_status st = j->x.send(ctx, s, in, epoch, 0, false);
+  // K6 has no clock: the head's time row carries 0
+  bw_status st = j->x.send(ctx, s, in, epoch, 0, refuse != BW_OK);
   if (st != BW_OK) return st;
-  // every rank reads the same epochs: all of them raise here, or none does
-  const u64* got_epoch = j->x.head(1);
-  for (int r = 0; r < W; ++r)
-    if (got_epoch[r] != got_epoch[0])
-      CTX_FAIL(ctx, BW_ERR_STATE, "join: rank 0 played epoch %llu and rank %d epoch %llu; every rank must pass the same epoch to one call",
-               (unsigned long long)got_epoch[0], r, (unsigned long long)got_epoch[r]);
-  if (j->pending && epoch < j->last_epoch) CTX_FAIL(ctx, BW_ERR_STATE, "join: epochs must not decrease");
+  // every rank reads the same head: all of them fail here, or none does
+  const u64 *got_epoch = j->x.head(1), *got_refused = j->x.head(3);
+  int refused = -1, epoch_differs = -1;
+  for (int r = W - 1; r >= 0; --r) {
+    if (got_refused[r]) refused = r;
+    if (got_epoch[r] != got_epoch[0]) epoch_differs = r;
+  }
+  const bool go = refused < 0 && epoch_differs < 0;
+  u64 n = 0;
+  if (go) {
+    BatchView bv;
+    n = j->x.received(ctx, bv);
+    if (n) k_xjoin_gather<<<ctx->sm_count * 4, 256, 0, s>>>(bv, n, j->k.d_keys, j->d_vals, j->d_side);
+    CU(ctx, cudaGetLastError());
+  }
+  // barrier 2 on every call, failed or not: past it no peer's next call stores into this region or its head before
+  // this rank has read them
+  st = j->x.done(ctx, s);
+  if (st != BW_OK) return st;
+  if (refuse != BW_OK) CTX_FAIL(ctx, refuse, "%s", why);
+  if (refused >= 0) CTX_FAIL(ctx, BW_ERR_STATE, "join: rank %d refused this call (its own error says why); no rank played it", refused);
+  if (epoch_differs >= 0)
+    CTX_FAIL(ctx, BW_ERR_STATE, "join: rank 0 played epoch %llu and rank %d epoch %llu; every rank must pass the same epoch to one call",
+             (unsigned long long)got_epoch[0], epoch_differs, (unsigned long long)got_epoch[epoch_differs]);
   if (!j->pending) {
     j->min_epoch = epoch;
     j->pending = true;
   }
   j->last_epoch = epoch;
   const u32 batch_no = j->batch_no++;
-  BatchView bv;
-  const u64 n = j->x.received(ctx, bv);
-  if (n) k_xjoin_gather<<<ctx->sm_count * 4, 256, 0, s>>>(bv, n, j->k.d_keys, j->d_vals, j->d_side);
-  CU(ctx, cudaGetLastError());
-  st = j->x.done(ctx, s);
-  if (st != BW_OK) return st;
   if (n) {
     st = keyed_group(ctx, j->k, j->k.d_keys, n, s);
     if (st != BW_OK) return st;
@@ -2919,8 +2946,8 @@ static bw_status join_apply_ranks(bw_join* j, const u64* keys, const uint8_t* si
 bw_status bw_join_apply(bw_join* j, const uint64_t* keys, const uint8_t* side, const uint64_t* vals, uint64_t rows, uint64_t epoch) {
   if (!j) return BW_ERR_SPEC;
   bw_ctx* ctx = j->ctx;
-  if (rows > j->spec.max_batch_rows) CTX_FAIL(ctx, BW_ERR_SPEC, "join: rows > max_batch_rows");
   if (ctx->world > 1) return join_apply_ranks(j, keys, side, vals, rows, epoch);
+  if (rows > j->spec.max_batch_rows) CTX_FAIL(ctx, BW_ERR_SPEC, "join: rows > max_batch_rows");
   if (j->pending && epoch < j->last_epoch) CTX_FAIL(ctx, BW_ERR_STATE, "join: epochs must not decrease");
   if (!j->pending) {
     j->min_epoch = epoch;

@@ -395,7 +395,11 @@ class KeyedJoin:
     same arguments and calls ``apply`` once per activation, with its own rows (possibly none) and the same epoch.  Each
     row goes to rank ``bw_route(key, world)``, which joins what arrived in (source rank, source order); ``vals`` is an
     opaque u64 payload that travels with its row.  A rank's ``advance`` / ``eof`` return the rows of the keys it owns.
-    Close it only once no rank calls it any more."""
+    An ``apply`` that cannot go ahead on one rank (more than ``max_batch_rows`` rows, a NULL column, an epoch below the
+    last one since that rank's last ``advance``) still takes part in the exchange: that rank raises its own error, every
+    other rank ``BW_ERR_STATE``, no rank plays the call, and the next call goes on as if it had not been made.  A full
+    key table or emit buffer raises on its owner's ``advance``, as on one GPU; the other ranks' keys stay exact.  Close
+    it only once no rank calls it any more."""
 
     INSERT = {"first": 0, "last": 1}
     EMIT = {"complete": 0, "final": 1, "running": 2}

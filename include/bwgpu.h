@@ -401,11 +401,16 @@ typedef struct bw_join_rows {
  *  - bw_join_apply is collective: every rank calls it once per activation with its own rows (possibly none) and the
  *    same epoch.  Each row goes to rank bw_route(key, W), the owner the window fold uses.  The owner joins what it
  *    received in (source rank, source order).  Ranks that pass different epochs to one call all get BW_ERR_STATE.
+ *  - A call that cannot go ahead on one rank (rows > max_batch_rows, a NULL column, an epoch below the last one since
+ *    that rank's last advance) still takes part in the exchange, so that no rank is left waiting: that rank returns its
+ *    own error, every other rank BW_ERR_STATE, and no rank plays the call.  A call that fails on every rank changes no
+ *    rank's state: the next call goes on as if it had not been made.
  *  - vals is an opaque 64-bit payload that travels with its row.
  *  - Rank r's bw_join_advance / bw_join_eof return the rows of the keys r owns, in the order below.  Merging every
  *    rank's rows of one activation and stably sorting them by (epoch, key string) gives exactly the rows a world-1 join
  *    returns when fed the rank-major concatenation of every rank's columns.
- * A full key table or emit buffer raises on the owning rank's advance, as on one GPU. */
+ * A full key table or emit buffer raises on the owning rank's advance, as on one GPU (and on every later advance and
+ * eof of that rank); the other ranks' keys stay exact, and the owner keeps taking part in every apply. */
 bw_status bw_join_create(bw_ctx* ctx, const bw_join_spec* spec, bw_join** out);
 void bw_join_destroy(bw_join* j);
 /* One activation: items of both sides in arrival order, side[i] in {0 = left, 1 = right}; host columns. */
